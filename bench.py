@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- scans/sec of the MAD-ICP registration hot path on B200.
+"""bench.py -- scans/sec of the MAD-ICP registration hot path on H100.
 
 Workload (BASELINE.json configs[2] at N=1, configs[3] at N>1): one synthetic 64-beam x 2048-azimuth
 scan (131 072 points -> ~19k moving leaves) registered against a 16-keyframe model with `--iters`
@@ -18,6 +18,9 @@ Gauss-Newton rounds (default 10, as BASELINE's configs[1]).  A *step* is one who
   --impl reference : the reference's CPU implementation of the path on the host cores: its own sources
            compiled against oracle/eigen_standin (oracle/_ref, shipped prebuilt) and the Eigen-free restatement
            (oracle/) are both timed and the faster one is the line's value (the stand-in is slower than Eigen).
+  --dump-outputs DIR : after the timed steps, what the last timed registration returned to its caller (pose, H, b,
+           matched flags, matched count, keyframe weight) as DIR/<name>.npy, so that two builds can be compared output
+           for output on the same seeded inputs.
 """
 import argparse
 import json
@@ -36,7 +39,7 @@ METRIC = "scans/sec (130k-pt scan vs 16-keyframe model)"
 K_MODEL = 16
 
 
-def parse():
+def parse(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=200)
@@ -51,7 +54,19 @@ def parse():
                     help="how many of them the CPU pipeline also runs (trajectory error and keyframe decisions)")
     ap.add_argument("--beams", type=int, default=64)
     ap.add_argument("--azimuths", type=int, default=2048)
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed registration's outputs to DIR/<name>.npy (float64)")
+    return ap.parse_args(argv)
+
+
+def dump_outputs(out_dir, res):
+    """What register_fetch hands its caller after the last timed step: 3x4 pose, H (6x6), b (6), per-moving-leaf
+    matched flags, matched count and det(H^-1).  A few hundred kB at the default size."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"pose": res["X"], "H": res["H"], "b": res["b"], "matched": res["matched"],
+              "n_matched": [res["n_matched"]], "weight": [res["weight"]]}
+    for name, v in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.asarray(v, dtype=np.float64))
 
 
 def workload_name(a, n):
@@ -64,9 +79,7 @@ def workload_name(a, n):
 
 # --------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """Polls NVML (SM clock + clock-event reasons) while the timed region runs.  (The polling period is not what costs
-    the host-timed `e2e` its efficiency at N > 1: 2, 10 and 50 ms measured the same within the run-to-run spread at N=2,
-    profiles/r03_sampler_period_2gpu.txt.)"""
+    """Polls NVML (SM clock + clock-event reasons) while the timed region runs."""
     PERIOD_S = float(os.environ.get("MADICP_BENCH_SAMPLER_MS", "2")) * 1e-3
     BITS = {0x4: "sw_power_cap", 0x8: "hw_slowdown", 0x20: "sw_thermal_slowdown", 0x40: "hw_thermal_slowdown",
             0x80: "hw_power_brake_slowdown"}
@@ -133,10 +146,8 @@ def _sibling_sets(cores):
 def share_of_cores(cores, k, m, sibling_sets=None):
     """The k-th of m shares of `cores`, in WHOLE physical cores: ranks next to one socket should not end up on each
     other's hyperthreads.  (The sorted CPU list cut into m runs does that on a host numbered [0..31 | 64..95] per socket:
-    rank 0 gets the CPUs 0-15 and rank 2 their siblings 64-79.  At N=2 the two cuts measure the same,
-    profiles/r03_pinning_2gpu.txt; whether it is what the host-timed `e2e` loses at N=8 -- 0.76 of N x the single-GPU
-    rate against 0.99 for the device-timed `value` -- could not be measured in round 2.)"""
-    if os.environ.get("MADICP_BENCH_PIN_LEGACY"):  # the old cut, for A/B runs (profiles/r03_pinning_2gpu.txt)
+    rank 0 gets the CPUs 0-15 and rank 2 their siblings 64-79.)"""
+    if os.environ.get("MADICP_BENCH_PIN_LEGACY"):  # the old cut, for A/B runs
         share = max(4, len(cores) // m)
         return sorted(cores)[k * share:(k + 1) * share] or sorted(cores)
     sets = sibling_sets if sibling_sets is not None else _sibling_sets(cores)
@@ -204,19 +215,20 @@ def algorithmic_bytes(reg, depth_tables, trace, iters, L):
 
 
 # --------------------------------------------------------------------------------------------
-def latency_model(walked, visits, iters, K, L, measured_s, sm=148, warps_per_sm=24):
+def latency_model(walked, visits, iters, K, L, measured_s, sm, clk_ghz, warps_per_sm=24):
     """Latency floor of one k_gn_loop launch (what bounds the kernel, DESIGN.md 4.1): an SM runs its warp-items in passes
     of `warps_per_sm` resident warps, and a pass cannot be shorter than the chain of DEPENDENT operations of one item:
       * memory: a walk is one L2 round trip per two tree levels + the leaf record; a remembered item the memo word + the
         leaf record;
-      * arithmetic (added in the second half of round 2; `floor_memory_only_ms` keeps the earlier definition): the FP64
-        operations of one item that depend on each other -- pose applied (4), displacement, norm, square root and margin
-        of the memo check (17), gate, error, Jacobian and scale (13), counted in kernels.cuh / device_kernels.cuh -- at the
-        ~19 cycles a dependent FP64 operation takes on this part (scripts/fp64_probe.cu), and the 8 dependent DMMAs of the
-        fold at ~30;
+      * arithmetic (`floor_memory_only_ms` leaves it out): the FP64 operations of one item that depend on each other --
+        pose applied (4), displacement, norm, square root and margin of the memo check (17), gate, error, Jacobian and
+        scale (13), counted in kernels.cuh / device_kernels.cuh -- at 17 cycles per dependent FP64 operation (measured on
+        an H100 by scripts/fp64_probe.cu: 16.4-17.1 cycles per element of a dependent add chain), and the 8 dependent
+        DMMAs of the fold at ~30 (assumed, not measured on the H100);
     and every round ends with the fold (one L2 round trip), the 6x6 solve + exponential map (~150 dependent FP64
-    operations) and the pose hand-over (one L2 round trip).  Nothing here is a tuning constant of the kernel."""
-    clk_ghz, l2_lat, fp64_lat, dmma_lat = 1.92, 250.0, 19.0, 30.0
+    operations) and the pose hand-over (one L2 round trip), an L2 hit taken as ~250 cycles (assumed, not measured on the
+    H100).  `sm` and `clk_ghz` are the device's SM count and SM clock.  Nothing here is a tuning constant of the kernel."""
+    l2_lat, fp64_lat, dmma_lat = 250.0, 17.0, 30.0
     chain_ops = 4 + 17 + 13
     items_sm = K * L / sm / 32.0
     passes = int(np.ceil(items_sm / float(warps_per_sm)))
@@ -236,7 +248,9 @@ def latency_model(walked, visits, iters, K, L, measured_s, sm=148, warps_per_sm=
                         "sm_ghz": clk_ghz, "resident_warps_per_sm": warps_per_sm},
             "note": "lower bound on the launch time if every dependent load were an L2 hit, every dependent FP64 operation "
                     "issued the cycle its operand arrived and nothing else cost time; frac = floor / measured (1.0 = at the "
-                    "latency floor); frac_memory_only is the figure reported until the first half of round 2"}
+                    "latency floor); frac_memory_only counts the dependent memory round trips alone; the FP64 latency was "
+                    "measured on an H100 (scripts/fp64_probe.cu), the L2 hit and DMMA latencies are assumptions, not "
+                    "H100 measurements"}
 
 
 def cpu_reference_leg(a, steps, warmup, budget_s=None):
@@ -475,7 +489,7 @@ def main():
     L = means.shape[0]
     pinned = torch.from_numpy(means).pin_memory()
     X0 = case["T_guess"]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=f"cuda:{dev}")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=f"cuda:{dev}")  # > 50 MB L2
 
     def l2_flush():
         with torch.cuda.stream(stream):
@@ -520,6 +534,8 @@ def main():
     sampler.start()
     total_ms, launches = timed_resident(reg)
     res = reg.register_fetch(want_matched=True)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, res)
 
     # ---------------- end to end through the public call with host buffers (`e2e`)
     for _ in range(3):
@@ -593,15 +609,11 @@ def main():
         if os.path.exists(peaks_path):
             peak, peak_src = json.load(open(peaks_path))["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)"
         else:
-            peak, peak_src = 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+            peak, peak_src = 3350.0, "H100 SXM data sheet, 3.35 TB/s (not measured)"
         avg_launch_s = (total_ms * 1e-3) / a.steps
         achieved = abytes / avg_launch_s / 1e9
-        prof = {}
-        tp = os.path.join(ROOT, "profiles", "gn_loop_traffic.json")
-        if os.path.exists(tp):
-            prof = json.load(open(tp))
-        # L2 read bandwidth of THIS device, measured here: repeated reduction of a 48 MiB (L2-resident) buffer
-        buf = torch.empty(48 << 20, dtype=torch.uint8, device=f"cuda:{dev}").view(torch.float32)
+        # L2 read bandwidth of THIS device, measured here: repeated reduction of a 32 MiB (L2-resident) buffer
+        buf = torch.empty(32 << 20, dtype=torch.uint8, device=f"cuda:{dev}").view(torch.float32)
         for _ in range(3):
             buf.sum()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -611,15 +623,15 @@ def main():
         e1.record()
         torch.cuda.synchronize(dev)
         l2_peak = 20 * buf.numel() * 4 / (e0.elapsed_time(e1) * 1e-3) / 1e9
-        l2_bytes = prof.get("l2_to_l1_bytes_per_launch")
-        l2 = {"bytes_per_launch": l2_bytes, "achieved": (l2_bytes / avg_launch_s / 1e9) if l2_bytes else None,
-              "peak": l2_peak, "unit": "GB/s", "frac": (l2_bytes / avg_launch_s / 1e9 / l2_peak) if l2_bytes else None,
-              "source": "lts__t_sectors_srcunit_tex_op_read.sum x 32 B of the committed ncu capture (profiles/); peak = "
-                        "torch sum over a 48 MiB L2-resident buffer, measured in this run"}
-        lat = latency_model(walked, visits, a.iters, K_MODEL, L, avg_launch_s)
+        l2 = {"bytes_per_launch": None, "achieved": None, "peak": l2_peak, "unit": "GB/s", "frac": None,
+              "source": "L2-to-L1 bytes of the kernel: not measured (needs a hardware-counter profile); peak = torch sum "
+                        "over a 32 MiB L2-resident buffer, measured in this run"}
+        props = torch.cuda.get_device_properties(dev)
+        sm_ghz = (sampler.max_mhz or 1980.0) * 1e-3  # NVML's maximum SM clock; else the H100 SXM's 1.98 GHz
+        lat = latency_model(walked, visits, a.iters, K_MODEL, L, avg_launch_s, sm=props.multi_processor_count, clk_ghz=sm_ghz)
         rf = {"kernel": "k_gn_loop (persistent: search + linearize + reduce + solve, all GN rounds)", "bound": "hbm",
               "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-              "traffic": prof.get("dram_bytes_per_launch"),
+              "traffic": None,
               "algorithmic_bytes_per_launch": abytes, "node_visits_per_launch": visits, "peak_source": peak_src,
               "avg_launch_ms": avg_launch_s * 1e3, "model_bytes": model_bytes, "l2": l2, "latency_model": lat,
               "note": "SURVEY 8d's algorithmic bytes are those of the reference's algorithm (every pair walked in every round); "

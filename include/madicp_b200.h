@@ -1,4 +1,4 @@
-/* madicp_b200.h -- C ABI of libmadicp_b200.so: the B200 (sm_100a) implementation of MAD-ICP's
+/* madicp_b200.h -- C ABI of libmadicp_b200.so: the H100 (sm_90a) implementation of MAD-ICP's
  * per-scan registration hot path.  Plain pointers and sizes only; no C++/torch types cross this
  * boundary.  The reference has no FFI of its own -- its boundary is the C++ class API
  * (MADtree / MADicp) that Pipeline and the pybind wrappers call -- so each entry point below cites
@@ -14,7 +14,7 @@
  *     b is 6, ordered [t_x t_y t_z w_x w_y w_z] as in the reference (odometry/mad_icp.cpp:112-115).
  *   - a context is driven by one host thread at a time.
  *   - there is NO CPU fallback: every madicp_* compute call runs CUDA kernels and fails with
- *     MADICP_ERR_CUDA when no sm_100-class device is usable.
+ *     MADICP_ERR_CUDA when no sm_90 (H100) device is usable.
  */
 #ifndef MADICP_B200_H
 #define MADICP_B200_H
@@ -37,7 +37,7 @@ extern "C" {
 
 /* ----------------------------------------------------------------------------------------------
  * Flat MAD-tree node record: 64 bytes, 64-byte aligned, breadth-first order, the two children of
- * a node adjacent (right = link + 1).  One 64-byte record = two 256-bit loads on sm_100a.
+ * a node adjacent (right = link + 1).  One 64-byte record = four 128-bit loads on sm_90a.
  *   internal node : mean = centroid, dir = eigenvectors.col(2) (split direction), link = index of
  *                   the left child (>= 1)
  *   leaf          : mean = cloud point nearest the centroid, dir = eigenvectors.col(0) (surface
@@ -259,7 +259,7 @@ int madicp_comm_world(const madicp_ctx_t* ctx);
 
 /* Measures, on the resident model and moving leaves, the per-pass cost of each persistent-kernel shape the
  * automatic choice considers (a few one-round registrations each) and uses it from then on.  Optional: without it
- * a prior measured on B200 is used.  Returns the number of shapes measured. */
+ * a prior measured on an H100 is used.  Returns the number of shapes measured. */
 int madicp_calibrate(madicp_ctx_t* ctx, const double X0[12]);
 
 /* Tuning and debug entry points (clock stamps, kernel shape override) are declared in madicp_b200_debug.h. */

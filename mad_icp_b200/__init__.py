@@ -1,4 +1,4 @@
-"""mad_icp_b200 -- B200 (sm_100a) implementation of MAD-ICP's per-scan registration hot path.
+"""mad_icp_b200 -- H100 (sm_90a) implementation of MAD-ICP's per-scan registration hot path.
 
 Layout: csrc/ (CUDA kernels + C ABI + host flat-tree builder + device tree build/ingest), csrc/facade/ (C++
 classes and pybind modules with the reference's names: pymadtree, pymadicp, pypeline, pyvector -> pybind/),

@@ -1,4 +1,4 @@
-// reference_backend.cpp -- the B200 backend as a drop-in replacement for TWO translation units of
+// reference_backend.cpp -- the CUDA backend as a drop-in replacement for TWO translation units of
 // rvp-group/mad-icp: tools/mad_tree.cpp and odometry/mad_icp.cpp.
 //
 // It is compiled against the reference's OWN, UNMODIFIED headers (<tools/mad_tree.h>, <odometry/mad_icp.h>) and
@@ -94,7 +94,7 @@ MADtree::MADtree(const ContainerTypePtr vec, const IteratorType begin, const Ite
 // mad_tree_wrapper.h:41).  The caller's vector is read, not reordered.
 void MADtree::build(const ContainerTypePtr, const IteratorType begin, const IteratorType end, const double b_max,
                     const double b_min, const int level, const int max_parallel_level, MADtree* parent, MADtree*) {
-  if (level != 0 || parent) throw std::logic_error("MADtree (B200 backend): only whole trees can be built");
+  if (level != 0 || parent) throw std::logic_error("MADtree (CUDA backend): only whole trees can be built");
   const int64_t n = int64_t(end - begin);
   madtree_t* flat = nullptr;
   check(madtree_build(n > 0 ? &(*begin)(0) : nullptr, n, b_max, b_min, 1 << std::max(0, max_parallel_level), &flat),

@@ -1,4 +1,4 @@
-// arith.h -- single-source FP64 primitives shared by host C++ and sm_100a device code.
+// arith.h -- single-source FP64 primitives shared by host C++ and sm_90a device code.
 //
 // Bit-exact correspondence indices require the descent predicate
 //   ((q - mean) . dir) < 0                        (reference: tools/mad_tree.cpp:148)

@@ -1,5 +1,5 @@
 // capi.cu -- kernels' launch side and the madicp_* C ABI (include/madicp_b200.h).
-// No CPU fallback: every compute entry point launches the sm_100a kernels of kernels.cuh.
+// No CPU fallback: every compute entry point launches the sm_90a kernels of kernels.cuh.
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 
@@ -213,7 +213,7 @@ static int configure_gn(madicp_ctx* c, int threads, int ctas) {
 // and its time grows with the number of resident warps (L1 contention, fewer registers per thread).  With W
 // warps per SM and n warp-items per SM the passes are ceil(n / W).  The per-pass cost of every one-CTA-per-SM
 // shape is a property of the device AND the workload, so it is not tabulated: the context starts from a prior
-// (relative costs measured on B200, profiles/r01zg_probe_shapes.txt) and replaces it by what madicp_calibrate
+// (relative costs measured on an H100, ctx.hpp) and replaces it by what madicp_calibrate
 // measures on the resident model and moving leaves (called by the pipeline once the model has its keyframes).
 static int pick_shape(madicp_ctx* c, int64_t items) {
   if (!c->gn_auto) return MADICP_OK;
@@ -263,8 +263,8 @@ int madicp_create(madicp_ctx_t** out, int device, int max_keyframes) {
   CK(cudaSetDevice(device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major < 10) {
-    set_error("madicp_create: device is not sm_100-class; kernels are built for sm_100a only");
+  if (prop.major != 9 || prop.minor != 0) {  // sm_90a code loads on compute capability 9.0 only
+    set_error("madicp_create: device is not sm_90 (H100); kernels are built for sm_90a only");
     return MADICP_ERR_CUDA;
   }
   madicp_ctx* c = new madicp_ctx;

@@ -111,10 +111,11 @@ struct madicp_ctx {
   const void* gn_kernel = nullptr;
   size_t gn_smem = 0;
   // one-CTA-per-SM shapes the automatic choice considers, with the cost of one full pass of each (any unit):
-  // a prior until madicp_calibrate measures them on the resident workload
+  // a prior until madicp_calibrate measures them on the resident workload.  The prior: 10-round registrations of the
+  // bench workload (16 keyframes, 19 202 moving leaves) on an H100 SXM at a 400 W limit, time / passes, in 10 ns
   static constexpr int kNumAutoShapes = 6;
   static constexpr int kAutoShapes[kNumAutoShapes] = {768, 1024, 896, 704, 640, 512};
-  double pass_cost[kNumAutoShapes] = {9500.0, 11500.0, 10400.0, 9500.0, 8400.0, 7600.0};
+  double pass_cost[kNumAutoShapes] = {5570.0, 8260.0, 7480.0, 5650.0, 5325.0, 4650.0};
   bool calibrated = false;
   int last_iters = 0;
   long long* d_dbg = nullptr;  // MADICP_MAX_ITERS x 8 clock stamps when debug timing is on

@@ -639,8 +639,8 @@ k_gn_loop(const __grid_constant__ GnArgs A) {
       if (threadIdx.x < 6) s_b[threadIdx.x] = s_tot[threadIdx.x * 8 + 6];
       __syncthreads();
       if (last_round && threadIdx.x >= 32) {
-        // the last round's other results leave on three other warps while thread 0 solves (on thread 0 they added
-        // 4.5k cycles to every registration: profiles/r03b_variant_probe.txt, variants 1 -> 3)
+        // the last round's other results leave on three other warps while thread 0 solves (on thread 0 they lengthen
+        // every registration's serial tail)
         if (threadIdx.x == 32) unpack_Hb(s_tot, st->H, st->b);
         if (threadIdx.x == 64) st->weight = inv_det6_dev(s_tot, 8);
         if (threadIdx.x == 96) {

@@ -1,5 +1,5 @@
 // flat_tree.cpp -- host-side MAD-tree builder producing the breadth-first 64-byte record layout the
-// sm_100a kernels walk (include/madicp_b200.h: madtree_*).
+// sm_90a kernels walk (include/madicp_b200.h: madtree_*).
 //
 // What it computes is the reference's MADtree (tools/mad_tree.cpp:47-130 build, :154-163 leaf order,
 // :165-172 applyTransform; helpers tools/utils.h:38-97); how it is organised is not: instead of one

@@ -279,7 +279,7 @@ void root_sums_host(const T* p, int64_t n, double* S) {
 // A few resident host threads for work that is handed over and collected later (the roots' sums of staged clouds).
 // std::async(std::launch::async) creates a thread per call: in a process with CUDA and a large address space that
 // is tens to hundreds of microseconds ON THE CALLING THREAD per staged scan -- the thread that is about to launch
-// the next registration (profiles/r03ab: up to 0.33 ms per scan of the stream outside Pipeline.compute).
+// the next registration.
 // Leaked on purpose (detached workers may still wait on it at exit); created at first use, i.e. after any fork()
 // the caller did before touching CUDA.
 class Background {

@@ -338,12 +338,12 @@ class Registrar:
         return buf[:rows]
 
     def debug_cta_cycles(self, rounds):
-        buf = np.zeros(rounds * 148 * 8, np.int64)
+        buf = np.zeros(rounds * 2048, np.int64)  # room for grids of up to 2048 CTAs
         grid = check(capi.lib().madicp_debug_cta_cycles(self._h, buf.ctypes.data_as(C.POINTER(C.c_int64)), buf.size))
         return buf[:rounds * grid].reshape(rounds, grid)
 
     def debug_cta_stamps(self, plane, rounds):
-        buf = np.zeros(rounds * 148 * 8, np.int64)
+        buf = np.zeros(rounds * 2048, np.int64)
         grid = check(capi.lib().madicp_debug_cta_stamps(self._h, plane, buf.ctypes.data_as(C.POINTER(C.c_int64)), buf.size))
         return buf[:rounds * grid].reshape(rounds, grid)
 

@@ -6,10 +6,11 @@
 // cpu_baseline / `--impl reference` legs of bench.py may use it.  The product
 // (mad_icp_b200/) never includes, links or calls anything in this directory.
 //
-// PARITY STATUS: the reference ships no tests/golden vectors, and Eigen is absent
-// from this image (no network).  Two anchors exist:
-//  (1) tests/test_reference_pin.py compiles the reference's OWN sources (from
-//      /root/reference, unmodified) against oracle/eigen_standin and requires this
+// PARITY STATUS: the reference ships no tests/golden vectors, and it is built here
+// without Eigen.  Two anchors exist:
+//  (1) tests/test_reference_pin.py pins to the reference's OWN sources (from
+//      a checkout of the reference, unmodified, compiled against oracle/eigen_standin; their
+//      outputs are stored under tests/golden/) and requires this
 //      restatement to equal them BIT FOR BIT (trees, searches, every GN round,
 //      the streamed Pipeline).  Control flow, statement order and data handling
 //      are therefore the reference's, verified.
@@ -22,7 +23,7 @@
 //      product mirrors it.
 //
 // Each function cites the reference file:line it follows (paths relative to
-// /root/reference/mad_icp/src).
+// the reference's mad_icp/src).
 //
 // Build flags (oracle/Makefile): -O3 -fopenmp -std=c++17 -ffp-contract=off, no
 // -march=native, no -ffast-math (reference: mad_icp/CMakeLists.txt:6-8,38-40).

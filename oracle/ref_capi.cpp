@@ -2,8 +2,8 @@
 // oracle/ref_capi.cpp -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 //
 // C entry points over the UNMODIFIED reference classes (MADtree, MADicp, Pipeline), whose sources
-// are compiled where they lie under /root/reference by oracle/Makefile (target _ref) against
-// oracle/eigen_standin (this image has no Eigen).  The entry points mirror the orc_* functions of
+// are compiled where they lie in a checkout of the reference by oracle/Makefile (target _ref) against
+// oracle/eigen_standin (no Eigen installation needed).  The entry points mirror the orc_* functions of
 // oracle_capi.cpp one for one, so tests/test_reference_pin.py can run the reference and the
 // restatement on the same inputs and compare them coefficient by coefficient.
 //

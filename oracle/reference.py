@@ -2,9 +2,9 @@
 
 TEST INFRASTRUCTURE.  The library is the reference's OWN sources (tools/mad_tree.cpp,
 odometry/mad_icp.cpp, odometry/pipeline.cpp, odometry/vel_estimator.cpp) compiled where they lie under
-/root/reference against oracle/eigen_standin (this image has no Eigen), plus oracle/ref_capi.cpp.  It exists
-to pin the restatement (oracle/oracle.py) and, on the GPU box, as the timed CPU arm of bench.py.  It is
-built only where /root/reference exists; the built file is git-ignored and travels with the snapshot.
+REF_SRC (the reference checkout's mad_icp/src) against oracle/eigen_standin, plus oracle/ref_capi.cpp.  It exists
+to pin the restatement (oracle/oracle.py: tests/golden/make_reference_pin.py records its outputs) and as the timed
+CPU arm of bench.py.  It is built only where the reference sources are; the built file is git-ignored.
 """
 import ctypes as C
 import os
@@ -16,7 +16,8 @@ from .oracle import _b, _d, _dp, _i, _ip, _bp, _pose12
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SO = os.path.join(_HERE, "_ref", "libmadicp_ref.so")
-REF_SRC = "/root/reference/mad_icp/src"
+# where the reference checkout's mad_icp/src lies: $MADICP_REFERENCE_SRC, by default /root/reference/mad_icp/src
+REF_SRC = os.environ.get("MADICP_REFERENCE_SRC", "/root/reference/mad_icp/src")
 _lib = None
 
 
@@ -25,7 +26,7 @@ def available():
 
 
 def build(force=False):
-    """`make ref` in oracle/ (needs /root/reference; a no-op when the prebuilt library is current)."""
+    """`make ref` in oracle/ (needs the reference sources at REF_SRC; a no-op when the prebuilt library is current)."""
     if not os.path.isdir(REF_SRC):
         if os.path.exists(_SO):
             return _SO
@@ -182,5 +183,5 @@ def variant(so_name, make_target=None):
     if make_target and os.path.isdir(REF_SRC):
         subprocess.check_call(["make", "-C", _HERE, "-s", make_target])
     if not os.path.exists(mod._SO):
-        raise RuntimeError(f"{mod._SO} is missing (built where /root/reference exists: make -C oracle {make_target})")
+        raise RuntimeError(f"{mod._SO} is missing (built where the reference sources are, REF_SRC: make -C oracle {make_target})")
     return mod

@@ -1,5 +1,5 @@
-"""Host MAD-tree build timing as a function of the thread count (run on the GPU box: the container's
-vCPUs do not scale).  Usage: python scripts/build_probe.py"""
+"""Host MAD-tree build timing as a function of the thread count (run it on a host with
+many physical cores).  Usage: python scripts/build_probe.py"""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

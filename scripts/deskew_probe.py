@@ -1,4 +1,4 @@
-"""Host deskew timing per thread count (run on the GPU box; the container's vCPUs do not scale)."""
+"""Host deskew timing per thread count (run it on a host with many physical cores)."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

@@ -34,7 +34,7 @@ for iters in (1, 2, 5, 10, 15, 20):
     c = timed(lambda: reg.register_async(X0, iters), cold=True)
     print(f"gn_loop iters={iters:2d}: warm median {w[0]:8.1f} us (min {w[1]:8.1f})   cold median {c[0]:8.1f} us (min {c[1]:8.1f})")
 
-# per-round phase breakdown (SM cycles @ ~1.965 GHz) per walk mode and shape
+# per-round phase breakdown (SM cycles) per walk mode and shape
 reg.debug_timing(True, fetch=False)
 for mode in (4, 1):
     pass

@@ -44,11 +44,11 @@ for _ in range(3):
 d = reg.debug_timing(True)
 start, end, pub = (reg.debug_cta_stamps(p, 10).astype(np.float64) for p in (1, 2, 3))
 folded, handed = d[:, 6].astype(np.float64), d[:, 7].astype(np.float64)
-ghz = 1.965
+ghz = torch.cuda.get_device_properties(0).clock_rate * 1e-6  # the device's SM clock (kHz -> GHz)
 print("   CTA 0 (cycles): fold wait", d[:, 2].tolist(), " solve+publish", d[:, 4].tolist())
 for it in (0, 3, 8):
     t0 = start[it].min()
-    rel = lambda a: (a - t0) * ghz  # ns -> SM cycles (the timer ticks every ~256 ns = 500 cycles)
+    rel = lambda a: (a - t0) * ghz  # ns -> SM cycles (the timer ticks every ~256 ns)
     print(f"   round {it} (cycles after the first CTA started): items end min/p50/max {rel(end[it]).min():.0f}/{np.median(rel(end[it])):.0f}/{rel(end[it]).max():.0f}"
           f"  tile out max {rel(pub[it]).max():.0f}  folded {rel(folded[it]):.0f}  pose out {rel(handed[it]):.0f}"
           f"  next starts min/p50/max {rel(start[it + 1]).min():.0f}/{np.median(rel(start[it + 1])):.0f}/{rel(start[it + 1]).max():.0f}")

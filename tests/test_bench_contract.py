@@ -43,6 +43,27 @@ def test_product_arm_needs_a_gpu(built):
     assert "CUDA" in (p.stderr + p.stdout)
 
 
+def test_dump_outputs_writes_what_register_fetch_returns(tmp_path):
+    sys.path.insert(0, ROOT)
+    import numpy as np
+    import bench
+    res = dict(X=np.arange(12.0).reshape(3, 4), H=np.eye(6), b=np.ones(6), matched=np.array([1, 0, 1], np.uint8),
+               n_matched=2, weight=0.5)
+    bench.dump_outputs(str(tmp_path / "out"), res)
+    got = {p.stem: np.load(p) for p in (tmp_path / "out").glob("*.npy")}
+    assert sorted(got) == ["H", "b", "matched", "n_matched", "pose", "weight"]
+    assert all(v.dtype == np.float64 for v in got.values())
+    assert (got["pose"] == res["X"]).all() and (got["matched"] == [1, 0, 1]).all() and got["n_matched"][0] == 2
+
+
+def test_dump_outputs_option_is_parsed():
+    sys.path.insert(0, ROOT)
+    import bench
+    a = bench.parse(["--gpus", "1", "--steps", "7", "--warmup", "2", "--dump-outputs", "out"])
+    assert a.dump_outputs == "out" and a.steps == 7 and a.warmup == 2
+    assert bench.parse([]).dump_outputs is None
+
+
 def test_ranks_next_to_one_socket_get_whole_physical_cores():
     """bench.pin_to_gpu: four ranks next to a 32-core / 64-thread socket numbered [0..31 | 64..95] must not sit on each
     other's hyperthreads (the sorted CPU list cut into four runs did exactly that)."""
@@ -65,16 +86,16 @@ def test_ranks_next_to_one_socket_get_whole_physical_cores():
 
 
 def test_latency_model_is_a_pure_function_of_the_walk_counts():
-    """bench.latency_model on the numbers of profiles/r03f_bench.json: the memory-only floor is the figure the earlier
-    bench lines carried (0.0312 ms, frac 0.183); the full floor adds the dependent FP64 chain of every pass."""
+    """bench.latency_model on the walk counts of one bench run of a 148-SM part at 1.92 GHz: the memory-only floor is
+    0.0296 ms (frac 0.174); the full floor adds the dependent FP64 chain of every pass."""
     sys.path.insert(0, ROOT)
     import bench
     walked = [307232, 281829, 107440, 14523, 1799, 206, 9, 0, 0, 0]
-    m = bench.latency_model(walked, 46436884, 10, 16, 19202, 0.1703627222031355e-3)
+    m = bench.latency_model(walked, 46436884, 10, 16, 19202, 0.1703627222031355e-3, sm=148, clk_ghz=1.92)
     assert m["passes_per_round"] == 3 and abs(m["mean_nodes_per_walk"] - 15.1146) < 1e-3
-    assert abs(m["floor_memory_only_ms"] - 0.031205134883585593) < 1e-9
-    assert abs(m["frac_memory_only"] - 0.18316879702343278) < 1e-9
-    extra_cycles = 10 * 3 * (34 * 19.0 + 8 * 30.0)
+    assert abs(m["floor_memory_only_ms"] - 0.02964263488358559) < 1e-9
+    assert abs(m["frac_memory_only"] - 0.17399718964481317) < 1e-9
+    extra_cycles = 10 * 3 * (34 * 17.0 + 8 * 30.0)
     assert abs(m["floor_ms"] - (m["floor_memory_only_ms"] + extra_cycles / 1.92e9 * 1e3)) < 1e-12
     assert m["floor_memory_only_ms"] < m["floor_ms"] < m["measured_ms"] and 0 < m["frac"] < 1
     json.dumps(m)  # goes into the bench line as it is

@@ -14,7 +14,7 @@ import pytest
 from mad_icp_b200 import synth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SRC = "/root/reference/mad_icp/src"
+from oracle.reference import REF_SRC  # noqa: E402
 
 
 def _find_eigen():

@@ -1,7 +1,7 @@
 """The drop-in boundary, proven (`-m gpu`): oracle/_ref/libmadicp_ref_gpu.so is the reference's UNMODIFIED
 odometry/pipeline.cpp + odometry/vel_estimator.cpp, compiled against its own headers and linked with
 mad_icp_b200/csrc/adapter/reference_backend.cpp in place of its tools/mad_tree.cpp + odometry/mad_icp.cpp
-(`make -C oracle ref_gpu`; built where /root/reference exists, shipped prebuilt).  It is driven through the same C
+(`make -C oracle ref_gpu`, run by build() where the reference's sources are: oracle/reference.py REF_SRC).  It is driven through the same C
 entry points (oracle/ref_capi.cpp) as the CPU build of the reference, and must agree with it: keyframe decisions
 equal scan for scan, poses within 1e-5 rad / 1e-4 m, registration loop H/b 1e-12, correspondences bit-exact."""
 import os
@@ -20,7 +20,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def libs():
     from oracle import reference as R
     if not os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libmadicp_ref_gpu.so")) and not os.path.isdir(R.REF_SRC):
-        pytest.skip("oracle/_ref/libmadicp_ref_gpu.so not shipped (it is built where /root/reference exists)")
+        pytest.skip("oracle/_ref/libmadicp_ref_gpu.so not built (it needs the reference sources, oracle/reference.py REF_SRC)")
     G = R.variant("libmadicp_ref_gpu.so", "ref_gpu")
     R.lib()
     G.lib()

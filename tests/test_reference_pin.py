@@ -1,102 +1,95 @@
 """Pins the CPU restatement (oracle/) against the reference's OWN sources.
 
-oracle/_ref/libmadicp_ref.so is tools/mad_tree.cpp, odometry/mad_icp.cpp, odometry/vel_estimator.cpp and
-odometry/pipeline.cpp compiled unmodified from /root/reference against oracle/eigen_standin (no Eigen in
-this image).  Everything the reference decides -- split order, leaf selection, normal inheritance, NaN
-handling of 1-point nodes, gate, kernel, accumulation order, keyframe promotion -- runs as written by its
-authors; the restatement must reproduce it bit for bit.  What stays unpinned is the evaluation order
-INSIDE Eigen's operators, which the stand-in takes from the restatement (see its header).
+tests/golden/reference_pin.json holds SHA-256 digests (tests/util.py: digest) of every array the reference computed
+for the cases below: tools/mad_tree.cpp, odometry/mad_icp.cpp, odometry/vel_estimator.cpp and odometry/pipeline.cpp
+compiled unmodified against oracle/eigen_standin (`make -C oracle ref`) and run through the same case functions by
+tests/golden/make_reference_pin.py.  Everything the reference decides -- split order, leaf selection, normal
+inheritance, NaN handling of 1-point nodes, gate, kernel, accumulation order, keyframe promotion -- runs as written by
+its authors; the restatement must reproduce it bit for bit, i.e. every array must hash to the reference's digest.
+What stays unpinned is the evaluation order INSIDE Eigen's operators, which the stand-in takes from the restatement
+(see its header).
 
-CPU only.  Skipped where neither /root/reference nor a prebuilt oracle/_ref exists.
+CPU only; needs nothing outside the repository.
 """
-import ctypes as C
+import json
+import os
+import types
 
 import numpy as np
 import pytest
 
 from mad_icp_b200 import synth
+from util import digest
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_pin.json")
 
 
-@pytest.fixture(scope="module")
-def ref(built):
-    from oracle import reference as R
-    if not R.available():
-        pytest.skip("no /root/reference and no prebuilt oracle/_ref")
-    R.lib()
-    return R
+def backend(oracle_module):
+    """The CPU restatement behind the interface the case functions use (make_reference_pin.py: reference_backend)."""
+    O = oracle_module
+    return types.SimpleNamespace(Tree=lambda pts, max_parallel_level=0, **kw: O.OracleTree(pts, **kw), icp_run=O.icp_run,
+                                 Pipeline=O.OraclePipeline, deskew=O.deskew, idx_kw={})
 
 
-def _same_tree(a, b):
-    ea, eb = a.export(), b.export()
-    assert a.num_nodes == b.num_nodes and a.num_leaves == b.num_leaves
-    for k in ea:
-        if ea[k].dtype.kind == "f":  # eigenvectors of 1-point nodes are NaN in both (0/0 covariance)
-            assert np.array_equal(ea[k], eb[k], equal_nan=True), k
-        else:
-            assert np.array_equal(ea[k], eb[k]), k
-    assert np.array_equal(a.cloud(), b.cloud())  # the build reorders and writes into the caller's vector
+def tree_arrays(t):
+    out = dict(t.export())
+    out["cloud"] = t.cloud()  # the build reorders and writes into the caller's vector
+    out["shape"] = np.array([t.num_nodes, t.num_leaves])
+    return out
 
 
-@pytest.mark.parametrize("b_max", [0.2, 1e-5])
-def test_tree_build_is_the_references(oracle, ref, b_max):
+def icp_arrays(r, with_idx=True):
+    keys = ("X_hist", "H_hist", "b_hist", "X", "matched") + (("idx_hist",) if with_idx else ())
+    return {k: np.asarray(r[k]) for k in keys}
+
+
+# ---------------------------------------------------------------------------------------------- cases
+# Every case maps a backend to {name: {key: array}}; the same functions produce the stored digests.
+def case_tree_build(M, b_max):
     np.random.seed(42)
     cloud = synth.four_walls(points_per_wall=2000)
-    _same_tree(oracle.OracleTree(cloud, b_max=b_max), ref.ReferenceTree(cloud, b_max=b_max))
+    return {"tree": tree_arrays(M.Tree(cloud, b_max=b_max))}
 
 
-def test_tree_build_lidar_scan_and_async_levels(oracle, ref):
+def case_lidar_scan_and_async_levels(M):
     """max_parallel_level > 0 takes the reference's std::async branch (mad_tree.cpp:106-128): same tree."""
     case = synth.registration_case(K=1, beams=32, azimuths=1024)
     pts = case["scans"][0]
-    o = oracle.OracleTree(pts)
-    _same_tree(o, ref.ReferenceTree(pts, max_parallel_level=0))
-    _same_tree(o, ref.ReferenceTree(pts, max_parallel_level=3))
-    o.apply_transform(case["kf_poses"][0])
-    r = ref.ReferenceTree(pts)
-    r.apply_transform(case["kf_poses"][0])
-    _same_tree(o, r)
-    q = case["query"][:5000]
-    assert np.array_equal(o.search(q), r.search(q))
+    out = {f"level{lv}": tree_arrays(M.Tree(pts, max_parallel_level=lv)) for lv in (0, 3)}
+    t = M.Tree(pts)
+    t.apply_transform(case["kf_poses"][0])
+    out["transformed"] = tree_arrays(t)
+    out["search"] = {"idx": t.search(case["query"][:5000])}
+    return out
 
 
-def test_degenerate_clouds(oracle, ref):
+def case_degenerate_clouds(M):
     rs = np.random.RandomState(3)
-    for pts in (rs.rand(1, 3), rs.rand(2, 3), rs.rand(3, 3), np.repeat(rs.rand(1, 3), 50, axis=0),
-                np.c_[rs.rand(200, 2), np.zeros(200)], np.c_[rs.rand(64), np.zeros((64, 2))]):
-        _same_tree(oracle.OracleTree(pts, b_max=0.05), ref.ReferenceTree(pts, b_max=0.05))
+    clouds = (rs.rand(1, 3), rs.rand(2, 3), rs.rand(3, 3), np.repeat(rs.rand(1, 3), 50, axis=0),
+              np.c_[rs.rand(200, 2), np.zeros(200)], np.c_[rs.rand(64), np.zeros((64, 2))])
+    return {f"cloud{i}": tree_arrays(M.Tree(pts, b_max=0.05)) for i, pts in enumerate(clouds)}
 
 
-@pytest.mark.parametrize("K,threads", [(1, 1), (3, 2), (4, 4)])
-def test_registration_loop_is_the_references(oracle, ref, K, threads):
+def case_registration_loop(M, K, threads):
     case = synth.registration_case(K=K, beams=16, azimuths=512)
-    kfo, kfr = [], []
+    kf = []
     for s in range(K):
-        a, b = oracle.OracleTree(case["scans"][s]), ref.ReferenceTree(case["scans"][s])
-        a.apply_transform(case["kf_poses"][s])
-        b.apply_transform(case["kf_poses"][s])
-        kfo.append(a)
-        kfr.append(b)
-    mo, mr = oracle.OracleTree(case["query"]), ref.ReferenceTree(case["query"])
-    ro = oracle.icp_run(kfo, mo, case["T_guess"], iters=10, num_threads=threads)
-    rr = ref.icp_run(kfr, mr, case["T_guess"], iters=10, num_threads=threads, record_idx=True)
-    for k in ("X_hist", "H_hist", "b_hist", "X", "matched"):
-        assert np.array_equal(ro[k], rr[k]), k
-    # the correspondences themselves: the reference's bestMatchingLeafFast on its own X_ * mean_, every round
-    assert np.array_equal(np.asarray(ro["idx_hist"]), rr["idx_hist"])
+        t = M.Tree(case["scans"][s])
+        t.apply_transform(case["kf_poses"][s])
+        kf.append(t)
+    r = M.icp_run(kf, M.Tree(case["query"]), case["T_guess"], iters=10, num_threads=threads, **M.idx_kw)
+    # idx_hist: the correspondences themselves, the reference's bestMatchingLeafFast on its own X_ * mean_, every round
+    return {"icp": icp_arrays(r)}
 
 
-def test_four_walls_demo_is_the_references(oracle, ref):
-    """apps/utils/tools/mad_registration.py through both: same 15 poses, same H/b, converge to identity."""
+def case_four_walls_demo(M):
+    """apps/utils/tools/mad_registration.py: 15 poses and H/b, converging to identity."""
     np.random.seed(42)
     cloud = synth.four_walls(points_per_wall=1000)
     T = np.eye(4)
     T[:3, :3] = synth.euler_xyz(0.1, 0.1, 0.1)
     T[:3, 3] = np.random.rand(3)
-    ro = oracle.icp_run([oracle.OracleTree(cloud)], oracle.OracleTree(cloud), T, iters=15, record_matches=False)
-    rr = ref.icp_run([ref.ReferenceTree(cloud)], ref.ReferenceTree(cloud), T, iters=15)
-    for k in ("X_hist", "H_hist", "b_hist", "X", "matched"):
-        assert np.array_equal(ro[k], rr[k]), k
-    assert np.abs(rr["X"] - np.eye(4)[:3]).max() < 1e-6
+    return {"icp": icp_arrays(M.icp_run([M.Tree(cloud)], M.Tree(cloud), T, iters=15), with_idx=False)}
 
 
 def _sequence(n, beams=16, azimuths=512):
@@ -106,70 +99,114 @@ def _sequence(n, beams=16, azimuths=512):
         yield 0.1 * i, np.ascontiguousarray(synth.lidar_scan(scene, base, beams=beams, azimuths=azimuths, seed=100 + i))
 
 
-@pytest.mark.parametrize("deskew", [False, True])
-def test_pipeline_is_the_references(oracle, ref, deskew):
-    """Streaming odometry: pose, smoothed velocity and keyframe decisions of every scan, bit for bit.
-    (The keyframe weight det(H^-1) is computed by two independently written LU routines; only the
-    decisions it drives are compared.)"""
-    L = oracle.lib()
-    L.orc_pipeline_create.restype = C.c_void_p
-    L.orc_pipeline_create.argtypes = [C.c_double, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double,
-                                      C.c_int, C.c_int, C.c_int]
-    L.orc_pipeline_compute.argtypes = [C.c_void_p, C.c_double, oracle._dp, C.c_int]
-    L.orc_pipeline_state.argtypes = [C.c_void_p, oracle._dp]
-    L.orc_pipeline_free.argtypes = [C.c_void_p]
-    po = C.c_void_p(L.orc_pipeline_create(10.0, int(deskew), 0.2, 0.1, 0.8, 0.1, 0.02, 4, 4, 0))
-    pr = ref.ReferencePipeline(deskew=deskew, num_keyframes=4, num_threads=4)
-    st = np.zeros(23)
-    promoted = 0
-    for i, (stamp, pts) in enumerate(_sequence(16)):
-        L.orc_pipeline_compute(po, stamp, oracle._d(pts), pts.shape[0])
-        L.orc_pipeline_state(po, oracle._d(st))
-        pr.compute(stamp, pts)
-        sr = pr.state()
-        assert np.array_equal(st[:12], sr[:12]), i          # frame_to_map_
-        assert np.array_equal(st[12:16], sr[12:16]), i      # map updated, ids, number of keyframes
-        assert np.array_equal(st[17:], sr[17:]), i          # VelEstimator state
-        promoted += int(st[12])
-    assert promoted >= 4
-    L.orc_pipeline_free(po)
+def case_pipeline(M, deskew):
+    """Streaming odometry: pose (frame_to_map_), map updated / ids / number of keyframes and the VelEstimator state of
+    every scan.  (The keyframe weight det(H^-1), column 16, is computed by two independently written LU routines; only
+    the decisions it drives are compared.)"""
+    p = M.Pipeline(deskew=deskew, num_keyframes=4, num_threads=4)
+    st = []
+    for stamp, pts in _sequence(16):
+        p.compute(stamp, pts)
+        st.append(p.state())
+    st = np.array(st)
+    return {"state": {"pose": st[:, :12], "keyframes": st[:, 12:16], "velocity": st[:, 17:]}}
 
 
-def test_deskew_is_the_references(oracle, ref):
-    L = oracle.lib()
-    L.orc_pipeline_create.restype = C.c_void_p
-    L.orc_pipeline_create.argtypes = [C.c_double, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double,
-                                      C.c_int, C.c_int, C.c_int]
-    L.orc_pipeline_deskew.argtypes = [C.c_void_p, oracle._dp, C.c_int, oracle._dp, oracle._dp]
-    L.orc_pipeline_free.argtypes = [C.c_void_p]
-    po = C.c_void_p(L.orc_pipeline_create(10.0, 1, 0.2, 0.1, 0.8, 0.1, 0.02, 4, 1, 0))
-    pr = ref.ReferencePipeline(deskew=True, num_threads=1)
+def case_deskew(M):
     _, pts = next(_sequence(1))
     Ta, Tb = synth.pose_xyyaw(0.0, 1.0, 0.0), synth.pose_xyyaw(0.8, 1.05, 0.03)
-    mine = pts.copy()
-    L.orc_pipeline_deskew(po, oracle._d(mine), mine.shape[0], oracle._d(np.ascontiguousarray(Ta[:3])),
-                          oracle._d(np.ascontiguousarray(Tb[:3])))
-    assert np.array_equal(mine, pr.deskew(pts, Ta, Tb))
-    assert np.abs(mine - pts).max() > 1e-3  # it did something
-    L.orc_pipeline_free(po)
+    return {"deskew": {"points": M.deskew(pts, Ta, Tb)}}
 
 
-@pytest.mark.parametrize("b_max,b_min,rho_ker,b_ratio", [(0.1, 0.05, 0.05, 0.01), (0.4, 0.2, 0.3, 0.05), (0.2, 0.1, 1e-3, 0.0)])
-def test_parameter_sweep_is_the_references(oracle, ref, b_max, b_min, rho_ker, b_ratio):
+def case_parameter_sweep(M, b_max, b_min, rho_ker, b_ratio):
     """Other leaf sizes, kernel widths and gate ratios than the defaults: trees and every GN round."""
     case = synth.registration_case(K=2, beams=16, azimuths=512, seed=9)
-    kfo, kfr = [], []
-    for s, P in zip(case["scans"], case["kf_poses"]):
-        a, b = oracle.OracleTree(s, b_max=b_max, b_min=b_min), ref.ReferenceTree(s, b_max=b_max, b_min=b_min)
-        _same_tree(a, b)
-        a.apply_transform(P)
-        b.apply_transform(P)
-        kfo.append(a)
-        kfr.append(b)
-    mo = oracle.OracleTree(case["query"], b_max=b_max, b_min=b_min)
-    mr = ref.ReferenceTree(case["query"], b_max=b_max, b_min=b_min)
-    ro = oracle.icp_run(kfo, mo, case["T_guess"], iters=6, min_ball=b_max, rho_ker=rho_ker, b_ratio=b_ratio, num_threads=2,
-                        record_matches=False)
-    rr = ref.icp_run(kfr, mr, case["T_guess"], iters=6, min_ball=b_max, rho_ker=rho_ker, b_ratio=b_ratio, num_threads=2)
-    for k in ("X_hist", "H_hist", "b_hist", "X", "matched"):
-        assert np.array_equal(ro[k], rr[k], equal_nan=True) if ro[k].dtype.kind == "f" else np.array_equal(ro[k], rr[k]), k
+    out, kf = {}, []
+    for s, (pts, P) in enumerate(zip(case["scans"], case["kf_poses"])):
+        t = M.Tree(pts, b_max=b_max, b_min=b_min)
+        out[f"tree{s}"] = tree_arrays(t)
+        t.apply_transform(P)
+        kf.append(t)
+    mo = M.Tree(case["query"], b_max=b_max, b_min=b_min)
+    r = M.icp_run(kf, mo, case["T_guess"], iters=6, min_ball=b_max, rho_ker=rho_ker, b_ratio=b_ratio, num_threads=2)
+    out["icp"] = icp_arrays(r, with_idx=False)
+    return out
+
+
+SWEEP = [(0.1, 0.05, 0.05, 0.01), (0.4, 0.2, 0.3, 0.05), (0.2, 0.1, 1e-3, 0.0)]
+CASES = {f"tree_build[{b}]": (case_tree_build, dict(b_max=b)) for b in (0.2, 1e-5)}
+CASES["lidar_scan_and_async_levels"] = (case_lidar_scan_and_async_levels, {})
+CASES["degenerate_clouds"] = (case_degenerate_clouds, {})
+CASES.update({f"registration_loop[{K}-{t}]": (case_registration_loop, dict(K=K, threads=t)) for K, t in [(1, 1), (3, 2), (4, 4)]})
+CASES["four_walls_demo"] = (case_four_walls_demo, {})
+CASES.update({f"pipeline[{d}]": (case_pipeline, dict(deskew=d)) for d in (False, True)})
+CASES["deskew"] = (case_deskew, {})
+CASES.update({"parameter_sweep[%g-%g-%g-%g]" % p: (case_parameter_sweep, dict(zip(("b_max", "b_min", "rho_ker", "b_ratio"), p)))
+              for p in SWEEP})
+
+
+def digests(out):
+    return {part: {k: digest(v) for k, v in arrays.items()} for part, arrays in out.items()}
+
+
+# ---------------------------------------------------------------------------------------------- tests
+@pytest.fixture(scope="module")
+def pinned():
+    with open(GOLDEN) as f:
+        return json.load(f)
+
+
+@pytest.fixture(scope="module")
+def M(oracle):
+    return backend(oracle)
+
+
+def _run(M, pinned, name):
+    fn, kw = CASES[name]
+    out = fn(M, **kw)
+    got, want = digests(out), pinned[name]
+    assert set(got) == set(want), name
+    for part in want:
+        diff = [k for k in want[part] if got[part].get(k) != want[part][k]]
+        assert not diff, f"{name}/{part}: {diff} differ from the reference's"
+    return out
+
+
+@pytest.mark.parametrize("b_max", [0.2, 1e-5])
+def test_tree_build_is_the_references(M, pinned, b_max):
+    _run(M, pinned, f"tree_build[{b_max}]")
+
+
+def test_tree_build_lidar_scan_and_async_levels(M, pinned):
+    _run(M, pinned, "lidar_scan_and_async_levels")
+
+
+def test_degenerate_clouds(M, pinned):
+    _run(M, pinned, "degenerate_clouds")
+
+
+@pytest.mark.parametrize("K,threads", [(1, 1), (3, 2), (4, 4)])
+def test_registration_loop_is_the_references(M, pinned, K, threads):
+    _run(M, pinned, f"registration_loop[{K}-{threads}]")
+
+
+def test_four_walls_demo_is_the_references(M, pinned):
+    out = _run(M, pinned, "four_walls_demo")
+    assert np.abs(out["icp"]["X"] - np.eye(4)[:3]).max() < 1e-6
+
+
+@pytest.mark.parametrize("deskew", [False, True])
+def test_pipeline_is_the_references(M, pinned, deskew):
+    out = _run(M, pinned, f"pipeline[{deskew}]")
+    assert int(out["state"]["keyframes"][:, 0].sum()) >= 4
+
+
+def test_deskew_is_the_references(M, pinned):
+    out = _run(M, pinned, "deskew")
+    _, pts = next(_sequence(1))
+    assert np.abs(out["deskew"]["points"] - pts).max() > 1e-3  # it did something
+
+
+@pytest.mark.parametrize("b_max,b_min,rho_ker,b_ratio", SWEEP)
+def test_parameter_sweep_is_the_references(M, pinned, b_max, b_min, rho_ker, b_ratio):
+    _run(M, pinned, "parameter_sweep[%g-%g-%g-%g]" % (b_max, b_min, rho_ker, b_ratio))

@@ -1,4 +1,19 @@
+import hashlib
+
 import numpy as np
+
+
+def digest(a):
+    """SHA-256 of an array's values and shape: equal digests <=> np.array_equal(a, b, equal_nan=True) for arrays of
+    the same kind (floats compared as float64 with NaNs and the sign of zero made canonical, integers as int64)."""
+    a = np.asarray(a)
+    if a.dtype.kind == "f":
+        a = a.astype(np.float64) + 0.0  # -0.0 -> +0.0
+        a = np.where(np.isnan(a), np.nan, a)
+    elif a.dtype.kind in "iub":
+        a = a.astype(np.int64)
+    a = np.ascontiguousarray(a)
+    return hashlib.sha256(f"{a.dtype.kind}{a.shape}".encode() + a.tobytes()).hexdigest()
 
 
 def bits_equal(a, b):

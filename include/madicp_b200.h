@@ -225,6 +225,9 @@ int madicp_register_trace(madicp_ctx_t* ctx, double* X_trace, int max_rounds);
 /* Per round of the last madicp_register* call: how many (moving leaf, keyframe) pairs the kernel actually walked; the
  * others provably kept the leaf of their last walk (path memo, kernels.cuh).  Returns the number of rounds written. */
 int madicp_register_walked(madicp_ctx_t* ctx, int32_t* walked, int max_rounds);
+/* The same rounds: how many 64-byte quad records those walks loaded (a walk resumed below the root loads fewer).
+ * Returns the number of rounds written. */
+int madicp_register_walk_records(madicp_ctx_t* ctx, int64_t* records, int max_rounds);
 
 /* Pipeline::deskew (odometry/pipeline.cpp:79-123), host side: sorts the n points by azimuth, cuts the
  * sweep into 1024 chunks, applies to every chunk the pose interpolated from the relative motion of the

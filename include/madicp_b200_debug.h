@@ -30,10 +30,11 @@ int madicp_debug_cta_stamps(madicp_ctx_t* ctx, int plane, int64_t* out, int cap)
 int madicp_set_gn_grid(madicp_ctx_t* ctx, int threads_per_cta, int ctas_per_sm);
 
 
-/* Path memo of the persistent kernel (kernels.cuh, descend_t): enable = 0 walks every (leaf, keyframe) pair in every
- * round, as round 1 did.  Results are identical either way (the memo only skips walks it has proved unchanged);
- * this switch exists for A/B measurements and for the test that checks exactly that. */
-int madicp_debug_set_memo(madicp_ctx_t* ctx, int enable);
+/* Path memo of the persistent kernel (kernels.cuh, descend_t): mode 0 walks every (leaf, keyframe) pair from the root
+ * in every round; 1 skips the walks whose leaf is proved unchanged; 2 (the default) also resumes the other walks from
+ * the deepest record of their last path that is proved unchanged.  Results are identical in every mode (the memo only
+ * skips what it has proved); this switch exists for A/B measurements and for the test that checks exactly that. */
+int madicp_debug_set_memo(madicp_ctx_t* ctx, int mode);
 
 /* Diagnostic for madicp_deskew's sort: n pseudo-random keys over `distinct` values, sorted by std::sort
  * and by the threaded restatement of it; returns how many positions of the two permutations differ (0). */

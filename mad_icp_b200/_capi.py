@@ -73,6 +73,7 @@ SYMBOLS = {
     "madicp_register_fetch": (C.c_int, [vp, dp, dp, dp, bp, C.POINTER(C.c_int)]),
     "madicp_register_trace": (C.c_int, [vp, dp, C.c_int]),
     "madicp_register_walked": (C.c_int, [vp, ip, C.c_int]),
+    "madicp_register_walk_records": (C.c_int, [vp, C.POINTER(C.c_int64), C.c_int]),
     "madicp_search_cloud": (C.c_int, [vp, C.c_int, dp, C.c_int64, ip, dp, dp, dp]),
     "madicp_deskew": (C.c_int, [dp, C.c_int64, dp, dp, C.c_double, C.c_int]),
     "madicp_debug_sort_check": (C.c_int64, [C.c_int64, C.c_uint32, C.c_int64, C.c_int]),

@@ -292,7 +292,7 @@ int madicp_create(madicp_ctx_t** out, int device, int max_keyframes) {
   CK(cudaMallocHost(&c->h_pinned, sizeof(double) * 64));
   CK(cudaMallocHost(&c->h_state, sizeof(GnState)));
   CK(cudaMallocHost(&c->h_matched, kMatchedCap));
-  if (const char* e = getenv("MADICP_NO_MEMO")) c->use_memo = (atoi(e) == 0);
+  if (const char* e = getenv("MADICP_NO_MEMO")) c->memo_mode = (atoi(e) == 0) ? 2 : 0;
   int threads = 1024, ctas = 1;
   if (const char* e = getenv("MADICP_GN_SHAPE"))
     if (sscanf(e, "%d,%d", &threads, &ctas) == 2) c->gn_auto = false;
@@ -336,6 +336,8 @@ void madicp_destroy(madicp_ctx_t* c) {
   cudaFree(c->d_tiles);
   cudaFree(c->d_memo_leaf);
   cudaFree(c->d_memo_margin);
+  cudaFree(c->d_memo_ckpt);
+  cudaFree(c->d_memo_ckpt_up);
   cudaFree(c->d_state);
   cudaFree(c->d_X);
   cudaFree(c->d_comm);
@@ -905,18 +907,26 @@ static int register_enqueue(madicp_ctx* c, int iters, const double X0[12], int c
       CK(cudaStreamSynchronize(c->stream));
       cudaFree(c->d_memo_leaf);
       cudaFree(c->d_memo_margin);
+      cudaFree(c->d_memo_ckpt);
+      cudaFree(c->d_memo_ckpt_up);
       c->d_memo_leaf = nullptr;
       c->d_memo_margin = nullptr;
+      c->d_memo_ckpt = nullptr;
+      c->d_memo_ckpt_up = nullptr;
       c->cap_memo = 0;
       const size_t cap = need + need / 4;
       CK(cudaMalloc(&c->d_memo_leaf, cap * sizeof(int)));
       CK(cudaMalloc(&c->d_memo_margin, cap * sizeof(float)));
+      CK(cudaMalloc(&c->d_memo_ckpt, cap * sizeof(unsigned)));
+      CK(cudaMalloc(&c->d_memo_ckpt_up, cap * sizeof(float)));
       c->cap_memo = cap;
     }
     A.memo_leaf = c->d_memo_leaf;
     A.memo_margin = c->d_memo_margin;
+    A.memo_ckpt = c->d_memo_ckpt;
+    A.memo_ckpt_up = c->d_memo_ckpt_up;
     A.item_stride = int(stride);
-    A.use_memo = c->use_memo ? 1 : 0;
+    A.memo_mode = c->memo_mode;
     A.walk_buf = mb;
   }
   A.st = c->d_state;
@@ -1023,6 +1033,17 @@ int madicp_register_walked(madicp_ctx_t* c, int32_t* walked, int max_rounds) {
                      cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   memcpy(walked, c->h_state->walked[0], size_t(rows) * sizeof(int));
+  return rows;
+}
+
+int madicp_register_walk_records(madicp_ctx_t* c, int64_t* records, int max_rounds) {
+  if (!c || !records || c->last_iters < 1) return MADICP_ERR_INVALID;
+  CK(cudaSetDevice(c->device));
+  int rows = std::min(c->last_iters, max_rounds);
+  CK(cudaMemcpyAsync(c->h_state->walk_recs[0], c->d_state->walk_recs[(c->call_seq - 1u) & 1u],
+                     size_t(rows) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  for (int i = 0; i < rows; ++i) records[i] = int64_t(c->h_state->walk_recs[0][i]);
   return rows;
 }
 
@@ -1200,9 +1221,12 @@ int madicp_debug_cta_stamps(madicp_ctx_t* c, int plane, int64_t* out, int cap) {
   return c->gn_grid;
 }
 
-int madicp_debug_set_memo(madicp_ctx_t* c, int enable) {
-  if (!c) return MADICP_ERR_INVALID;
-  c->use_memo = enable != 0;
+int madicp_debug_set_memo(madicp_ctx_t* c, int mode) {
+  if (!c || mode < 0 || mode > 2) {
+    set_error("madicp_debug_set_memo: mode must be 0 (off), 1 (leaf memo) or 2 (leaf memo + resume)");
+    return MADICP_ERR_INVALID;
+  }
+  c->memo_mode = mode;
   return MADICP_OK;
 }
 

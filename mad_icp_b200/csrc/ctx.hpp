@@ -97,8 +97,10 @@ struct madicp_ctx {
   size_t cap_partial = 0;
   int* d_memo_leaf = nullptr;      // path memo of the persistent kernel (GnArgs), grid x item_stride each
   float* d_memo_margin = nullptr;
+  unsigned* d_memo_ckpt = nullptr;
+  float* d_memo_ckpt_up = nullptr;
   size_t cap_memo = 0;
-  bool use_memo = true;            // MADICP_NO_MEMO=1 / madicp_debug_set_memo(0): walk every item in every round
+  int memo_mode = 2;               // madicp_debug_set_memo; MADICP_NO_MEMO=1: 0 (walk every item from the root in every round)
   madicp::GnState* d_state = nullptr;
   double* d_X = nullptr;  // 12 (step API pose) + 36 + 6 scratch
   madicp::CommBlock* d_comm = nullptr;

@@ -374,14 +374,28 @@ struct GnArgs {
   // path memo (kernels.cuh, descend_t): per CTA-local item, CTA b owns [b * item_stride, (b + 1) * item_stride)
   int* memo_leaf;                          // pool index of the leaf the last walk of the item reached
   float* memo_margin;                      // how far its query may still move before a decision of that walk could change
+  unsigned* memo_ckpt;                     // slot-relative quad record a failed memo resumes the walk from (0: the root)
+  float* memo_ckpt_up;                     // margin of the decisions above that record, in excess of memo_margin
   int item_stride;
-  int walk_buf;                            // which half of GnState::walked this call counts into
-  int use_memo;                            // 0: every item is walked in every round (probe / A-B measurement)
+  int walk_buf;                            // which half of GnState::walked / walk_recs this call counts into
+  int memo_mode;                           // 0: every item is walked from the root in every round (probe / A-B measurement);
+                                           // 1: leaf memo only; 2: leaf memo + resume from the checkpoint
   long long* dbg;                          // nullable: per-round SM-clock stamps (madicp_debug_timing)
   long long* dbg_cta;                      // nullable: [plane][round][CTA]: item-phase cycles; %globaltimer at the start of
                                            // the round's items, at their end, after the tile went out (planes 1..3);
                                            // plane 4, first 16 entries of a round: CTA 0's fold trace (fold_tiles)
 };
+// Checkpoint policy (speed only: any checkpoint gives the reference's leaf).  A walk leaves its checkpoint at the deepest
+// record whose prefix margin would survive a further move of tau = scale x the item's charged displacement in the round
+// of the walk (round 0 has none: its gate radius instead).  Deeper saves more records when the next resume comes,
+// shallower makes it likelier that the resume is allowed at all.  A/B: make probe DEFS=-DMADICP_CKPT_TAU_SCALE=0.5
+#ifndef MADICP_CKPT_TAU_SCALE
+#define MADICP_CKPT_TAU_SCALE 1.0
+#endif
+__device__ __forceinline__ float ckpt_tau(int it, double moved, double ball) {
+  return __double2float_ru(MADICP_CKPT_TAU_SCALE * (it == 0 ? ball : moved));
+}
+
 __device__ __forceinline__ long long global_ns() {
   long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -419,7 +433,7 @@ k_gn_loop(const __grid_constant__ GnArgs A) {
   __shared__ double s_tot[kAcc];
   __shared__ double s_b[6];
   __shared__ double s_X[12], s_Xp[12];
-  __shared__ int s_qn;
+  __shared__ int s_qn, s_rn;
   __shared__ int s_count[WARPS];
   GnState* st = A.st;
   const unsigned L = unsigned(A.L);
@@ -487,9 +501,14 @@ k_gn_loop(const __grid_constant__ GnArgs A) {
 
   for (int i = (blockIdx.x * THREADS + threadIdx.x) * 16; i < A.zero_bytes; i += gridDim.x * THREADS * 16)
     *reinterpret_cast<uint4*>(A.zero_next + i) = make_uint4(0, 0, 0, 0);
-  if (blockIdx.x == 0 && threadIdx.x < MADICP_MAX_ITERS) st->walked[A.walk_buf ^ 1][threadIdx.x] = 0;  // the NEXT call's
+  if (blockIdx.x == 0 && threadIdx.x < MADICP_MAX_ITERS) {  // the NEXT call's counters
+    st->walked[A.walk_buf ^ 1][threadIdx.x] = 0;
+    st->walk_recs[A.walk_buf ^ 1][threadIdx.x] = 0;
+  }
   int* const memo_leaf = A.memo_leaf + size_t(blockIdx.x) * A.item_stride;
   float* const memo_margin = A.memo_margin + size_t(blockIdx.x) * A.item_stride;
+  unsigned* const memo_ckpt = A.memo_ckpt + size_t(blockIdx.x) * A.item_stride;
+  float* const memo_ckpt_up = A.memo_ckpt_up + size_t(blockIdx.x) * A.item_stride;
   auto item_at = [&](unsigned t0, unsigned& k, unsigned& q) {
     if (s_map) {
       const unsigned pk = s_map[t0 + lane];
@@ -518,6 +537,7 @@ k_gn_loop(const __grid_constant__ GnArgs A) {
       if (it == 0 && blockIdx.x == 0) st->X_trace[threadIdx.x] = x;
     }
     if (threadIdx.x == 32) s_qn = 0;
+    if (threadIdx.x == 33) s_rn = 0;
     __syncthreads();
     const bool last_round = (it == A.iters - 1);
     double c0 = 0.0, c1 = 0.0;
@@ -529,8 +549,9 @@ k_gn_loop(const __grid_constant__ GnArgs A) {
     // One pass in the static item order (the order of the sums is fixed).  From round 1 on an item keeps the leaf
     // of its last walk when its query has moved, since that walk, by less than the smallest margin of the walk
     // (kernels.cuh, descend_t): the margin is charged with every round's displacement (triangle inequality),
-    // rounded down; otherwise the lane walks again, in place.
-    int n_walked = 0;
+    // rounded down; otherwise the lane walks again, in place -- from the checkpoint of its last walk when the
+    // decisions above it still hold under the same charge, else from the root.
+    int n_walked = 0, n_recs = 0;
     for (unsigned t0 = warp * 32; t0 < t_total; t0 += THREADS) {
       unsigned k, q;
       item_at(t0, k, q);
@@ -545,9 +566,18 @@ k_gn_loop(const __grid_constant__ GnArgs A) {
         int leaf = -1;
         Rec f;
         double ww = 0.0;
-        if (it > 0 && A.use_memo) {
+        unsigned start = 0;                          // quad record the walk starts from, slot-relative (0: the root)
+        float prefix = __int_as_float(0x7f800000);   // margin of the decisions above it
+        double moved = 0.0;
+        if (it > 0 && A.memo_mode) {
           const float have = memo_margin[t];
           const int last = memo_leaf[t];
+          unsigned ck = 0;
+          float ck_up = 0.0f;
+          if (A.memo_mode == 2) {  // requested with the leaf's words: a lane that resumes waits for no further load
+            ck = memo_ckpt[t];
+            ck_up = memo_ckpt_up[t];
+          }
           // the remembered leaf's record is requested BEFORE the margin is checked: in the rounds where nearly every
           // pair keeps its leaf this takes one dependent memory round trip out of every item
           f = load_rec(A.model.recs + last);
@@ -557,21 +587,35 @@ k_gn_loop(const __grid_constant__ GnArgs A) {
           const double dx = mx - bx, dy = my - by, dz = mz - bz;
           // slack: |dir| - 1 and the orthonormality of the pose (1e-4 relative), FP64 evaluation error of the
           // reference expression at the new query (< 8 * 2^-53 * (|q|_1 + |mean|_1): 1e-9 absolute + 1e-12 |q|_1)
-          const double moved = 1.0001 * sqrt(dx * dx + dy * dy + dz * dz) + 1e-9 + 1e-12 * (fabs(mx) + fabs(my) + fabs(mz));
+          moved = 1.0001 * sqrt(dx * dx + dy * dy + dz * dz) + 1e-9 + 1e-12 * (fabs(mx) + fabs(my) + fabs(mz));
           const double left = double(have) - moved;
           if (left > 0.0) {
             memo_margin[t] = __double2float_rd(left);
             leaf = last;
+          } else if (ck != 0) {
+            // the checkpoint's margin is kept as its excess over the leaf margin, which charging leaves unchanged: the
+            // same displacements are charged against it without a store per kept item
+            const double ck_left = __dsub_rd(__dadd_rd(double(have), double(ck_up)), moved);
+            if (ck_left > 0.0) {
+              start = ck;
+              prefix = __double2float_rd(ck_left);
+            }
           }
         }
         if (leaf < 0) {
           double ww_walk;
-          float margin = __int_as_float(0x7f800000);
-          leaf = A.use_memo ? descend_t<true>(A.model, int(k), mx, my, mz, ww_walk, margin)
-                            : descend_t<false>(A.model, int(k), mx, my, mz, ww_walk, margin);
-          if (A.use_memo) {
+          const float tau = ckpt_tau(it, moved, m.ball);
+          float margin = prefix, ck_margin = 0.0f;
+          unsigned ckpt = start;
+          leaf = A.memo_mode ? descend_t<true>(A.model, int(k), mx, my, mz, ww_walk, margin, ckpt, ck_margin, tau, n_recs)
+                             : descend_t<false>(A.model, int(k), mx, my, mz, ww_walk, margin, ckpt, ck_margin, tau, n_recs);
+          if (A.memo_mode) {
             memo_leaf[t] = leaf;
             memo_margin[t] = margin;
+          }
+          if (A.memo_mode == 2) {
+            memo_ckpt[t] = ckpt;
+            memo_ckpt_up[t] = __fsub_rd(ck_margin, margin);  // >= 0: the leaf margin is the smaller
           }
           ++n_walked;
           ww = __ldg(A.model.ww + leaf);  // (1 - bbox0/min_ball)^2 of the leaf, mad_icp.cpp:97-98
@@ -588,7 +632,11 @@ k_gn_loop(const __grid_constant__ GnArgs A) {
       warp_accumulate(stage, v, c0, c1);
     }
     n_walked = __reduce_add_sync(0xffffffffu, n_walked);  // items walked by this CTA in this round
-    if (lane == 0 && n_walked) atomicAdd(&s_qn, n_walked);
+    n_recs = __reduce_add_sync(0xffffffffu, n_recs);      // ... and the quad records they loaded
+    if (lane == 0 && n_walked) {
+      atomicAdd(&s_qn, n_walked);
+      atomicAdd(&s_rn, n_recs);
+    }
     if (A.dbg && threadIdx.x == 0 && blockIdx.x == 0) A.dbg[it * 8 + 0] = clock64() - t_begin;  // item phase, CTA 0
     if (A.dbg_cta) {  // per-CTA item phase (slowest warp) + this warp's own time
       __syncthreads();
@@ -599,7 +647,10 @@ k_gn_loop(const __grid_constant__ GnArgs A) {
       if (threadIdx.x == 0 && blockIdx.x == 0) A.dbg[it * 8 + 5] = s_qn;
     }
     __syncthreads();  // every warp is done with its staging tile: s_red aliases them
-    if (threadIdx.x == 0 && s_qn) atomicAdd(&st->walked[A.walk_buf][it], s_qn);
+    if (threadIdx.x == 0 && s_qn) {
+      atomicAdd(&st->walked[A.walk_buf][it], s_qn);
+      atomicAdd(&st->walk_recs[A.walk_buf][it], (unsigned long long) s_rn);
+    }
     // Round barrier without a ticket: every CTA publishes its 48-value tile as epoch-tagged LL cells (value and flag
     // in one 16-byte store); CTA 0 -- the fixed folder -- polls the cells of all CTAs (the loads that find the flag
     // also bring the value), sums them in a fixed order, solves and publishes the next pose the same way.

@@ -24,7 +24,8 @@
 //     registers them against every keyframe: balanced across SMs, and the lanes of a warp / the warps of
 //     an SM share the upper levels in L1.  The inter-round barrier is ticket-free (epoch-tagged LL cells read with
 //     L2-coherent loads, no acquire fence), so L1 is never invalidated between rounds.
-//   * PATH MEMO.  From round 1 on a walk is skipped when the query provably cannot have left its leaf (descend_t).
+//   * PATH MEMO.  From round 1 on a walk is skipped when the query provably cannot have left its leaf, and otherwise
+//     resumed from the deepest record of its last path the query provably still reaches (descend_t).
 // No wgmma: there is no dense contraction.  The only tensor-pipe use is the FP64 DMMA fold of the
 // per-correspondence outer products (warp_accumulate), which exists to save registers.
 // Compiled with -fmad=false; exact predicates use __d*_rn intrinsics (arith.h).
@@ -128,6 +129,7 @@ struct GnState {
   double weight;    // det(H^-1) of the last round's H (Frame::weight_, odometry/pipeline.cpp:223)
   double X_trace[(MADICP_MAX_ITERS + 1) * 12];  // pose before round i; [iters] = final pose (debug / parity aid)
   int walked[2][MADICP_MAX_ITERS];  // [call parity] per round: (leaf, keyframe) pairs that were walked (the rest kept their leaf: path memo)
+  unsigned long long walk_recs[2][MADICP_MAX_ITERS];  // [call parity] per round: quad records those walks loaded
   LLCell X_ll[12];  // pose of the next round, published with its epoch: waiting CTAs get value and flag in one load
 };
 
@@ -268,13 +270,28 @@ __device__ __forceinline__ double leaf_weight(const FastRec& p) {
 // that slack) since the walk takes the same side at EVERY node of the path, i.e. reaches the same leaf.  The GN loop
 // uses this from round 1 on: between rounds the pose moves by millimetres, most walks are provably unchanged
 // and are skipped, and the decisions stay exactly the reference's FP64 ones.
+//
+// RESUME.  The same argument holds for any prefix of the path: a query that has moved by less than the smallest margin
+// of the decisions ABOVE a quad record still reaches that record, so a walk may start there instead of at the root
+// and ends in the reference's leaf.  `ckpt` (in) is the slot-relative record the walk starts from (0 = the root) and
+// `margin` (in) the prefix margin still left above it (+inf at the root).  On return `ckpt` is the deepest record of
+// the path whose prefix margin is >= `tau` (or the start record if none is) and `ckpt_margin` that prefix margin; the
+// leaf margin in `margin` is min(start prefix, the margins below).  `tau` only decides how deep the checkpoint sits,
+// i.e. speed, never the leaf.  `n_rec` counts the quad records loaded.
 template <bool MEMO>
-__device__ __forceinline__ int descend_t(const ModelView& M, int k, double qx, double qy, double qz, double& ww, float& margin) {
+__device__ __forceinline__ int descend_t(const ModelView& M, int k, double qx, double qy, double qz, double& ww, float& margin,
+                                         unsigned& ckpt, float& ckpt_margin, float tau, int& n_rec) {
   const QueryF q = make_query(qx, qy, qz);
   const unsigned qroot = unsigned(M.qroot[k]);
   const QuadRec* qbase = M.quad;  // uniform base + 32-bit pool index: one IMAD.WIDE per record address
-  unsigned g = qroot;
+  unsigned g = qroot + ckpt;
+  if (MEMO) ckpt_margin = margin;
   while (true) {  // two binary decisions per memory round trip
+    if (MEMO && margin >= tau) {  // prefix margin of record g: non-increasing along the path
+      ckpt = g - qroot;
+      ckpt_margin = margin;
+    }
+    ++n_rec;
     FastRec p0, p1, p2;
     int bfs0, child0, pad1, pad2;
     const char* rp = reinterpret_cast<const char*>(qbase + g);
@@ -322,8 +339,10 @@ __device__ __forceinline__ int descend_t(const ModelView& M, int k, double qx, d
 }
 
 __device__ __forceinline__ int descend(const ModelView& M, int k, double qx, double qy, double qz, double& ww) {
-  float unused = 0.0f;
-  return descend_t<false>(M, k, qx, qy, qz, ww, unused);
+  float unused = 0.0f, unused_ck = 0.0f;
+  unsigned root = 0;
+  int unused_n = 0;
+  return descend_t<false>(M, k, qx, qy, qz, ww, unused, root, unused_ck, 0.0f, unused_n);
 }
 
 // One correspondence (reference: odometry/mad_icp.cpp:81-101): gate, error, Jacobian, Huber scale,

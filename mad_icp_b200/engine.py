@@ -319,6 +319,13 @@ class Registrar:
         rows = check(capi.lib().madicp_register_walked(self._h, as_i(buf), 64), "madicp_register_walked")
         return buf[:rows].copy()
 
+    def register_walk_records(self):
+        """Per round of the last registration: quad records loaded by the walks (fewer when a walk resumes below the root)."""
+        buf = np.zeros(64, np.int64)
+        rows = check(capi.lib().madicp_register_walk_records(self._h, buf.ctypes.data_as(C.POINTER(C.c_int64)), 64),
+                     "madicp_register_walk_records")
+        return buf[:rows].copy()
+
     def search_cloud(self, slot, queries, want=("ordinals", "points", "normals", "dists")):
         q = np.ascontiguousarray(queries, dtype=np.float64).reshape(-1, 3)
         n = q.shape[0]
@@ -347,8 +354,12 @@ class Registrar:
         grid = check(capi.lib().madicp_debug_cta_stamps(self._h, plane, buf.ctypes.data_as(C.POINTER(C.c_int64)), buf.size))
         return buf[:rounds * grid].reshape(rounds, grid)
 
-    def set_memo(self, enable=True):
-        check(capi.lib().madicp_debug_set_memo(self._h, int(enable)))
+    def set_memo(self, mode=True):
+        """Path memo mode: 0 / False walks every pair from the root, 1 keeps proved leaves, 2 / True (the default)
+        also resumes the other walks from their checkpoint."""
+        if isinstance(mode, bool):
+            mode = 2 if mode else 0
+        check(capi.lib().madicp_debug_set_memo(self._h, int(mode)), "madicp_debug_set_memo")
 
     def set_gn_grid(self, threads_per_cta=1024, ctas_per_sm=1):
         return check(capi.lib().madicp_set_gn_grid(self._h, threads_per_cta, ctas_per_sm))

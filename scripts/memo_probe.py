@@ -1,4 +1,5 @@
-"""Persistent-kernel timing with and without the path memo; per-round phase stamps.  python scripts/memo_probe.py"""
+"""Persistent-kernel timing in the three path-memo modes; per-round walk counts, quad records loaded and phase stamps.
+python scripts/memo_probe.py [threads,ctas ...]"""
 import os, sys
 sys.path.insert(0, os.getcwd())
 import numpy as np, torch
@@ -22,10 +23,10 @@ def timed(iters, cold, n=20):
     return np.median(ts)
 for shape in tuple(tuple(int(v) for v in a.split(',')) for a in sys.argv[1:]) or ((768, 1), (704, 1), (1024, 1)):
     reg.set_gn_grid(*shape)
-    for memo in (True, False):
+    for memo in (2, 1, 0):  # leaf memo + resume, leaf memo only, every pair walked from the root
         reg.set_memo(memo)
         reg.debug_timing(False, fetch=False)
-        line = f"shape {shape} memo={int(memo)}:"
+        line = f"shape {shape} memo={memo}:"
         for iters in (1, 2, 5, 10, 15):
             line += f"  it{iters}: {timed(iters, False):.1f}/{timed(iters, True):.1f}"
         print(line + "  us warm/cold", flush=True)
@@ -34,6 +35,8 @@ for shape in tuple(tuple(int(v) for v in a.split(',')) for a in sys.argv[1:]) or
             reg.register_async(X0, 10); torch.cuda.synchronize()
         d = reg.debug_timing(True)
         print("   per round: walked items (CTA 0)", d[:, 5].tolist())
+        print("   per round: walked items (all)", reg.register_walked().tolist(), "quad records loaded",
+              reg.register_walk_records().tolist())
         print("   per round: warp0/CTA0 items", d[:, 0].tolist(), "all folded", d[:, 1].tolist(), "fold wait", d[:, 2].tolist(), "solve", d[:, 4].tolist())
         cta = reg.debug_cta_cycles(10)
         print("   per-CTA item phase: round 0 min/p50/max", int(cta[0].min()), int(np.median(cta[0])), int(cta[0].max()),

@@ -184,6 +184,44 @@ int madicp_put_keyframe_tree(madicp_ctx_t* ctx, int slot, const madtree_gpu_t* t
 int madicp_ingest(madicp_ctx_t* ctx, const void* xyz, int64_t n, int is_f32, int deskew, const double T_prev[12],
                   const double T_now[12], double sensor_hz, int num_threads, double* points_out);
 
+/* ---------------- raw sensor records (strided x/y/z fields + the dataset readers' range gate) ------------------
+ * A scan as the sensor delivers it: n records of `stride` bytes in host memory, x/y/z at byte offsets offset[0..2],
+ * all float32 (is_f32 != 0) or all float64, little-endian.  Examples: the bytes of a KITTI .bin (stride 16, offsets
+ * 0/4/8, float32), the `data` of a PointCloud2 (e.g. 48-byte Ouster records).  The readers' filter runs on the way
+ * in, with their arithmetic (apps/utils/kitti_reader.py:82-88, apps/utils/point_cloud2.py:77-87):
+ *   r = sqrt((x*x + y*y) + z*z) in the field type, no FMA; the bounds are rounded to the field type once;
+ *   range_mode 0: no gate, 1: min_range <= r <= max_range (KITTI), 2: min_range < r < max_range (PointCloud2);
+ *   drop_nan != 0: records with a NaN coordinate are dropped (point_cloud2.py:83).
+ * Kept records stay in record order: the cloud is the reader's output converted to float64, bit for bit.
+ * Invalid (MADICP_ERR_INVALID, with a message): null data, n outside 1..2^24, a field outside the stride, an offset or
+ * stride not a multiple of the field size, NaN bounds or min_range > max_range, an unknown mode, and a scan the gate
+ * leaves empty (the reference would build a tree from an empty range).
+ * A packed N x 3 cloud is the case stride 12 / 24, offsets 0/4/8 (or 0/8/16), mode 0. */
+#define MADICP_RANGE_NONE 0
+#define MADICP_RANGE_INCLUSIVE 1
+#define MADICP_RANGE_STRICT 2
+typedef struct madicp_points {
+  const void* data; /* host memory: field c of record i at data + i * stride + offset[c] */
+  int64_t n;        /* records */
+  int64_t stride;   /* bytes from one record to the next */
+  int32_t offset[3];
+  int32_t is_f32;
+  double min_range, max_range;
+  int32_t range_mode;
+  int32_t drop_nan;
+} madicp_points_t;
+/* madicp_ingest for records: gate + compaction + float64 conversion on the device (deskew == 0), or the deskew
+ * permutation over the kept records (deskew != 0).  n_kept (nullable) receives the number of kept points;
+ * points_out (nullable) n_kept x 3 doubles.  The kept cloud stays resident for madtree_gpu_build_resident. */
+int madicp_ingest_points(madicp_ctx_t* ctx, const madicp_points_t* desc, int deskew, const double T_prev[12],
+                         const double T_now[12], double sensor_hz, int num_threads, int64_t* n_kept, double* points_out);
+/* madicp_stage_cloud / madtree_gpu_build_batch for records: the same staged-prefix rules (a staged scan is reused when
+ * its descriptor is equal, field for field); each tree is that of its scan's kept points.  reserve_points: total
+ * records the batch will hold. */
+int madicp_stage_points(madicp_ctx_t* ctx, const madicp_points_t* desc, int64_t reserve_points);
+int madtree_gpu_build_batch_points(madicp_ctx_t* ctx, const madicp_points_t* descs, int count, double b_max, double b_min,
+                                   madtree_gpu_t** out);
+
 /* K1 only -- MADtree::bestMatchingLeafFast (tools/mad_tree.cpp:144-152) of X*mean for every moving
  * leaf against every active keyframe.  out_ordinals: K_active x L int32 on the host (row k = k-th
  * active slot in ascending slot order); values are getLeafs ordinals of the matched leaf. */

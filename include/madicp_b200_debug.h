@@ -40,6 +40,11 @@ int madicp_debug_set_memo(madicp_ctx_t* ctx, int mode);
  * and by the threaded restatement of it; returns how many positions of the two permutations differ (0). */
 int64_t madicp_debug_sort_check(int64_t n, uint32_t seed, int64_t distinct, int num_threads);
 
+/* The range gate of madicp_points_t on the host, the same predicate the device applies: keep[i] = 1 when record i
+ * survives, else 0.  Validates the descriptor like madicp_ingest_points, except that an empty result is allowed.
+ * Returns the number of kept records.  No device work. */
+int64_t madicp_debug_range_mask(const madicp_points_t* desc, uint8_t* keep);
+
 #ifdef __cplusplus
 }
 #endif

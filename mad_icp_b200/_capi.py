@@ -16,6 +16,17 @@ ip = C.POINTER(C.c_int32)
 bp = C.POINTER(C.c_uint8)
 vp = C.c_void_p
 
+
+class Points(C.Structure):
+    """madicp_points_t: raw sensor records (strided x/y/z fields) + the dataset readers' range gate."""
+    _fields_ = [("data", C.c_void_p), ("n", C.c_int64), ("stride", C.c_int64), ("offset", C.c_int32 * 3),
+                ("is_f32", C.c_int32), ("min_range", C.c_double), ("max_range", C.c_double), ("range_mode", C.c_int32),
+                ("drop_nan", C.c_int32)]
+
+
+assert C.sizeof(Points) == 64
+pts_p = C.POINTER(Points)
+
 # every symbol include/madicp_b200.h and include/madicp_b200_debug.h declare: name -> (restype, argtypes)
 SYMBOLS = {
     "madicp_last_error": (C.c_char_p, []),
@@ -57,6 +68,10 @@ SYMBOLS = {
     "madicp_set_moving_tree": (C.c_int, [vp, vp]),
     "madicp_get_moving": (C.c_int, [vp, dp, C.c_int]),
     "madicp_ingest": (C.c_int, [vp, vp, C.c_int64, C.c_int, C.c_int, dp, dp, C.c_double, C.c_int, dp]),
+    "madicp_ingest_points": (C.c_int, [vp, pts_p, C.c_int, dp, dp, C.c_double, C.c_int, C.POINTER(C.c_int64), dp]),
+    "madicp_stage_points": (C.c_int, [vp, pts_p, C.c_int64]),
+    "madtree_gpu_build_batch_points": (C.c_int, [vp, pts_p, C.c_int, C.c_double, C.c_double, C.POINTER(vp)]),
+    "madicp_debug_range_mask": (C.c_int64, [pts_p, bp]),
     "madicp_register_fetch_weight": (C.c_int, [vp, dp, dp, dp, bp, C.POINTER(C.c_int), dp]),
     "madicp_register_partial_async": (C.c_int, [vp, C.c_int, dp]),
     "madicp_calibrate": (C.c_int, [vp, dp]),

@@ -244,7 +244,7 @@ static int grid_for(const madicp_ctx* c, int64_t items) {
 extern "C" {
 
 const char* madicp_last_error(void) { return g_error.c_str(); }
-int madicp_abi_version(void) { return 2; }
+int madicp_abi_version(void) { return 3; }
 
 int madicp_create(madicp_ctx_t** out, int device, int max_keyframes) {
   if (!out || max_keyframes < 1 || max_keyframes > kMaxSlots) {

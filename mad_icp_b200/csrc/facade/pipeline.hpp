@@ -15,6 +15,7 @@
 #include <limits>
 
 #include "../pose_math.h"
+#include "../records.hpp"
 #include "facade.hpp"
 
 namespace madicp_b200 {
@@ -98,6 +99,8 @@ class Lookahead {
     std::vector<float> f32;
     const void* ext = nullptr;        // ... or the caller's buffer, kept alive by `keepalive` until its tree is built
     bool is_f32 = false;
+    bool records = false;             // raw sensor records (Pipeline::prefetchRecords): `pts` describes them
+    madicp_points_t pts{};
     std::shared_ptr<void> keepalive;
     size_t n = 0;
     madtree_gpu_t* tree = nullptr;
@@ -126,19 +129,46 @@ class Lookahead {
   }
 
  private:
+  // scans that can share one batch call: packed clouds of one element type, or records
+  static bool sameKind(const Job& a, const Job& b) { return a.records == b.records && (a.records || a.is_f32 == b.is_f32); }
+  // Builds the trees of the longest run of queued scans of the front's kind, up to the batch size.  A scan whose tree
+  // cannot be built (records the range gate leaves empty) fails the batch call as a whole: the run is then halved until
+  // the batch no longer contains it, and once the front scan fails on its own it is dropped from the queue and its
+  // error is raised -- in the compute() call that reaches that scan.  The scans after it stay queued.
   void buildBatch() {
-    // the longest run of queued scans of the front's element type, up to the batch size
-    std::vector<const void*> ptr;
-    std::vector<int64_t> n;
-    const bool f32 = fifo_.front().is_f32;
+    size_t k = 0;
+    const Job& front = fifo_.front();
     for (const Job& j : fifo_) {
-      if (int(ptr.size()) == batch_ || j.tree || j.is_f32 != f32) break;
-      ptr.push_back(j.data());
-      n.push_back(int64_t(j.n));
+      if (int(k) == batch_ || j.tree || !sameKind(j, front)) break;
+      ++k;
     }
-    std::vector<madtree_gpu_t*> out(ptr.size(), nullptr);
-    check(madtree_gpu_build_batch(ctx_, ptr.data(), n.data(), f32 ? 1 : 0, int(ptr.size()), b_max_, b_min_, out.data()),
-          "madtree_gpu_build_batch");
+    std::vector<madtree_gpu_t*> out;
+    for (;;) {
+      std::vector<const void*> ptr;
+      std::vector<int64_t> n;
+      std::vector<madicp_points_t> pts;
+      for (size_t i = 0; i < k; ++i) {
+        ptr.push_back(fifo_[i].data());
+        n.push_back(int64_t(fifo_[i].n));
+        pts.push_back(fifo_[i].pts);
+      }
+      out.assign(k, nullptr);
+      const int rc = front.records
+                         ? madtree_gpu_build_batch_points(ctx_, pts.data(), int(k), b_max_, b_min_, out.data())
+                         : madtree_gpu_build_batch(ctx_, ptr.data(), n.data(), front.is_f32 ? 1 : 0, int(k), b_max_, b_min_,
+                                                   out.data());
+      if (rc >= 0) break;
+      const std::string msg = std::string(front.records ? "madtree_gpu_build_batch_points" : "madtree_gpu_build_batch") +
+                              " failed (" + std::to_string(rc) + "): " + madicp_last_error();
+      madicp_stage_discard(ctx_);  // (the failed call consumed the early uploads, or they are given up here)
+      staged_ = 0;
+      if (k == 1) {
+        fifo_.pop_front();
+        stageQueued();
+        throw Error(msg);
+      }
+      k /= 2;
+    }
     built_ = out.size();
     staged_ = 0;  // (the batch call consumed or discarded every early upload)
     for (size_t i = 0; i < out.size(); ++i) {
@@ -155,8 +185,12 @@ class Lookahead {
   void stageQueued() {
     while (staged_ < size_t(batch_) && built_ + staged_ < fifo_.size()) {
       const Job& j = fifo_[built_ + staged_];
-      if (j.is_f32 != fifo_[built_].is_f32) break;
-      check(madicp_stage_cloud(ctx_, j.data(), int64_t(j.n), j.is_f32 ? 1 : 0, int64_t(batch_) * int64_t(j.n)), "madicp_stage_cloud");
+      if (!sameKind(j, fifo_[built_])) break;
+      if (j.records)
+        check(madicp_stage_points(ctx_, &j.pts, int64_t(batch_) * int64_t(j.n)), "madicp_stage_points");
+      else
+        check(madicp_stage_cloud(ctx_, j.data(), int64_t(j.n), j.is_f32 ? 1 : 0, int64_t(batch_) * int64_t(j.n)),
+              "madicp_stage_cloud");
       ++staged_;
     }
   }
@@ -249,6 +283,17 @@ class Pipeline {
     }
     computeRaw(stamp, xyz, n, true);
   }
+  // Raw sensor records with the dataset readers' range gate (include/madicp_b200.h, madicp_points_t), read in place:
+  // the same result as compute() on the reader's filtered array.  MADICP_GPU_BUILD=0: the kept points are packed on
+  // the host with the same predicate, then the host path runs.
+  void computeRecords(double stamp, const madicp_points_t& pts) {
+    if (!gpu_build_) {
+      compute(stamp, packRecords(pts));
+      return;
+    }
+    if (!pts.data || pts.n <= 0) throw Error("Pipeline.computeRecords: empty scan");
+    computeRaw(stamp, pts.data, size_t(pts.n), pts.is_f32 != 0, &pts);
+  }
   bool gpuBuild() const { return gpu_build_; }
   int lastIcpIterations() const { return last_iters_; }  // rounds the realtime budget allowed for the last scan
   // Hands a FUTURE scan over for a look-ahead (batched) tree build (see Lookahead).  compute() then consumes the
@@ -256,7 +301,8 @@ class Pipeline {
   // nothing) when look-ahead is not possible: host-built trees, or deskewing (the scan needs the latest poses).
   // keepalive: when given, the buffer is read in place (no copy) and the handle is dropped once compute() has consumed
   // the scan; without it the cloud is copied.
-  bool prefetch(const void* xyz, size_t n, bool is_f32, std::shared_ptr<void> keepalive = nullptr) {
+  bool prefetch(const void* xyz, size_t n, bool is_f32, std::shared_ptr<void> keepalive = nullptr,
+                const madicp_points_t* records = nullptr) {
     if (!gpu_build_ || deskew_ || !xyz || n == 0) return false;
     const auto p0 = clk();
     struct Tick {  // (the hand-over runs on the thread that launches the registrations: its cost is part of the scan's)
@@ -272,6 +318,13 @@ class Pipeline {
     Lookahead::Job j;
     j.n = n;
     j.is_f32 = is_f32;
+    if (records) {  // (read in place: the caller must hand over a keepalive)
+      if (!keepalive) throw Error("Pipeline.prefetchRecords: the records must be kept alive");
+      // a descriptor the library would reject must not enter the queue (every later batch would fail on it)
+      check(madicp::check_points(records, "Pipeline.prefetchRecords"), "Pipeline.prefetchRecords");
+      j.records = true;
+      j.pts = *records;
+    }
     if (keepalive) {
       j.ext = xyz;
       j.keepalive = std::move(keepalive);
@@ -283,16 +336,24 @@ class Pipeline {
     lookahead_->push(std::move(j));
     return true;
   }
+  bool prefetchRecords(const madicp_points_t& pts, std::shared_ptr<void> keepalive) {
+    return prefetch(pts.data, pts.n > 0 ? size_t(pts.n) : 0, pts.is_f32 != 0, std::move(keepalive), &pts);
+  }
   size_t prefetched() { return lookahead_ ? lookahead_->size() : 0; }
 
  private:
   // the scan's MAD-tree: ingest (+ deskew, pipeline.cpp:137-138) and build, on the device or on the host
-  std::unique_ptr<MADtree> makeTree(const void* xyz, size_t n, bool is_f32) {
+  std::unique_ptr<MADtree> makeTree(const void* xyz, size_t n, bool is_f32, const madicp_points_t* records) {
     if (lookahead_ && !lookahead_->empty())  // built ahead of time by a worker lane
       return std::unique_ptr<MADtree>(new MADtree(icp_.context(), lookahead_->pop(), b_max_));
     const bool dsk = deskew_ && is_initialized_ && trajectory_.size() > 1;
     const double* Ta = dsk ? trajectory_[trajectory_.size() - 2].m : nullptr;
     const double* Tb = dsk ? trajectory_[trajectory_.size() - 1].m : nullptr;
+    if (gpu_build_ && records) {
+      check(madicp_ingest_points(icp_.context(), records, dsk ? 1 : 0, Ta, Tb, sensor_hz_, std::max(1 << max_parallel_levels_, 1),
+                                 nullptr, nullptr), "madicp_ingest_points");
+      return std::unique_ptr<MADtree>(new MADtree(icp_.context(), b_max_, b_min_));
+    }
     if (gpu_build_) {
       check(madicp_ingest(icp_.context(), xyz, int64_t(n), is_f32 ? 1 : 0, dsk ? 1 : 0, Ta, Tb, sensor_hz_,
                           std::max(1 << max_parallel_levels_, 1), nullptr), "madicp_ingest");
@@ -308,7 +369,7 @@ class Pipeline {
     return std::unique_ptr<MADtree>(new MADtree(pts, n, b_max_, b_min_, max_parallel_levels_));
   }
 
-  void computeRaw(double stamp, const void* xyz, size_t n, bool is_f32) {
+  void computeRaw(double stamp, const void* xyz, size_t n, bool is_f32, const madicp_points_t* records = nullptr) {
     if (!xyz || n == 0) throw Error("Pipeline.compute: empty cloud");
     is_map_updated_ = false;
     if (!is_initialized_) {  // pipeline.cpp:267-284
@@ -316,7 +377,7 @@ class Pipeline {
       f->frame = int(seq_);
       f->to_map = frame_to_map_;
       f->stamp = stamp;
-      f->tree = makeTree(xyz, n, is_f32);
+      f->tree = makeTree(xyz, n, is_f32, records);
       keyframes_.push_back(f);
       current_ = f;
       trajectory_.push_back(detail::poseIdentity());
@@ -327,7 +388,7 @@ class Pipeline {
     const auto c0 = clk();
     const auto c1 = c0;
     auto cur = std::make_shared<FrameB>();
-    cur->tree = makeTree(xyz, n, is_f32);
+    cur->tree = makeTree(xyz, n, is_f32, records);
     const auto c2 = clk();
     double t[3], w[3];
     for (int a = 0; a < 3; ++a) {
@@ -411,6 +472,26 @@ class Pipeline {
                      int num_threads) {
     if (cloud.empty()) return;
     check(madicp_deskew(cloud[0].data(), int64_t(cloud.size()), T_prev.m, T_now.m, sensor_hz, num_threads), "madicp_deskew");
+  }
+
+  // the kept points of `pts` as a packed float64 cloud, with the predicate the device applies (records.hpp)
+  static ContainerType packRecords(const madicp_points_t& pts) {
+    check(madicp::check_points(&pts, "Pipeline.computeRecords"), "Pipeline.computeRecords");
+    ContainerType cloud;
+    cloud.reserve(size_t(pts.n));
+    auto pack = [&](auto zero) {
+      using T = decltype(zero);
+      const madicp::RecReader<T> rd(pts);
+      for (int64_t i = 0; i < pts.n; ++i) {
+        T x, y, z;
+        rd.xyz(i, x, y, z);
+        if (rd.keep(x, y, z)) cloud.push_back({double(x), double(y), double(z)});
+      }
+    };
+    if (pts.is_f32) pack(0.0f);
+    else pack(0.0);
+    if (cloud.empty()) throw Error("Pipeline.computeRecords: no point inside the range gate");
+    return cloud;
   }
 
   static std::chrono::steady_clock::time_point clk() { return std::chrono::steady_clock::now(); }

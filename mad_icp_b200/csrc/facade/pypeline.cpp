@@ -1,7 +1,29 @@
 // pypeline -- reference: mad_icp/src/pybind/pypeline.cpp:52-75 (Pipeline + VectorEigen3d), same ctor
 // arguments and method names; registration runs on the GPU.
+#include <limits>
+
 #include "pipeline.hpp"
 #include "py_common.hpp"
+
+// records (2-D float array with >= 3 columns, or 1-D structured with x/y/z) -> madicp_points_t, by records.layout
+static madicp_points_t records_arg(const py::object& records, double min_range, double max_range, bool inclusive,
+                                   bool drop_nan) {
+  const py::tuple t = py::module_::import("mad_icp_b200.records")
+                          .attr("layout")(records, min_range, max_range, inclusive, drop_nan)
+                          .cast<py::tuple>();
+  madicp_points_t d{};
+  d.data = reinterpret_cast<const void*>(t[0].cast<uintptr_t>());
+  d.n = t[1].cast<int64_t>();
+  d.stride = t[2].cast<int64_t>();
+  for (int c = 0; c < 3; ++c) d.offset[c] = t[size_t(3 + c)].cast<int32_t>();
+  d.is_f32 = t[6].cast<int32_t>();
+  d.min_range = t[7].cast<double>();
+  d.max_range = t[8].cast<double>();
+  d.range_mode = t[9].cast<int32_t>();
+  d.drop_nan = t[10].cast<int32_t>();
+  return d;
+}
+
 PYBIND11_MODULE(pypeline, m) {
   bind_vector_eigen3d(m);
   py::class_<mb::Pipeline>(m, "Pipeline")
@@ -62,6 +84,20 @@ PYBIND11_MODULE(pypeline, m) {
         if (a.ndim() != 2 || a.shape(1) != 3) throw py::cast_error();
         return p.prefetch(a.data(), size_t(a.shape(0)), false, hold(a));
       }, py::arg("cloud"))
+      // additions (not in the reference): raw sensor records, filtered on the way in like the dataset readers do
+      // (mad_icp_b200/records.py describes the array; it is read in place)
+      .def("computeRecords", [](mb::Pipeline& p, double stamp, const py::object& records, double min_range, double max_range,
+                                bool inclusive, bool drop_nan) {
+        p.computeRecords(stamp, records_arg(records, min_range, max_range, inclusive, drop_nan));
+      }, py::arg("stamp"), py::arg("records"), py::arg("min_range") = 0.0,
+         py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false)
+      .def("prefetchRecords", [](mb::Pipeline& p, const py::object& records, double min_range, double max_range,
+                                 bool inclusive, bool drop_nan) {
+        const madicp_points_t d = records_arg(records, min_range, max_range, inclusive, drop_nan);
+        py::object* ref = new py::object(records);  // dropped once the scan's tree is built (see prefetch)
+        return p.prefetchRecords(d, std::shared_ptr<void>(ref, [](void* q) { delete static_cast<py::object*>(q); }));
+      }, py::arg("records"), py::arg("min_range") = 0.0,
+         py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false)
       .def("prefetched", &mb::Pipeline::prefetched)
       .def("lastIcpIterations", &mb::Pipeline::lastIcpIterations)
       .def("gpuBuild", &mb::Pipeline::gpuBuild)

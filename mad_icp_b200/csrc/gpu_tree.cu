@@ -26,18 +26,24 @@
 
 #include "ctx.hpp"
 #include "gpu_tree_kernels.cuh"
+#include "records.hpp"
 
 using namespace madicp;
 using namespace madicp::gtb;
 
 // ingest.cpp (host half of the ingest, host libm service, a parallel-for on the library's host pool)
 void madicp_host_for(int n, int num_threads, const std::function<void(int)>& fn);
-int madicp_deskew_plan(const void* xyz, int is_f32, int64_t n, const double T_prev[12], const double T_now[12],
-                       double sensor_hz, int num_threads, int32_t* perm, uint16_t* chunk, double* poses, int* n_poses);
+int madicp_deskew_plan(const madicp_points_t& pts, const double T_prev[12], const double T_now[12], double sensor_hz,
+                       int num_threads, int32_t* perm, uint16_t* chunk, double* poses, int* n_poses, int64_t* n_kept);
 void madicp_host_trig(const double* args, double* res, int n, int num_threads);
 void madicp_host_hot(int on);
 
 namespace {
+
+struct RootSums {  // Sigma x, Sigma x x^T of a scan's kept points, and their number
+  std::array<double, 9> S;
+  int64_t kept;
+};
 
 struct BuildState {
   size_t cap = 0;  // points
@@ -70,7 +76,10 @@ struct BuildState {
   Ctl* h_ctl = nullptr;
   int* h_lvl = nullptr;
   // ingest staging
-  void* d_raw = nullptr;  // the raw scan as uploaded (float32 or float64), 3 * cap doubles
+  void* d_raw = nullptr;  // the raw scans as uploaded (packed float32 or records), raw_cap bytes
+  size_t raw_cap = 0;
+  int* h_kept = nullptr;  // mapped: kept points of every scan, counted by the device's compaction (k_compact)
+  int kept_check = 0;     // scans of the resident cloud whose h_kept the next build compares with the host's count
   int* d_perm = nullptr;
   unsigned short* d_chunk = nullptr;
   double* d_poses = nullptr;
@@ -80,18 +89,19 @@ struct BuildState {
   double* h_root = nullptr;  // pinned: the root's sums when the host computes them
   double root_S[9];          // ... of the cloud madicp_ingest left in P[0] (valid when has_root_S)
   bool has_root_S = false;
-  int64_t n_resident = 0;  // points of the cloud madicp_ingest left in P[0]
+  int64_t n_resident = 0;  // points of the cloud madicp_ingest left in P[0] (the kept ones)
   uint64_t seq = 0;        // builds so far (madtree_gpu_export is valid for the latest one only)
   int threads = 16;
-  // early uploads for the next batch (madicp_stage_cloud): clouds already on their way into P[0] / d_raw, back to back
+  // early uploads for the next batch (madicp_stage_cloud / madicp_stage_points): scans already on their way into P[0]
+  // (packed float64) or d_raw (anything else, each scan on a 16-byte boundary), back to back
   struct Staged {
-    const void* ptr;
-    int64_t n;
-    std::shared_future<std::array<double, 9>> root;  // the root's sums, running on a host thread since the cloud was staged
+    madicp_points_t d;
+    std::shared_future<RootSums> root;  // the root's sums and the kept count, on a host thread since the scan was staged
   };
   std::vector<Staged> staged;
-  int64_t staged_points = 0;
-  bool staged_f32 = false, stage_closed = false;
+  int64_t staged_points = 0;  // records
+  size_t staged_bytes = 0;    // end of the last staged scan in d_raw
+  bool staged_raw = false, stage_closed = false;
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t copy_ev = nullptr, idle_ev = nullptr;  // copies done / the working buffers are free again
   std::vector<void*> dev_allocs, host_allocs;
@@ -130,9 +140,10 @@ void release(BuildState* bs) {
 }
 
 // `slot`: where the lane keeps its working memory (the context's own lane, or a builder's)
-int ensure_state(void** slot, cudaStream_t stream, size_t n, BuildState** out) {
+// n: records (every per-point array is indexed by record before the compaction), raw_bytes: the raw buffer
+int ensure_state(void** slot, cudaStream_t stream, size_t n, size_t raw_bytes, BuildState** out) {
   BuildState* bs = static_cast<BuildState*>(*slot);
-  if (bs && bs->cap >= n) {
+  if (bs && bs->cap >= n && bs->raw_cap >= raw_bytes) {
     *out = bs;
     return MADICP_OK;
   }
@@ -148,6 +159,8 @@ int ensure_state(void** slot, cudaStream_t stream, size_t n, BuildState** out) {
   size_t cap = size_t(1) << 17;
   while (cap < n) cap <<= 1;
   bs->cap = cap;
+  bs->raw_cap = 3 * sizeof(double) * cap;  // a packed float64 cloud's worth; records may need more
+  while (bs->raw_cap < raw_bytes) bs->raw_cap <<= 1;
   {  // host threads for the libm calls and the roots' sums: half the CPUs this process may run on (its affinity mask,
     // not the machine: eight ranks pinned to 16 CPUs each must not start 32 threads apiece), 4..32
     // (MADICP_HOST_THREADS overrides)
@@ -202,10 +215,11 @@ int ensure_state(void** slot, cudaStream_t stream, size_t n, BuildState** out) {
   if (!rc) rc = host_alloc(bs, &bs->h_offs, size_t(kMaxBatch) + 1);
   if (!rc) rc = host_alloc(bs, &bs->h_out, size_t(kMaxBatch));
   if (!rc) {
-    double* raw = nullptr;
-    rc = dev_alloc(bs, &raw, 3 * cap);
+    char* raw = nullptr;
+    rc = dev_alloc(bs, &raw, bs->raw_cap);
     bs->d_raw = raw;
   }
+  if (!rc) rc = host_alloc(bs, &bs->h_kept, size_t(kMaxBatch));
   if (!rc) rc = dev_alloc(bs, &bs->d_perm, cap);
   if (!rc) rc = dev_alloc(bs, &bs->d_chunk, cap);
   if (!rc) rc = dev_alloc(bs, &bs->d_poses, size_t(65536) * 12);
@@ -237,7 +251,9 @@ int ensure_state(void** slot, cudaStream_t stream, size_t n, BuildState** out) {
   *out = bs;
   return MADICP_OK;
 }
-int ensure_state(madicp_ctx* c, size_t n, BuildState** out) { return ensure_state(&c->build_state, c->stream, n, out); }
+int ensure_state(madicp_ctx* c, size_t n, size_t raw_bytes, BuildState** out) {
+  return ensure_state(&c->build_state, c->stream, n, raw_bytes, out);
+}
 
 // Whatever was staged for a batch (madicp_stage_cloud) is given up: `st` waits for the copies in flight, which write
 // into the buffers the caller is about to use.
@@ -263,17 +279,37 @@ int mark_idle(BuildState* bs, cudaStream_t st) {
 
 // Sigma x, Sigma x x^T of the whole cloud in array order (tools/utils.h:55-73) on the calling host thread: the root's
 // nine chains are the longest dependent-add chains of the build (n adds each; a CPU core retires one per ~1 ns, the
-// device one per ~10 ns), and the host has the cloud in hand while it is being copied up.
-template <class T>
-void root_sums_host(const T* p, int64_t n, double* S) {
+// device one per ~10 ns), and the host has the cloud in hand while it is being copied up.  The same pass applies the
+// scan's range gate (records.hpp): the sums run over the kept points in record order, and their count is the offset
+// of the next scan in a forest.
+template <class T, bool kPacked>
+int64_t root_sums_host(const madicp_points_t& d, double* S) {
+  const RecReader<T> rd(d);
+  const T* p = static_cast<const T*>(d.data);
+  int64_t kept = 0;
   double s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0, s5 = 0, s6 = 0, s7 = 0, s8 = 0;
-  for (int64_t i = 0; i < n; ++i) {
-    const double x = double(p[3 * i]), y = double(p[3 * i + 1]), z = double(p[3 * i + 2]);
+  for (int64_t i = 0; i < d.n; ++i) {
+    T fx, fy, fz;
+    if (kPacked) {  // (the packed N x 3 cloud, no gate: plain indexed loads)
+      fx = p[3 * i]; fy = p[3 * i + 1]; fz = p[3 * i + 2];
+    } else {
+      rd.xyz(i, fx, fy, fz);
+      if (!rd.keep(fx, fy, fz)) continue;
+    }
+    ++kept;
+    const double x = double(fx), y = double(fy), z = double(fz);
     s0 += x; s1 += y; s2 += z;
     s3 += x * x; s4 += y * x; s5 += z * x;
     s6 += y * y; s7 += z * y; s8 += z * z;
   }
   S[0] = s0; S[1] = s1; S[2] = s2; S[3] = s3; S[4] = s4; S[5] = s5; S[6] = s6; S[7] = s7; S[8] = s8;
+  return kept;
+}
+int64_t root_sums_host(const madicp_points_t& d, double* S) {
+  const int e = d.is_f32 ? 4 : 8;
+  const bool packed = !points_gated(d) && d.stride == 3 * e && d.offset[0] == 0 && d.offset[1] == e && d.offset[2] == 2 * e;
+  if (d.is_f32) return packed ? root_sums_host<float, true>(d, S) : root_sums_host<float, false>(d, S);
+  return packed ? root_sums_host<double, true>(d, S) : root_sums_host<double, false>(d, S);
 }
 
 // A few resident host threads for work that is handed over and collected later (the roots' sums of staged clouds).
@@ -284,7 +320,7 @@ void root_sums_host(const T* p, int64_t n, double* S) {
 // the caller did before touching CUDA.
 class Background {
  public:
-  using Result = std::array<double, 9>;
+  using Result = RootSums;
   explicit Background(int threads) {
     for (int i = 0; i < threads; ++i) std::thread([this]() { loop(); }).detach();
   }
@@ -327,8 +363,11 @@ int blocks(int64_t n, int per = kBlock) { return int(std::max<int64_t>(1, (n + p
 // stream `st`, as ONE forest: the level loop is the same for one tree or sixteen, and so is its latency (the in-order
 // sums are dependent-add chains; sixteen roots are sixteen chains side by side).  root_S (nullable):
 // the root's sums, already computed by the host.
+// check_kept: the first check_kept trees come from the device's compaction, whose counts (bs->h_kept) must equal the
+// host's (offs) -- compared at the first host synchronisation; a mismatch fails the build instead of building a
+// different tree.
 int build_forest(madicp_ctx* c, BuildState* bs, cudaStream_t st, int n_trees, const int* offs, double b_max, double b_min,
-                 const double* root_S, madtree_gpu** out) {
+                 const double* root_S, int check_kept, madtree_gpu** out) {
   if (!(b_max > 0.0) || !std::isfinite(b_max) || !std::isfinite(b_min)) {
     set_error("madtree_gpu_build: b_max must be finite and > 0, b_min finite");
     return MADICP_ERR_INVALID;
@@ -417,6 +456,13 @@ int build_forest(madicp_ctx* c, BuildState* bs, cudaStream_t st, int n_trees, co
     CK(cudaStreamSynchronize(st));  // the level's one host round trip: libm for the eigen-decomposition
     const auto ts1 = now();
     t_sync += us(ts0, ts1);
+    if (depth == 0)
+      for (int b = 0; b < check_kept; ++b)
+        if (bs->h_kept[b] != offs[b + 1] - offs[b]) {
+          set_error("madtree_gpu_build: scan " + std::to_string(b) + ": the device kept " + std::to_string(bs->h_kept[b]) +
+                    " points, the host " + std::to_string(offs[b + 1] - offs[b]));
+          return MADICP_ERR_STATE;
+        }
     if (depth > 0) {
       nl = bs->h_ctl[depth - 1].n_next;
       total_leaves += bs->h_ctl[depth - 1].n_leaves;
@@ -511,7 +557,7 @@ int build_forest(madicp_ctx* c, BuildState* bs, cudaStream_t st, int n_trees, co
 int build_resident(madicp_ctx* c, BuildState* bs, cudaStream_t st, int64_t n, double b_max, double b_min, const double* root_S,
                    madtree_gpu** out) {
   const int offs[2] = {0, int(n)};
-  return build_forest(c, bs, st, 1, offs, b_max, b_min, root_S, out);
+  return build_forest(c, bs, st, 1, offs, b_max, b_min, root_S, bs->kept_check, out);
 }
 
 }  // namespace
@@ -524,6 +570,245 @@ void madicp_gpu_build_release(madicp_ctx* c) {
   c->build_state = nullptr;
 }
 
+namespace {
+
+size_t align16(size_t x) { return (x + 15) & ~size_t(15); }
+// a packed float64 cloud without a gate is copied straight into the point buffer; everything else goes through d_raw
+bool is_direct(const madicp_points_t& d) {
+  return !d.is_f32 && d.stride == 24 && d.offset[0] == 0 && d.offset[1] == 8 && d.offset[2] == 16 && !points_gated(d);
+}
+// layout of one scan for the device (RecSrc, gpu_tree_kernels.cuh); raw: its byte offset in d_raw, first: its first record
+RecSrc rec_src(const madicp_points_t& d, size_t raw, int first) {
+  RecSrc s{};
+  s.raw = (long long) raw;
+  s.first = first;
+  s.stride = int(d.stride);
+  const int e = d.is_f32 ? 4 : 8;
+  const int lo = std::min(d.offset[0], std::min(d.offset[1], d.offset[2]));
+  const int hi = std::max(d.offset[0], std::max(d.offset[1], d.offset[2])) + e;
+  const int vbase = lo & ~15;
+  s.vec = (d.stride % 16 == 0) ? (hi - vbase <= 16 ? 1 : (hi - vbase <= 32 ? 2 : 0)) : 0;
+  s.vbase = s.vec ? vbase : 0;
+  for (int c = 0; c < 3; ++c) s.off[c] = d.offset[c] - s.vbase;
+  s.is_f32 = d.is_f32 ? 1 : 0;
+  s.mode = (unsigned char) d.range_mode;
+  s.drop_nan = d.drop_nan ? 1 : 0;
+  s.lo = d.is_f32 ? double(float(d.min_range)) : d.min_range;  // rounded to the field type once
+  s.hi = d.is_f32 ? double(float(d.max_range)) : d.max_range;
+  return s;
+}
+// Order-preserving compaction of the gated records of B (d_raw) into P[0]; the kept count of every scan goes to
+// bs->h_kept.
+int launch_compaction(madicp_ctx* c, BuildState* bs, cudaStream_t st, const RecBatch& B) {
+  const char* raw = static_cast<const char*>(bs->d_raw);
+  const int tiles = (B.n_rec + kTile - 1) / kTile;
+  k_gate_flags<<<blocks(B.n_rec), kBlock, 0, st>>>(B, raw, bs->flag);
+  k_scan_tiles<<<tiles, kTile, 0, st>>>(bs->flag, B.n_rec, bs->G, bs->tile);
+  k_scan_tile_sums<<<1, 1024, 0, st>>>(bs->tile, tiles);
+  k_compact<<<blocks(std::max(B.n_rec, B.count)), kBlock, 0, st>>>(B, raw, bs->flag, bs->G, bs->tile, bs->P[0], bs->h_kept);
+  c->launches += 4;
+  CK(cudaGetLastError());
+  return MADICP_OK;
+}
+
+// The batch build behind madtree_gpu_build_batch and madtree_gpu_build_batch_points (descriptors validated).
+int build_batch(madicp_ctx* c, const madicp_points_t* d, int count, double b_max, double b_min, madtree_gpu** out,
+                const char* fn) {
+  bool direct = true, gated = false;
+  int first[kMaxBatch + 1];
+  size_t raw_off[kMaxBatch + 1];
+  first[0] = 0;
+  raw_off[0] = 0;
+  for (int b = 0; b < count; ++b) {
+    direct = direct && is_direct(d[b]);
+    gated = gated || points_gated(d[b]);
+    if (int64_t(first[b]) + d[b].n > (int64_t(1) << 26)) {
+      set_error(std::string(fn) + ": more than 2^26 points in the batch");
+      return MADICP_ERR_INVALID;
+    }
+    first[b + 1] = first[b] + int(d[b].n);
+    raw_off[b + 1] = align16(raw_off[b] + size_t(d[b].n) * size_t(d[b].stride));
+  }
+  const int n_rec = first[count];
+  CK(cudaSetDevice(c->device));
+  BuildState* bs = static_cast<BuildState*>(c->build_state);
+  cudaStream_t st = c->stream;
+  const size_t raw_bytes = direct ? 0 : raw_off[count];
+  if (bs && (bs->cap < size_t(n_rec) || bs->raw_cap < raw_bytes)) {  // the lane is about to be re-allocated: early uploads are lost
+    int e = drop_staged(bs, st);
+    if (e) return e;
+  }
+  int rc = ensure_state(c, size_t(n_rec), raw_bytes, &bs);
+  if (rc) return rc;
+  const auto ta0 = std::chrono::steady_clock::now();
+  // scans uploaded ahead of time (madicp_stage_cloud / _points): the longest prefix of this batch staged in this order
+  int n_staged = 0;
+  if (!bs->staged.empty() && bs->staged_raw == !direct)
+    while (n_staged < count && n_staged < int(bs->staged.size()) && same_points(bs->staged[size_t(n_staged)].d, d[n_staged]))
+      ++n_staged;
+  std::vector<std::shared_future<RootSums>> early;
+  for (int b = 0; b < n_staged; ++b) early.push_back(bs->staged[size_t(b)].root);
+  rc = drop_staged(bs, st);  // (st waits for every early copy, used or not: they all write into the buffers used here)
+  if (rc) return rc;
+  char* raw = static_cast<char*>(bs->d_raw);
+  for (int b = n_staged; b < count; ++b) {
+    if (direct) CK(cudaMemcpyAsync(bs->P[0] + size_t(first[b]) * 3, d[b].data, size_t(d[b].n) * 24, cudaMemcpyHostToDevice, st));
+    else CK(cudaMemcpyAsync(raw + raw_off[b], d[b].data, points_bytes(d[b]), cudaMemcpyHostToDevice, st));
+  }
+  bs->n_resident = 0;  // the concatenated clouds are not "the resident cloud" of madtree_gpu_build_resident
+  bs->has_root_S = false;
+  bs->kept_check = 0;
+  if (!direct) {
+    RecBatch B;
+    B.count = count;
+    B.n_rec = n_rec;
+    for (int b = 0; b < count; ++b) B.s[b] = rec_src(d[b], raw_off[b], first[b]);
+    if (gated) {
+      if (int e = launch_compaction(c, bs, st, B)) return e;
+    } else {
+      k_ingest<<<blocks(n_rec), kBlock, 0, st>>>(B, raw, nullptr, nullptr, bs->d_poses, n_rec, bs->P[0]);
+      c->launches++;
+    }
+  }
+  const auto ta1 = std::chrono::steady_clock::now();
+  // the roots' sums and the kept counts on the host, one scan per host thread, while the scans are being copied up
+  std::vector<double> S(size_t(count) * 9);
+  std::vector<int64_t> kept(static_cast<size_t>(count));
+  if (count > n_staged) madicp_host_for(count - n_staged, bs->threads, [&](int k) {
+    const int b = n_staged + k;
+    kept[size_t(b)] = root_sums_host(d[b], S.data() + size_t(b) * 9);
+  });
+  for (int b = 0; b < n_staged; ++b) {
+    const RootSums& r = early[size_t(b)].get();
+    memcpy(S.data() + size_t(b) * 9, r.S.data(), sizeof(r.S));
+    kept[size_t(b)] = r.kept;
+  }
+  int offs[kMaxBatch + 1];
+  offs[0] = 0;
+  for (int b = 0; b < count; ++b) {
+    if (kept[size_t(b)] == 0) {
+      set_error(std::string(fn) + ": scan " + std::to_string(b) + " has no point inside the range gate");
+      return MADICP_ERR_INVALID;
+    }
+    offs[b + 1] = offs[b] + int(kept[size_t(b)]);
+  }
+  const auto tb0 = std::chrono::steady_clock::now();
+  rc = build_forest(c, bs, st, count, offs, b_max, b_min, S.data(), gated ? count : 0, out);
+  if (getenv("MADICP_BUILD_TIMING"))
+    fprintf(stderr, "%s: %d scans (%d staged), copies enqueued %.0f us, roots' sums on the host %.0f us, forest build %.0f us\n",
+            fn, count, n_staged, std::chrono::duration<double, std::micro>(ta1 - ta0).count(),
+            std::chrono::duration<double, std::micro>(tb0 - ta1).count(),
+            std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - tb0).count());
+  return rc;
+}
+
+// The early upload behind madicp_stage_cloud and madicp_stage_points (descriptor validated).
+int stage(madicp_ctx* c, const madicp_points_t& d, int64_t reserve_points) {
+  CK(cudaSetDevice(c->device));
+  BuildState* bs = static_cast<BuildState*>(c->build_state);
+  if (bs && bs->stage_closed) return MADICP_OK;
+  const bool raw = !is_direct(d);
+  const size_t bytes = size_t(d.n) * size_t(d.stride);
+  if (!bs || bs->staged.empty()) {
+    const int64_t res = std::max(reserve_points, d.n);
+    const size_t res_bytes = raw ? size_t(res) * size_t(d.stride) + 16 * size_t(kMaxBatch) : 0;
+    int rc = ensure_state(c, size_t(res), res_bytes, &bs);
+    if (rc) return rc;
+    CK(cudaEventRecord(bs->idle_ev, c->stream));  // whatever is queued on the context's stream may still use the buffers
+    CK(cudaStreamWaitEvent(bs->copy_stream, bs->idle_ev, 0));
+    bs->staged_raw = raw;
+    bs->staged_points = 0;
+    bs->staged_bytes = 0;
+    bs->n_resident = 0;  // the cloud madicp_ingest left is about to be overwritten
+    bs->has_root_S = false;
+    bs->kept_check = 0;
+  }
+  const size_t at = align16(bs->staged_bytes);
+  if (bs->staged_raw != raw || size_t(bs->staged_points + d.n) > bs->cap || (raw && at + bytes > bs->raw_cap) ||
+      int(bs->staged.size()) >= kMaxBatch) {
+    bs->stage_closed = true;  // staged scans lie back to back: nothing after a gap
+    return MADICP_OK;
+  }
+  if (raw) CK(cudaMemcpyAsync(static_cast<char*>(bs->d_raw) + at, d.data, points_bytes(d), cudaMemcpyHostToDevice, bs->copy_stream));
+  else CK(cudaMemcpyAsync(bs->P[0] + size_t(bs->staged_points) * 3, d.data, bytes, cudaMemcpyHostToDevice, bs->copy_stream));
+  // the root's sums (root_sums_host) start now too, on a background thread: the caller is about to wait for the device
+  auto sums = background().submit([d]() {
+    RootSums r;
+    r.kept = root_sums_host(d, r.S.data());
+    return r;
+  });
+  bs->staged.push_back({d, std::move(sums)});
+  bs->staged_points += d.n;
+  if (raw) bs->staged_bytes = at + bytes;
+  return MADICP_OK;
+}
+
+// The ingest behind madicp_ingest and madicp_ingest_points (descriptor validated).
+int ingest(madicp_ctx* c, const madicp_points_t& d, int deskew, const double T_prev[12], const double T_now[12],
+           double sensor_hz, int num_threads, int64_t* n_kept, double* points_out, const char* fn) {
+  CK(cudaSetDevice(c->device));
+  BuildState* bs = nullptr;
+  const int64_t n = d.n;
+  const size_t bytes = size_t(n) * size_t(d.stride);
+  int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
+  if (!rc) rc = ensure_state(c, size_t(n), bytes, &bs);
+  if (rc) return rc;
+  cudaStream_t st = c->stream;
+  bs->n_resident = 0;
+  bs->kept_check = 0;
+  // the raw scan goes up while the host works out the order (deskew) or the root's sums
+  CK(cudaMemcpyAsync(bs->d_raw, d.data, points_bytes(d), cudaMemcpyHostToDevice, st));
+  const char* raw = static_cast<const char*>(bs->d_raw);
+  RecBatch B;
+  B.count = 1;
+  B.n_rec = int(n);
+  B.s[0] = rec_src(d, 0, 0);
+  int64_t kept = n;
+  if (deskew) {
+    CK(cudaStreamSynchronize(st));  // h_perm / h_chunk / h_poses of the previous scan have been consumed
+    int n_poses = 0;
+    rc = madicp_deskew_plan(d, T_prev, T_now, sensor_hz, num_threads, bs->h_perm, bs->h_chunk, bs->h_poses, &n_poses, &kept);
+    if (rc) return rc;
+    if (kept > 0) {
+      CK(cudaMemcpyAsync(bs->d_perm, bs->h_perm, size_t(kept) * sizeof(int), cudaMemcpyHostToDevice, st));
+      CK(cudaMemcpyAsync(bs->d_chunk, bs->h_chunk, size_t(kept) * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
+      CK(cudaMemcpyAsync(bs->d_poses, bs->h_poses, size_t(n_poses) * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
+      k_ingest<<<blocks(kept), kBlock, 0, st>>>(B, raw, bs->d_perm, bs->d_chunk, bs->d_poses, int(kept), bs->P[0]);
+      c->launches++;
+    }
+  } else if (points_gated(d)) {
+    if (int e = launch_compaction(c, bs, st, B)) return e;
+    kept = root_sums_host(d, bs->root_S);
+    bs->kept_check = 1;
+  } else {
+    k_ingest<<<blocks(n), kBlock, 0, st>>>(B, raw, nullptr, nullptr, bs->d_poses, int(n), bs->P[0]);
+    c->launches++;
+    root_sums_host(d, bs->root_S);
+  }
+  CK(cudaGetLastError());
+  if (kept == 0) {
+    bs->kept_check = 0;
+    set_error(std::string(fn) + ": no point inside the range gate");
+    return MADICP_ERR_INVALID;
+  }
+  bs->n_resident = kept;
+  bs->has_root_S = !deskew;  // (a deskewed cloud exists on the device only: its root sums run there)
+  if (n_kept) *n_kept = kept;
+  if (points_out) {
+    CK(cudaMemcpyAsync(points_out, bs->P[0], size_t(kept) * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (bs->kept_check && bs->h_kept[0] != kept) {
+      set_error(std::string(fn) + ": the device kept " + std::to_string(bs->h_kept[0]) + " points, the host " +
+                std::to_string(kept));
+      bs->n_resident = 0;
+      return MADICP_ERR_STATE;
+    }
+  }
+  return MADICP_OK;
+}
+
+}  // namespace
+
 extern "C" {
 
 // A batch of scans -> their trees, built as one forest (build_forest): what Pipeline.prefetch feeds.
@@ -534,66 +819,29 @@ int madtree_gpu_build_batch(madicp_ctx_t* c, const void* const* clouds, const in
     return MADICP_ERR_INVALID;
   }
   MADICP_TRY
-  int offs[kMaxBatch + 1];
-  offs[0] = 0;
+  madicp_points_t d[kMaxBatch];
   for (int b = 0; b < count; ++b) {
-    if (!clouds[b] || n_points[b] <= 0 || n_points[b] > (int64_t(1) << 24) || int64_t(offs[b]) + n_points[b] > (int64_t(1) << 26)) {
+    if (!clouds[b] || n_points[b] <= 0 || n_points[b] > (int64_t(1) << 24)) {
       set_error("madtree_gpu_build_batch: empty cloud, or more than 2^26 points in the batch");
       return MADICP_ERR_INVALID;
     }
-    offs[b + 1] = offs[b] + int(n_points[b]);
+    d[b] = packed_points(clouds[b], n_points[b], is_f32);
   }
-  CK(cudaSetDevice(c->device));
-  BuildState* bs = static_cast<BuildState*>(c->build_state);
-  cudaStream_t st = c->stream;
-  if (bs && bs->cap < size_t(offs[count])) {  // the lane is about to be re-allocated: early uploads are lost
-    int e = drop_staged(bs, st);
-    if (e) return e;
-  }
-  int rc = ensure_state(c, size_t(offs[count]), &bs);
-  if (rc) return rc;
-  const auto ta0 = std::chrono::steady_clock::now();
-  const size_t elt = is_f32 ? sizeof(float) : sizeof(double);
-  char* dst = is_f32 ? static_cast<char*>(bs->d_raw) : reinterpret_cast<char*>(bs->P[0]);
-  // clouds uploaded ahead of time (madicp_stage_cloud): the longest prefix of this batch that was staged in this order
-  int n_staged = 0;
-  if (!bs->staged.empty() && bs->staged_f32 == (is_f32 != 0))
-    while (n_staged < count && n_staged < int(bs->staged.size()) && bs->staged[size_t(n_staged)].ptr == clouds[n_staged] &&
-           bs->staged[size_t(n_staged)].n == n_points[n_staged])
-      ++n_staged;
-  std::vector<std::shared_future<std::array<double, 9>>> early;
-  for (int b = 0; b < n_staged; ++b) early.push_back(bs->staged[size_t(b)].root);
-  rc = drop_staged(bs, st);  // (st waits for every early copy, used or not: they all write into dst)
-  if (rc) return rc;
-  for (int b = n_staged; b < count; ++b)
-    CK(cudaMemcpyAsync(dst + size_t(offs[b]) * 3 * elt, clouds[b], size_t(n_points[b]) * 3 * elt, cudaMemcpyHostToDevice, st));
-  if (is_f32) {
-    k_ingest<<<blocks(offs[count]), kBlock, 0, st>>>(bs->d_raw, 1, nullptr, nullptr, bs->d_poses, offs[count], bs->P[0]);
-    c->launches++;
-  }
-  bs->n_resident = 0;  // the concatenated clouds are not "the resident cloud" of madtree_gpu_build_resident
-  bs->has_root_S = false;
-  const auto ta1 = std::chrono::steady_clock::now();
-  // the roots' sums on the host, one scan per host thread, while the clouds are being copied up (see root_sums_host)
-  std::vector<double> S(size_t(count) * 9);
-  if (count > n_staged) madicp_host_for(count - n_staged, bs->threads, [&](int k) {
-    const int b = n_staged + k;
-    if (is_f32) root_sums_host(static_cast<const float*>(clouds[b]), n_points[b], S.data() + size_t(b) * 9);
-    else root_sums_host(static_cast<const double*>(clouds[b]), n_points[b], S.data() + size_t(b) * 9);
-  });
-  for (int b = 0; b < n_staged; ++b) {
-    const std::array<double, 9> r = early[size_t(b)].get();
-    memcpy(S.data() + size_t(b) * 9, r.data(), sizeof(r));
-  }
-  const auto tb0 = std::chrono::steady_clock::now();
-  rc = build_forest(c, bs, st, count, offs, b_max, b_min, S.data(), out);
-  if (getenv("MADICP_BUILD_TIMING"))
-    fprintf(stderr, "madtree_gpu_build_batch: %d scans, copies enqueued %.0f us, roots' sums on the host %.0f us, forest build %.0f us\n",
-            count, std::chrono::duration<double, std::micro>(ta1 - ta0).count(),
-            std::chrono::duration<double, std::micro>(tb0 - ta1).count(),
-            std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - tb0).count());
-  return rc;
+  return build_batch(c, d, count, b_max, b_min, out, "madtree_gpu_build_batch");
   MADICP_CATCH("madtree_gpu_build_batch")
+}
+
+int madtree_gpu_build_batch_points(madicp_ctx_t* c, const madicp_points_t* descs, int count, double b_max, double b_min,
+                                   madtree_gpu_t** out) {
+  if (!c || !descs || !out || count < 1 || count > kMaxBatch) {
+    set_error("madtree_gpu_build_batch_points: bad arguments (1..64 scans)");
+    return MADICP_ERR_INVALID;
+  }
+  for (int b = 0; b < count; ++b)
+    if (int e = check_points(descs + b, "madtree_gpu_build_batch_points")) return e;
+  MADICP_TRY
+  return build_batch(c, descs, count, b_max, b_min, out, "madtree_gpu_build_batch_points");
+  MADICP_CATCH("madtree_gpu_build_batch_points")
 }
 
 int madicp_stage_cloud(madicp_ctx_t* c, const void* cloud, int64_t n, int is_f32, int64_t reserve_points) {
@@ -602,37 +850,19 @@ int madicp_stage_cloud(madicp_ctx_t* c, const void* cloud, int64_t n, int is_f32
     return MADICP_ERR_INVALID;
   }
   MADICP_TRY
-  CK(cudaSetDevice(c->device));
-  BuildState* bs = static_cast<BuildState*>(c->build_state);
-  if (bs && bs->stage_closed) return MADICP_OK;
-  if (!bs || bs->staged.empty()) {
-    int rc = ensure_state(c, size_t(std::max(reserve_points, n)), &bs);
-    if (rc) return rc;
-    CK(cudaEventRecord(bs->idle_ev, c->stream));  // whatever is queued on the context's stream may still use the buffers
-    CK(cudaStreamWaitEvent(bs->copy_stream, bs->idle_ev, 0));
-    bs->staged_f32 = is_f32 != 0;
-    bs->staged_points = 0;
-    bs->n_resident = 0;  // the cloud madicp_ingest left is about to be overwritten
-    bs->has_root_S = false;
-  }
-  if (bs->staged_f32 != (is_f32 != 0) || size_t(bs->staged_points + n) > bs->cap || int(bs->staged.size()) >= kMaxBatch) {
-    bs->stage_closed = true;  // staged clouds lie back to back: nothing after a gap
-    return MADICP_OK;
-  }
-  const size_t elt = is_f32 ? sizeof(float) : sizeof(double);
-  char* dst = is_f32 ? static_cast<char*>(bs->d_raw) : reinterpret_cast<char*>(bs->P[0]);
-  CK(cudaMemcpyAsync(dst + size_t(bs->staged_points) * 3 * elt, cloud, size_t(n) * 3 * elt, cudaMemcpyHostToDevice, bs->copy_stream));
-  // the root's sums (root_sums_host) start now too, on a background thread: the caller is about to wait for the device
-  auto sums = background().submit([cloud, n, is_f32]() {
-    std::array<double, 9> S{};
-    if (is_f32) root_sums_host(static_cast<const float*>(cloud), n, S.data());
-    else root_sums_host(static_cast<const double*>(cloud), n, S.data());
-    return S;
-  });
-  bs->staged.push_back({cloud, n, std::move(sums)});
-  bs->staged_points += n;
-  return MADICP_OK;
+  return stage(c, packed_points(cloud, n, is_f32), reserve_points);
   MADICP_CATCH("madicp_stage_cloud")
+}
+
+int madicp_stage_points(madicp_ctx_t* c, const madicp_points_t* desc, int64_t reserve_points) {
+  if (!c || reserve_points > (int64_t(1) << 26)) {
+    set_error("madicp_stage_points: bad arguments");
+    return MADICP_ERR_INVALID;
+  }
+  if (int e = check_points(desc, "madicp_stage_points")) return e;
+  MADICP_TRY
+  return stage(c, *desc, reserve_points);
+  MADICP_CATCH("madicp_stage_points")
 }
 
 int madicp_stage_discard(madicp_ctx_t* c) {
@@ -659,11 +889,12 @@ int madtree_gpu_build(madicp_ctx_t* c, const double* points_xyz, int64_t n, doub
   CK(cudaSetDevice(c->device));
   BuildState* bs = nullptr;
   int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
-  if (!rc) rc = ensure_state(c, size_t(n), &bs);
+  if (!rc) rc = ensure_state(c, size_t(n), 0, &bs);
   if (rc) return rc;
   CK(cudaMemcpyAsync(bs->P[0], points_xyz, size_t(n) * 3 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   bs->n_resident = n;
-  root_sums_host(points_xyz, n, bs->root_S);
+  bs->kept_check = 0;
+  root_sums_host(packed_points(points_xyz, n, 0), bs->root_S);
   bs->has_root_S = true;
   return build_resident(c, bs, c->stream, n, b_max, b_min, bs->root_S, out);
   MADICP_CATCH("madtree_gpu_build")
@@ -714,44 +945,43 @@ int madicp_ingest(madicp_ctx_t* c, const void* xyz, int64_t n, int is_f32, int d
     return MADICP_ERR_INVALID;
   }
   MADICP_TRY
-  CK(cudaSetDevice(c->device));
-  BuildState* bs = nullptr;
-  int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
-  if (!rc) rc = ensure_state(c, size_t(n), &bs);
-  if (rc) return rc;
-  const size_t raw_bytes = size_t(n) * 3 * (is_f32 ? sizeof(float) : sizeof(double));
-  cudaStream_t st = c->stream;
-  // the raw scan goes up while the host works out the order (deskew only)
-  CK(cudaMemcpyAsync(bs->d_raw, xyz, raw_bytes, cudaMemcpyHostToDevice, st));
-  const int* d_perm = nullptr;
-  const unsigned short* d_chunk = nullptr;
-  if (deskew) {
-    CK(cudaStreamSynchronize(st));  // h_perm / h_chunk / h_poses of the previous scan have been consumed
-    int n_poses = 0;
-    rc = madicp_deskew_plan(xyz, is_f32, n, T_prev, T_now, sensor_hz, num_threads, bs->h_perm, bs->h_chunk, bs->h_poses,
-                            &n_poses);
-    if (rc) return rc;
-    CK(cudaMemcpyAsync(bs->d_perm, bs->h_perm, size_t(n) * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(bs->d_chunk, bs->h_chunk, size_t(n) * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(bs->d_poses, bs->h_poses, size_t(n_poses) * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
-    d_perm = bs->d_perm;
-    d_chunk = bs->d_chunk;
-  }
-  k_ingest<<<blocks(n), kBlock, 0, st>>>(bs->d_raw, is_f32, d_perm, d_chunk, bs->d_poses, int(n), bs->P[0]);
-  c->launches++;
-  CK(cudaGetLastError());
-  bs->n_resident = n;
-  bs->has_root_S = !deskew;  // (a deskewed cloud exists on the device only: its root sums run there)
-  if (!deskew) {
-    if (is_f32) root_sums_host(static_cast<const float*>(xyz), n, bs->root_S);
-    else root_sums_host(static_cast<const double*>(xyz), n, bs->root_S);
-  }
-  if (points_out) {
-    CK(cudaMemcpyAsync(points_out, bs->P[0], size_t(n) * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return MADICP_OK;
+  return ingest(c, packed_points(xyz, n, is_f32), deskew, T_prev, T_now, sensor_hz, num_threads, nullptr, points_out,
+                "madicp_ingest");
   MADICP_CATCH("madicp_ingest")
+}
+
+int madicp_ingest_points(madicp_ctx_t* c, const madicp_points_t* desc, int deskew, const double T_prev[12],
+                         const double T_now[12], double sensor_hz, int num_threads, int64_t* n_kept, double* points_out) {
+  if (!c || (deskew && (!T_prev || !T_now || !(sensor_hz > 0.0)))) {
+    set_error("madicp_ingest_points: bad arguments");
+    return MADICP_ERR_INVALID;
+  }
+  if (int e = check_points(desc, "madicp_ingest_points")) return e;
+  MADICP_TRY
+  return ingest(c, *desc, deskew, T_prev, T_now, sensor_hz, num_threads, n_kept, points_out, "madicp_ingest_points");
+  MADICP_CATCH("madicp_ingest_points")
+}
+
+int64_t madicp_debug_range_mask(const madicp_points_t* desc, uint8_t* keep) {
+  if (int e = check_points(desc, "madicp_debug_range_mask")) return e;
+  if (!keep) {
+    set_error("madicp_debug_range_mask: null output");
+    return MADICP_ERR_INVALID;
+  }
+  int64_t kept = 0;
+  auto run = [&](auto zero) {
+    using T = decltype(zero);
+    const RecReader<T> rd(*desc);
+    for (int64_t i = 0; i < desc->n; ++i) {
+      T x, y, z;
+      rd.xyz(i, x, y, z);
+      keep[i] = rd.keep(x, y, z) ? 1 : 0;
+      kept += keep[i];
+    }
+  };
+  if (desc->is_f32) run(0.0f);
+  else run(0.0);
+  return kept;
 }
 
 }  // extern "C"

@@ -22,6 +22,7 @@
 #include "../../include/madicp_b200.h"
 #include "arith.h"
 #include "eig3.h"
+#include "range_gate.h"
 
 namespace madicp {
 namespace gtb {
@@ -842,23 +843,118 @@ k_records(Nodes N, int n_nodes, int n_points, const int* __restrict__ G, const i
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Ingest (odometry/pipeline.cpp:79-123 + the float32 -> float64 conversion of the readers): out[i] = T[chunk[i]] *
-// in[perm[i]], with the reference's operand order (Isometry * point = R p + t, dot3 rows) and no FMA.
-// perm == nullptr: identity; chunk == nullptr: no transform (conversion only).
+// Raw records (madicp_points_t) as uploaded: the scans of a batch lie in the raw buffer one after the other, each
+// starting on a 16-byte boundary.  Their layouts travel as a __grid_constant__ kernel parameter (no copy, no host
+// buffer that a later call could overwrite while a copy is pending).  A record is read with the widest aligned loads
+// its stride allows: when the stride is a multiple of 16 and x, y, z lie within one (two) aligned 16-byte chunk(s),
+// one (two) 128-bit load(s) -- one per KITTI record, one per 48-byte Ouster record -- else one load per field.
+struct RecSrc {
+  long long raw;       // byte offset of the scan's first record in the raw buffer
+  int first;           // index of that record in the batch's record sequence
+  int stride;          // bytes
+  int off[3];          // byte offsets of x, y, z: from `vbase` when vec > 0, from the record start otherwise
+  int vbase;           // start of the first 16-byte chunk holding x, y, z
+  unsigned char is_f32, vec, mode, drop_nan;  // vec: 128-bit loads per record (0: one load per field)
+  double lo, hi;       // the gate's bounds, already rounded to the field type
+};
+struct RecBatch {
+  int count;  // scans
+  int n_rec;  // records of all scans
+  RecSrc s[kMaxBatch];
+};
+
+__device__ __forceinline__ unsigned chunk_word(const uint4& a, const uint4& b, int k) {  // word k of the 32 bytes a|b
+  const int j = k & 3;
+  const unsigned wa = j == 0 ? a.x : j == 1 ? a.y : j == 2 ? a.z : a.w;
+  const unsigned wb = j == 0 ? b.x : j == 1 ? b.y : j == 2 ? b.z : b.w;
+  return k < 4 ? wa : wb;
+}
+__device__ __forceinline__ int rec_scan(const RecBatch& B, int r) {  // scan of record r: first[lo] <= r < first[lo + 1]
+  int lo = 0, hi = B.count;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (B.s[mid].first <= r) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+// record r of the batch -> float64 x, y, z; returns whether the scan's range gate keeps it (range_gate.h)
+__device__ __forceinline__ bool read_record(const RecBatch& B, const char* __restrict__ raw, int r, double& x, double& y,
+                                            double& z) {
+  const RecSrc& s = B.s[rec_scan(B, r)];
+  const char* rec = raw + s.raw + (long long)(r - s.first) * s.stride;
+  if (s.is_f32) {
+    float fx, fy, fz;
+    if (s.vec) {
+      const uint4 a = __ldg(reinterpret_cast<const uint4*>(rec + s.vbase));
+      const uint4 b = s.vec > 1 ? __ldg(reinterpret_cast<const uint4*>(rec + s.vbase + 16)) : a;
+      fx = __uint_as_float(chunk_word(a, b, s.off[0] >> 2));
+      fy = __uint_as_float(chunk_word(a, b, s.off[1] >> 2));
+      fz = __uint_as_float(chunk_word(a, b, s.off[2] >> 2));
+    } else {
+      fx = __ldg(reinterpret_cast<const float*>(rec + s.off[0]));
+      fy = __ldg(reinterpret_cast<const float*>(rec + s.off[1]));
+      fz = __ldg(reinterpret_cast<const float*>(rec + s.off[2]));
+    }
+    x = double(fx); y = double(fy); z = double(fz);
+    return range_keep<float>(fx, fy, fz, float(s.lo), float(s.hi), s.mode, s.drop_nan);
+  }
+  if (s.vec) {
+    const uint4 a = __ldg(reinterpret_cast<const uint4*>(rec + s.vbase));
+    const uint4 b = s.vec > 1 ? __ldg(reinterpret_cast<const uint4*>(rec + s.vbase + 16)) : a;
+    const int kx = s.off[0] >> 2, ky = s.off[1] >> 2, kz = s.off[2] >> 2;
+    x = __hiloint2double(int(chunk_word(a, b, kx + 1)), int(chunk_word(a, b, kx)));
+    y = __hiloint2double(int(chunk_word(a, b, ky + 1)), int(chunk_word(a, b, ky)));
+    z = __hiloint2double(int(chunk_word(a, b, kz + 1)), int(chunk_word(a, b, kz)));
+  } else {
+    x = __ldg(reinterpret_cast<const double*>(rec + s.off[0]));
+    y = __ldg(reinterpret_cast<const double*>(rec + s.off[1]));
+    z = __ldg(reinterpret_cast<const double*>(rec + s.off[2]));
+  }
+  return range_keep<double>(x, y, z, s.lo, s.hi, s.mode, s.drop_nan);
+}
+
+// Order-preserving compaction of the gated records (no deskew): flags -> the tile scan above (k_scan_tiles +
+// k_scan_tile_sums: G[i] + tile[i >> 10] = kept records before i) -> every kept record converted and written at its
+// rank.  The scans of a batch lie back to back, so that rank is also the point's position in the forest.  No atomics
+// anywhere: the order is the records' order.
 __global__ void __launch_bounds__(kBlock)
-k_ingest(const void* __restrict__ in, int is_f32, const int* __restrict__ perm, const unsigned short* __restrict__ chunk,
-         const double* __restrict__ poses /* n_chunks x 12 */, int n, double* __restrict__ out) {
+k_gate_flags(const __grid_constant__ RecBatch B, const char* __restrict__ raw, unsigned char* __restrict__ flag) {
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  if (i >= B.n_rec) return;
+  double x, y, z;
+  flag[i] = read_record(B, raw, i, x, y, z) ? 1 : 0;
+}
+// kept (mapped host memory): kept points of every scan, for the build to compare with the host's count
+__global__ void __launch_bounds__(kBlock)
+k_compact(const __grid_constant__ RecBatch B, const char* __restrict__ raw, const unsigned char* __restrict__ flag,
+          const int* __restrict__ G, const int* __restrict__ tile_off, double* __restrict__ out, int* __restrict__ kept) {
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  const int n = B.n_rec;
+  auto rank = [&](int r) {  // kept records before r
+    return r < n ? G[r] + tile_off[r >> 10] : G[n - 1] + tile_off[(n - 1) >> 10] + int(flag[n - 1]);
+  };
+  if (i < B.count) kept[i] = rank(i + 1 < B.count ? B.s[i + 1].first : n) - rank(B.s[i].first);
+  if (i >= n || !flag[i]) return;
+  double x, y, z;
+  read_record(B, raw, i, x, y, z);
+  const size_t o = size_t(rank(i));
+  out[3 * o] = x;
+  out[3 * o + 1] = y;
+  out[3 * o + 2] = z;
+}
+
+// Ingest (odometry/pipeline.cpp:79-123 + the float32 -> float64 conversion of the readers): out[i] = T[chunk[i]] *
+// record(perm[i]), with the reference's operand order (Isometry * point = R p + t, dot3 rows) and no FMA.
+// perm == nullptr: identity; chunk == nullptr: no transform (conversion only).  The gate is not applied here: perm
+// holds kept records only (madicp_deskew_plan), and without perm the batch has no gate.
+__global__ void __launch_bounds__(kBlock)
+k_ingest(const __grid_constant__ RecBatch B, const char* __restrict__ raw, const int* __restrict__ perm,
+         const unsigned short* __restrict__ chunk, const double* __restrict__ poses /* n_chunks x 12 */, int n,
+         double* __restrict__ out) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
   if (i >= n) return;
-  const size_t s = size_t(perm ? perm[i] : i);
   double x, y, z;
-  if (is_f32) {
-    const float* p = static_cast<const float*>(in) + 3 * s;
-    x = double(p[0]); y = double(p[1]); z = double(p[2]);
-  } else {
-    const double* p = static_cast<const double*>(in) + 3 * s;
-    x = p[0]; y = p[1]; z = p[2];
-  }
+  read_record(B, raw, perm ? perm[i] : i, x, y, z);
   if (chunk) {
     const double* X = poses + size_t(chunk[i]) * 12;
     double ox, oy, oz;

@@ -26,10 +26,7 @@
 #include "../../include/madicp_b200_debug.h"
 #include "host_pool.hpp"
 #include "pose_math.h"
-
-namespace madicp {
-void set_error(const std::string& msg);
-}
+#include "records.hpp"
 
 namespace {
 using madicp_host::default_init_allocator;
@@ -236,16 +233,19 @@ extern "C" int madicp_deskew(double* points_xyz, int64_t n, const double T_prev[
 // an ORDER or calls libm -- azimuths (atan2), the reference's sort permutation, the chunk of every sorted position,
 // the chunk poses (sin/cos inside the exponential map) -- and nothing that touches the points' values: the gather,
 // the float -> double conversion and the rigid transform run on the device.
-// perm[i] = input index of the point at sorted position i; chunk[i] = its pose; poses: (*n_poses) x 12 row-major.
-int madicp_deskew_plan(const void* xyz, int is_f32, int64_t n, const double T_prev[12], const double T_now[12],
-                       double sensor_hz, int num_threads, int32_t* perm, uint16_t* chunk, double* poses, int* n_poses) {
-  if (!xyz || !T_prev || !T_now || n <= 0 || n > (int64_t(1) << 30) || !(sensor_hz > 0.0)) {
+// The records are read through their descriptor and the range gate (records.hpp) is applied in the azimuth pass: the
+// sort sees the kept points in record order, exactly the cloud the reader would have handed over.
+// perm[i] = record index of the kept point at sorted position i; chunk[i] = its pose; poses: (*n_poses) x 12
+// row-major; *n_kept = number of kept points (entries of perm / chunk).
+int madicp_deskew_plan(const madicp_points_t& pts, const double T_prev[12], const double T_now[12], double sensor_hz,
+                       int num_threads, int32_t* perm, uint16_t* chunk, double* poses, int* n_poses, int64_t* n_kept) {
+  const int64_t n_rec = pts.n;
+  if (!pts.data || !T_prev || !T_now || n_rec <= 0 || n_rec > (int64_t(1) << 30) || !(sensor_hz > 0.0)) {
     madicp::set_error("madicp_ingest: bad arguments");
     return MADICP_ERR_INVALID;
   }
   int threads = num_threads < 1 ? 1 : (num_threads > 64 ? 64 : num_threads);
-  if (n < 20000) threads = 1;
-  const size_t un = size_t(n);
+  if (n_rec < 20000) threads = 1;
   const double ts = 1. / sensor_hz;
   Pose a, b;
   std::memcpy(a.m, T_prev, sizeof(a.m));
@@ -256,17 +256,32 @@ int madicp_deskew_plan(const void* xyz, int is_f32, int64_t n, const double T_pr
   const double vel[6] = {rel.m[3] / ts, rel.m[7] / ts, rel.m[11] / ts, w[0] / ts, w[1] / ts, w[2] / ts};
   const double resolution = 2 * M_PI / double(kChunks), delta = ts / double(kChunks - 1);
   madicp_host::HotScope hot;
-  RawVec<Item> items(un);
-  const float* xf = static_cast<const float*>(xyz);
-  const double* xd = static_cast<const double*>(xyz);
-  for_chunks(threads, un, 8192, [&](size_t c0, size_t c1) {
-    for (size_t i = c0; i < c1; ++i) {
-      const double x = is_f32 ? double(xf[3 * i]) : xd[3 * i], y = is_f32 ? double(xf[3 * i + 1]) : xd[3 * i + 1];
-      items[i] = Item{std::atan2(y, x), int32_t(i), 0};
-    }
-  });
+  RawVec<Item> items(static_cast<size_t>(n_rec));
+  auto azimuths = [&](auto zero) {  // (pad = 1: the record survives the gate)
+    using T = decltype(zero);
+    const madicp::RecReader<T> rd(pts);
+    for_chunks(threads, size_t(n_rec), 8192, [&](size_t c0, size_t c1) {
+      for (size_t i = c0; i < c1; ++i) {
+        T x, y, z;
+        rd.xyz(int64_t(i), x, y, z);
+        items[i] = Item{std::atan2(double(y), double(x)), int32_t(i), rd.keep(x, y, z) ? 1 : 0};
+      }
+    });
+  };
+  if (pts.is_f32) azimuths(0.0f);
+  else azimuths(0.0);
+  size_t un = size_t(n_rec);
+  if (madicp::points_gated(pts)) {  // the kept records, in record order
+    un = 0;
+    for (size_t i = 0; i < size_t(n_rec); ++i)
+      if (items[i].pad) items[un++] = items[i];
+  }
+  *n_kept = int64_t(un);
+  *n_poses = 0;
+  if (un == 0) return MADICP_OK;
+  const int64_t n = int64_t(un);
   if (threads > 1) sort_like_std(items.data(), items.data() + un, threads);
-  else std::sort(items.begin(), items.end(), KeyLess());
+  else std::sort(items.begin(), items.begin() + ptrdiff_t(un), KeyLess());
   RawVec<int32_t> cid(un);
   int32_t last = 0;
   sweep(items.data(), n, resolution, cid, last);

@@ -1,0 +1,85 @@
+// records.hpp -- host side of madicp_points_t (include/madicp_b200.h): validation, field reads, the range gate
+// (range_gate.h) with its bounds rounded to the field type.  Shared by gpu_tree.cu and ingest.cpp.
+#pragma once
+#include <algorithm>
+#include <cmath>
+#include <cstdint>
+#include <cstring>
+#include <string>
+
+#include "../../include/madicp_b200.h"
+#include "range_gate.h"
+
+namespace madicp {
+void set_error(const std::string& msg);
+
+// the packed N x 3 cloud of madicp_ingest / madicp_stage_cloud / madtree_gpu_build_batch
+inline madicp_points_t packed_points(const void* xyz, int64_t n, int is_f32) {
+  madicp_points_t d{};
+  const int32_t e = is_f32 ? 4 : 8;
+  d.data = xyz;
+  d.n = n;
+  d.stride = 3 * e;
+  d.offset[0] = 0; d.offset[1] = e; d.offset[2] = 2 * e;
+  d.is_f32 = is_f32 ? 1 : 0;
+  d.range_mode = kGateNone;
+  return d;
+}
+inline bool points_gated(const madicp_points_t& d) { return d.range_mode != kGateNone || d.drop_nan; }
+// bytes from the first record's start to the end of the last record's last field: what is read (and uploaded), so
+// that a view whose last record is cut short (e.g. the x/y/z columns of a larger array) is never read past its end
+inline size_t points_bytes(const madicp_points_t& d) {
+  const int64_t e = d.is_f32 ? 4 : 8;
+  const int64_t end = std::max(d.offset[0], std::max(d.offset[1], d.offset[2])) + e;
+  return size_t((d.n - 1) * d.stride + end);
+}
+inline bool same_points(const madicp_points_t& a, const madicp_points_t& b) {
+  return a.data == b.data && a.n == b.n && a.stride == b.stride && a.offset[0] == b.offset[0] && a.offset[1] == b.offset[1] &&
+         a.offset[2] == b.offset[2] && (a.is_f32 != 0) == (b.is_f32 != 0) && a.min_range == b.min_range &&
+         a.max_range == b.max_range && a.range_mode == b.range_mode && (a.drop_nan != 0) == (b.drop_nan != 0);
+}
+
+// MADICP_OK, or MADICP_ERR_INVALID with a message naming `fn`
+inline int check_points(const madicp_points_t* d, const char* fn) {
+  auto bad = [fn](const std::string& why) {
+    set_error(std::string(fn) + ": " + why);
+    return MADICP_ERR_INVALID;
+  };
+  if (!d) return bad("null descriptor");
+  if (!d->data) return bad("null data");
+  if (d->n < 1 || d->n > (int64_t(1) << 24)) return bad("n must be 1..2^24 records");
+  const int64_t e = d->is_f32 ? 4 : 8;
+  if (d->stride < 1 || d->stride > 65536 || d->stride % e)
+    return bad("stride must be a positive multiple of the field size, at most 65536 bytes");
+  for (int c = 0; c < 3; ++c) {
+    if (d->offset[c] < 0 || d->offset[c] + e > d->stride) return bad("field " + std::to_string(c) + " does not fit the stride");
+    if (d->offset[c] % e) return bad("field " + std::to_string(c) + " offset is not a multiple of the field size");
+  }
+  if (std::isnan(d->min_range) || std::isnan(d->max_range)) return bad("NaN range bound");
+  if (d->min_range > d->max_range) return bad("min_range > max_range");
+  if (d->range_mode < kGateNone || d->range_mode > kGateStrict) return bad("range_mode must be 0, 1 or 2");
+  return MADICP_OK;
+}
+
+// The gate of one descriptor in field type T
+template <class T>
+struct RecReader {
+  const char* base;
+  int64_t stride;
+  int32_t off[3];
+  T lo, hi;
+  int mode, drop_nan;
+  bool gated;
+  explicit RecReader(const madicp_points_t& d)
+      : base(static_cast<const char*>(d.data)), stride(d.stride), off{d.offset[0], d.offset[1], d.offset[2]},
+        lo(T(d.min_range)), hi(T(d.max_range)), mode(d.range_mode), drop_nan(d.drop_nan), gated(points_gated(d)) {}
+  void xyz(int64_t i, T& x, T& y, T& z) const {
+    const char* r = base + i * stride;
+    std::memcpy(&x, r + off[0], sizeof(T));
+    std::memcpy(&y, r + off[1], sizeof(T));
+    std::memcpy(&z, r + off[2], sizeof(T));
+  }
+  bool keep(T x, T y, T z) const { return !gated || range_keep<T>(x, y, z, lo, hi, mode, drop_nan); }
+};
+
+}  // namespace madicp

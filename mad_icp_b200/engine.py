@@ -3,11 +3,13 @@ and `Registrar` (one GPU: keyframe slots + moving leaves + the persistent Gauss-
 These are the objects the reference-named facade (mad_icp_b200.api / the pybind modules) and
 bench.py drive; they add no arithmetic of their own."""
 import ctypes as C
+import math
 
 import numpy as np
 
 from . import _capi as capi
 from ._capi import MadIcpError, as_b, as_d, as_i, check, pose12
+from .records import describe
 
 
 class FlatTree:
@@ -210,6 +212,36 @@ class Registrar:
         check(capi.lib().madicp_ingest(self._h, a.ctypes.data_as(C.c_void_p), n, int(a.dtype == np.float32), int(deskew),
                                        Tp, Tn, sensor_hz, num_threads, as_d(out)), "madicp_ingest")
         return out
+
+    # ---- raw sensor records (records.describe: strided x/y/z + the readers' range gate), read in place
+    def ingest_records(self, records, min_range=0.0, max_range=math.inf, inclusive=True, drop_nan=False, deskew=False,
+                       T_prev=None, T_now=None, sensor_hz=10.0, num_threads=1, want_points=False):
+        """Records -> device-resident float64 cloud of the kept points (madicp_ingest_points).  Returns the kept points
+        (want_points) or their number."""
+        d = describe(records, min_range, max_range, inclusive, drop_nan)
+        out = np.empty((d.n, 3)) if want_points else None
+        kept = C.c_int64(0)
+        Tp = as_d(pose12(T_prev)) if T_prev is not None else None
+        Tn = as_d(pose12(T_now)) if T_now is not None else None
+        check(capi.lib().madicp_ingest_points(self._h, C.byref(d), int(deskew), Tp, Tn, sensor_hz, num_threads,
+                                              C.byref(kept), as_d(out)), "madicp_ingest_points")
+        return out[:kept.value].copy() if want_points else kept.value
+
+    def stage_records(self, records, reserve_points=0, **gate):
+        """Early upload of the records of a scan of the NEXT build_trees_records call (madicp_stage_points); pass the
+        same array and gate there, unchanged."""
+        d = describe(records, **gate)
+        self._staged_keepalive.append(records)
+        check(capi.lib().madicp_stage_points(self._h, C.byref(d), int(reserve_points)), "madicp_stage_points")
+
+    def build_trees_records(self, records_list, b_max=0.2, b_min=0.1, **gate):
+        """Several scans of records at once: one forest build, a DeviceTree per scan (madtree_gpu_build_batch_points)."""
+        k = len(records_list)
+        descs = (capi.Points * k)(*[describe(r, **gate) for r in records_list])
+        out = (C.c_void_p * k)()
+        check(capi.lib().madtree_gpu_build_batch_points(self._h, descs, k, b_max, b_min, out), "madtree_gpu_build_batch_points")
+        self._staged_keepalive.clear()
+        return [DeviceTree(C.c_void_p(out[i]), self) for i in range(k)]
 
     def set_moving_tree(self, tree):
         check(capi.lib().madicp_set_moving_tree(self._h, tree._h), "madicp_set_moving_tree")

@@ -222,6 +222,32 @@ int madicp_stage_points(madicp_ctx_t* ctx, const madicp_points_t* desc, int64_t 
 int madtree_gpu_build_batch_points(madicp_ctx_t* ctx, const madicp_points_t* descs, int count, double b_max, double b_min,
                                    madtree_gpu_t** out);
 
+/* KITTI's vertical-angle correction, applied to the kept points after the range gate, bit for bit with the reader's
+ * (apps/utils/kitti_reader.py:72-79, 90-91; scipy 1.18):
+ *   rotation_vectors = np.cross(points, np.array([0., 0., 1.]))
+ *   norms = np.linalg.norm(rotation_vectors, axis=1).reshape(-1, 1)
+ *   rotations = R.from_rotvec(angle * rotation_vectors / norms)          (angle: np.radians(0.205) in the reader)
+ *   points = rotations.apply(points)
+ * The gate still decides on the raw values.  A point with x = y = 0 becomes a NaN row, as in the reader.  An enabled
+ * correction with a NaN or infinite angle is MADICP_ERR_INVALID; a point whose rotation angle the library cannot
+ * evaluate exactly (float64 coordinates with |x|, |y| below ~1e-154, not both zero) fails the call with
+ * MADICP_ERR_STATE instead of producing a different point. */
+typedef struct madicp_vcorr {
+  double angle;    /* radians */
+  int32_t enabled; /* 0: no correction */
+  int32_t reserved;
+} madicp_vcorr_t;
+/* The _points calls with a correction: vcorr (nullable: none) for the scan, or `count` entries for the batch, one per
+ * scan.  The _points calls are these with vcorr = NULL.  A staged scan is reused when its descriptor and its
+ * correction are equal. */
+int madicp_ingest_points_ex(madicp_ctx_t* ctx, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int deskew,
+                            const double T_prev[12], const double T_now[12], double sensor_hz, int num_threads,
+                            int64_t* n_kept, double* points_out);
+int madicp_stage_points_ex(madicp_ctx_t* ctx, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
+                           int64_t reserve_points);
+int madtree_gpu_build_batch_points_ex(madicp_ctx_t* ctx, const madicp_points_t* descs, const madicp_vcorr_t* vcorrs,
+                                      int count, double b_max, double b_min, madtree_gpu_t** out);
+
 /* K1 only -- MADtree::bestMatchingLeafFast (tools/mad_tree.cpp:144-152) of X*mean for every moving
  * leaf against every active keyframe.  out_ordinals: K_active x L int32 on the host (row k = k-th
  * active slot in ascending slot order); values are getLeafs ordinals of the matched leaf. */

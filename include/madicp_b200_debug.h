@@ -45,6 +45,11 @@ int64_t madicp_debug_sort_check(int64_t n, uint32_t seed, int64_t distinct, int 
  * Returns the number of kept records.  No device work. */
 int64_t madicp_debug_range_mask(const madicp_points_t* desc, uint8_t* keep);
 
+/* The kept points of madicp_points_t, corrected by `vcorr` (nullable: none), on the host with the restatement the
+ * device applies: out receives (return value) x 3 doubles, at most desc->n rows.  Validates like
+ * madicp_debug_range_mask; MADICP_ERR_STATE when a point's rotation angle falls outside the table.  No device work. */
+int64_t madicp_debug_correct_points(const madicp_points_t* desc, const madicp_vcorr_t* vcorr, double* out);
+
 #ifdef __cplusplus
 }
 #endif

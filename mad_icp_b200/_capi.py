@@ -27,6 +27,14 @@ class Points(C.Structure):
 assert C.sizeof(Points) == 64
 pts_p = C.POINTER(Points)
 
+
+class Vcorr(C.Structure):
+    """madicp_vcorr_t: KITTI's vertical-angle correction of the kept points (enabled != 0)."""
+    _fields_ = [("angle", C.c_double), ("enabled", C.c_int32), ("reserved", C.c_int32)]
+
+
+vc_p = C.POINTER(Vcorr)
+
 # every symbol include/madicp_b200.h and include/madicp_b200_debug.h declare: name -> (restype, argtypes)
 SYMBOLS = {
     "madicp_last_error": (C.c_char_p, []),
@@ -72,6 +80,10 @@ SYMBOLS = {
     "madicp_stage_points": (C.c_int, [vp, pts_p, C.c_int64]),
     "madtree_gpu_build_batch_points": (C.c_int, [vp, pts_p, C.c_int, C.c_double, C.c_double, C.POINTER(vp)]),
     "madicp_debug_range_mask": (C.c_int64, [pts_p, bp]),
+    "madicp_ingest_points_ex": (C.c_int, [vp, pts_p, vc_p, C.c_int, dp, dp, C.c_double, C.c_int, C.POINTER(C.c_int64), dp]),
+    "madicp_stage_points_ex": (C.c_int, [vp, pts_p, vc_p, C.c_int64]),
+    "madtree_gpu_build_batch_points_ex": (C.c_int, [vp, pts_p, vc_p, C.c_int, C.c_double, C.c_double, C.POINTER(vp)]),
+    "madicp_debug_correct_points": (C.c_int64, [pts_p, vc_p, dp]),
     "madicp_register_fetch_weight": (C.c_int, [vp, dp, dp, dp, bp, C.POINTER(C.c_int), dp]),
     "madicp_register_partial_async": (C.c_int, [vp, C.c_int, dp]),
     "madicp_calibrate": (C.c_int, [vp, dp]),

@@ -99,8 +99,9 @@ class Lookahead {
     std::vector<float> f32;
     const void* ext = nullptr;        // ... or the caller's buffer, kept alive by `keepalive` until its tree is built
     bool is_f32 = false;
-    bool records = false;             // raw sensor records (Pipeline::prefetchRecords): `pts` describes them
-    madicp_points_t pts{};
+    bool records = false;             // raw sensor records (Pipeline::prefetchRecords): `pts` describes them, `vc` is
+    madicp_points_t pts{};            // their vertical correction (disabled: none)
+    madicp_vcorr_t vc{};
     std::shared_ptr<void> keepalive;
     size_t n = 0;
     madtree_gpu_t* tree = nullptr;
@@ -129,7 +130,8 @@ class Lookahead {
   }
 
  private:
-  // scans that can share one batch call: packed clouds of one element type, or records
+  // scans that can share one batch call: packed clouds of one element type, or records (each with its own correction:
+  // the batch call takes one per scan)
   static bool sameKind(const Job& a, const Job& b) { return a.records == b.records && (a.records || a.is_f32 == b.is_f32); }
   // Builds the trees of the longest run of queued scans of the front's kind, up to the batch size.  A scan whose tree
   // cannot be built (records the range gate leaves empty) fails the batch call as a whole: the run is then halved until
@@ -147,14 +149,16 @@ class Lookahead {
       std::vector<const void*> ptr;
       std::vector<int64_t> n;
       std::vector<madicp_points_t> pts;
+      std::vector<madicp_vcorr_t> vc;
       for (size_t i = 0; i < k; ++i) {
         ptr.push_back(fifo_[i].data());
         n.push_back(int64_t(fifo_[i].n));
         pts.push_back(fifo_[i].pts);
+        vc.push_back(fifo_[i].vc);
       }
       out.assign(k, nullptr);
       const int rc = front.records
-                         ? madtree_gpu_build_batch_points(ctx_, pts.data(), int(k), b_max_, b_min_, out.data())
+                         ? madtree_gpu_build_batch_points_ex(ctx_, pts.data(), vc.data(), int(k), b_max_, b_min_, out.data())
                          : madtree_gpu_build_batch(ctx_, ptr.data(), n.data(), front.is_f32 ? 1 : 0, int(k), b_max_, b_min_,
                                                    out.data());
       if (rc >= 0) break;
@@ -187,7 +191,7 @@ class Lookahead {
       const Job& j = fifo_[built_ + staged_];
       if (!sameKind(j, fifo_[built_])) break;
       if (j.records)
-        check(madicp_stage_points(ctx_, &j.pts, int64_t(batch_) * int64_t(j.n)), "madicp_stage_points");
+        check(madicp_stage_points_ex(ctx_, &j.pts, &j.vc, int64_t(batch_) * int64_t(j.n)), "madicp_stage_points");
       else
         check(madicp_stage_cloud(ctx_, j.data(), int64_t(j.n), j.is_f32 ? 1 : 0, int64_t(batch_) * int64_t(j.n)),
               "madicp_stage_cloud");
@@ -284,15 +288,18 @@ class Pipeline {
     computeRaw(stamp, xyz, n, true);
   }
   // Raw sensor records with the dataset readers' range gate (include/madicp_b200.h, madicp_points_t), read in place:
-  // the same result as compute() on the reader's filtered array.  MADICP_GPU_BUILD=0: the kept points are packed on
-  // the host with the same predicate, then the host path runs.
-  void computeRecords(double stamp, const madicp_points_t& pts) {
+  // the same result as compute() on the reader's filtered array -- corrected by `vc` (nullable: none) like KITTI's
+  // reader with apply_correction.  MADICP_GPU_BUILD=0: the kept points are packed (and corrected) on the host with the
+  // same restatement, then the host path runs.
+  void computeRecords(double stamp, const madicp_points_t& pts, const madicp_vcorr_t* vc = nullptr) {
+    check(madicp::check_vcorr(vc, "Pipeline.computeRecords"), "Pipeline.computeRecords");
     if (!gpu_build_) {
-      compute(stamp, packRecords(pts));
+      compute(stamp, packRecords(pts, vc));
       return;
     }
     if (!pts.data || pts.n <= 0) throw Error("Pipeline.computeRecords: empty scan");
-    computeRaw(stamp, pts.data, size_t(pts.n), pts.is_f32 != 0, &pts);
+    const madicp_vcorr_t v = madicp::vcorr_of(vc);
+    computeRaw(stamp, pts.data, size_t(pts.n), pts.is_f32 != 0, &pts, &v);
   }
   bool gpuBuild() const { return gpu_build_; }
   int lastIcpIterations() const { return last_iters_; }  // rounds the realtime budget allowed for the last scan
@@ -302,7 +309,7 @@ class Pipeline {
   // keepalive: when given, the buffer is read in place (no copy) and the handle is dropped once compute() has consumed
   // the scan; without it the cloud is copied.
   bool prefetch(const void* xyz, size_t n, bool is_f32, std::shared_ptr<void> keepalive = nullptr,
-                const madicp_points_t* records = nullptr) {
+                const madicp_points_t* records = nullptr, const madicp_vcorr_t* vc = nullptr) {
     if (!gpu_build_ || deskew_ || !xyz || n == 0) return false;
     const auto p0 = clk();
     struct Tick {  // (the hand-over runs on the thread that launches the registrations: its cost is part of the scan's)
@@ -322,8 +329,10 @@ class Pipeline {
       if (!keepalive) throw Error("Pipeline.prefetchRecords: the records must be kept alive");
       // a descriptor the library would reject must not enter the queue (every later batch would fail on it)
       check(madicp::check_points(records, "Pipeline.prefetchRecords"), "Pipeline.prefetchRecords");
+      check(madicp::check_vcorr(vc, "Pipeline.prefetchRecords"), "Pipeline.prefetchRecords");
       j.records = true;
       j.pts = *records;
+      j.vc = madicp::vcorr_of(vc);
     }
     if (keepalive) {
       j.ext = xyz;
@@ -336,22 +345,23 @@ class Pipeline {
     lookahead_->push(std::move(j));
     return true;
   }
-  bool prefetchRecords(const madicp_points_t& pts, std::shared_ptr<void> keepalive) {
-    return prefetch(pts.data, pts.n > 0 ? size_t(pts.n) : 0, pts.is_f32 != 0, std::move(keepalive), &pts);
+  bool prefetchRecords(const madicp_points_t& pts, std::shared_ptr<void> keepalive, const madicp_vcorr_t* vc = nullptr) {
+    return prefetch(pts.data, pts.n > 0 ? size_t(pts.n) : 0, pts.is_f32 != 0, std::move(keepalive), &pts, vc);
   }
   size_t prefetched() { return lookahead_ ? lookahead_->size() : 0; }
 
  private:
   // the scan's MAD-tree: ingest (+ deskew, pipeline.cpp:137-138) and build, on the device or on the host
-  std::unique_ptr<MADtree> makeTree(const void* xyz, size_t n, bool is_f32, const madicp_points_t* records) {
+  std::unique_ptr<MADtree> makeTree(const void* xyz, size_t n, bool is_f32, const madicp_points_t* records,
+                                    const madicp_vcorr_t* vc) {
     if (lookahead_ && !lookahead_->empty())  // built ahead of time by a worker lane
       return std::unique_ptr<MADtree>(new MADtree(icp_.context(), lookahead_->pop(), b_max_));
     const bool dsk = deskew_ && is_initialized_ && trajectory_.size() > 1;
     const double* Ta = dsk ? trajectory_[trajectory_.size() - 2].m : nullptr;
     const double* Tb = dsk ? trajectory_[trajectory_.size() - 1].m : nullptr;
     if (gpu_build_ && records) {
-      check(madicp_ingest_points(icp_.context(), records, dsk ? 1 : 0, Ta, Tb, sensor_hz_, std::max(1 << max_parallel_levels_, 1),
-                                 nullptr, nullptr), "madicp_ingest_points");
+      check(madicp_ingest_points_ex(icp_.context(), records, vc, dsk ? 1 : 0, Ta, Tb, sensor_hz_,
+                                    std::max(1 << max_parallel_levels_, 1), nullptr, nullptr), "madicp_ingest_points");
       return std::unique_ptr<MADtree>(new MADtree(icp_.context(), b_max_, b_min_));
     }
     if (gpu_build_) {
@@ -369,7 +379,8 @@ class Pipeline {
     return std::unique_ptr<MADtree>(new MADtree(pts, n, b_max_, b_min_, max_parallel_levels_));
   }
 
-  void computeRaw(double stamp, const void* xyz, size_t n, bool is_f32, const madicp_points_t* records = nullptr) {
+  void computeRaw(double stamp, const void* xyz, size_t n, bool is_f32, const madicp_points_t* records = nullptr,
+                  const madicp_vcorr_t* vc = nullptr) {
     if (!xyz || n == 0) throw Error("Pipeline.compute: empty cloud");
     is_map_updated_ = false;
     if (!is_initialized_) {  // pipeline.cpp:267-284
@@ -377,7 +388,7 @@ class Pipeline {
       f->frame = int(seq_);
       f->to_map = frame_to_map_;
       f->stamp = stamp;
-      f->tree = makeTree(xyz, n, is_f32, records);
+      f->tree = makeTree(xyz, n, is_f32, records, vc);
       keyframes_.push_back(f);
       current_ = f;
       trajectory_.push_back(detail::poseIdentity());
@@ -388,7 +399,7 @@ class Pipeline {
     const auto c0 = clk();
     const auto c1 = c0;
     auto cur = std::make_shared<FrameB>();
-    cur->tree = makeTree(xyz, n, is_f32, records);
+    cur->tree = makeTree(xyz, n, is_f32, records, vc);
     const auto c2 = clk();
     double t[3], w[3];
     for (int a = 0; a < 3; ++a) {
@@ -474,22 +485,26 @@ class Pipeline {
     check(madicp_deskew(cloud[0].data(), int64_t(cloud.size()), T_prev.m, T_now.m, sensor_hz, num_threads), "madicp_deskew");
   }
 
-  // the kept points of `pts` as a packed float64 cloud, with the predicate the device applies (records.hpp)
-  static ContainerType packRecords(const madicp_points_t& pts) {
+  // the kept points of `pts` as a packed float64 cloud, corrected by `vc` (nullable), with the predicate and the
+  // restatement the device applies (records.hpp)
+  static ContainerType packRecords(const madicp_points_t& pts, const madicp_vcorr_t* vc) {
     check(madicp::check_points(&pts, "Pipeline.computeRecords"), "Pipeline.computeRecords");
+    madicp::VcorrTable table;
+    const bool corrected = madicp::vcorr_of(vc).enabled != 0;
+    if (corrected) madicp::vcorr_table_fill(vc->angle, &table);
     ContainerType cloud;
     cloud.reserve(size_t(pts.n));
+    bool bad = false;
     auto pack = [&](auto zero) {
-      using T = decltype(zero);
-      const madicp::RecReader<T> rd(pts);
+      const madicp::RecReader<decltype(zero)> rd(pts, corrected ? &table : nullptr);
       for (int64_t i = 0; i < pts.n; ++i) {
-        T x, y, z;
-        rd.xyz(i, x, y, z);
-        if (rd.keep(x, y, z)) cloud.push_back({double(x), double(y), double(z)});
+        Vector3d p;
+        if (rd.kept_point(i, p[0], p[1], p[2], bad)) cloud.push_back(p);
       }
     };
     if (pts.is_f32) pack(0.0f);
     else pack(0.0);
+    if (bad) throw Error("Pipeline.computeRecords: a point's rotation angle lies outside the table of the vertical correction");
     if (cloud.empty()) throw Error("Pipeline.computeRecords: no point inside the range gate");
     return cloud;
   }

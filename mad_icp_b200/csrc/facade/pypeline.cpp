@@ -24,8 +24,18 @@ static madicp_points_t records_arg(const py::object& records, double min_range, 
   return d;
 }
 
+// apply_correction / vertical_angle_offset (KittiReader's names) -> madicp_vcorr_t
+static madicp_vcorr_t vcorr_arg(bool apply_correction, double vertical_angle_offset) {
+  madicp_vcorr_t v{};
+  v.angle = vertical_angle_offset;
+  v.enabled = apply_correction ? 1 : 0;
+  return v;
+}
+
 PYBIND11_MODULE(pypeline, m) {
   bind_vector_eigen3d(m);
+  // KittiReader.vertical_angle_offset, np.radians(0.205), as records.py computes it: the default bit for bit
+  const double kVerticalAngle = py::module_::import("mad_icp_b200.records").attr("VERTICAL_ANGLE_OFFSET").cast<double>();
   py::class_<mb::Pipeline>(m, "Pipeline")
       .def(py::init<double, bool, double, double, double, double, double, int, int, bool>(), py::arg("sensor_hz"),
            py::arg("deskew"), py::arg("b_max"), py::arg("rho_ker"), py::arg("p_th"), py::arg("b_min"), py::arg("b_ratio"),
@@ -85,19 +95,24 @@ PYBIND11_MODULE(pypeline, m) {
         return p.prefetch(a.data(), size_t(a.shape(0)), false, hold(a));
       }, py::arg("cloud"))
       // additions (not in the reference): raw sensor records, filtered on the way in like the dataset readers do
-      // (mad_icp_b200/records.py describes the array; it is read in place)
+      // (mad_icp_b200/records.py describes the array; it is read in place); apply_correction: KITTI's vertical-angle
+      // correction of the kept points, as KittiReader applies it
       .def("computeRecords", [](mb::Pipeline& p, double stamp, const py::object& records, double min_range, double max_range,
-                                bool inclusive, bool drop_nan) {
-        p.computeRecords(stamp, records_arg(records, min_range, max_range, inclusive, drop_nan));
+                                bool inclusive, bool drop_nan, bool apply_correction, double vertical_angle_offset) {
+        const madicp_vcorr_t v = vcorr_arg(apply_correction, vertical_angle_offset);
+        p.computeRecords(stamp, records_arg(records, min_range, max_range, inclusive, drop_nan), &v);
       }, py::arg("stamp"), py::arg("records"), py::arg("min_range") = 0.0,
-         py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false)
+         py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false,
+         py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle)
       .def("prefetchRecords", [](mb::Pipeline& p, const py::object& records, double min_range, double max_range,
-                                 bool inclusive, bool drop_nan) {
+                                 bool inclusive, bool drop_nan, bool apply_correction, double vertical_angle_offset) {
         const madicp_points_t d = records_arg(records, min_range, max_range, inclusive, drop_nan);
+        const madicp_vcorr_t v = vcorr_arg(apply_correction, vertical_angle_offset);
         py::object* ref = new py::object(records);  // dropped once the scan's tree is built (see prefetch)
-        return p.prefetchRecords(d, std::shared_ptr<void>(ref, [](void* q) { delete static_cast<py::object*>(q); }));
+        return p.prefetchRecords(d, std::shared_ptr<void>(ref, [](void* q) { delete static_cast<py::object*>(q); }), &v);
       }, py::arg("records"), py::arg("min_range") = 0.0,
-         py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false)
+         py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false,
+         py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle)
       .def("prefetched", &mb::Pipeline::prefetched)
       .def("lastIcpIterations", &mb::Pipeline::lastIcpIterations)
       .def("gpuBuild", &mb::Pipeline::gpuBuild)

@@ -33,8 +33,9 @@ using namespace madicp::gtb;
 
 // ingest.cpp (host half of the ingest, host libm service, a parallel-for on the library's host pool)
 void madicp_host_for(int n, int num_threads, const std::function<void(int)>& fn);
-int madicp_deskew_plan(const madicp_points_t& pts, const double T_prev[12], const double T_now[12], double sensor_hz,
-                       int num_threads, int32_t* perm, uint16_t* chunk, double* poses, int* n_poses, int64_t* n_kept);
+int madicp_deskew_plan(const madicp_points_t& pts, const VcorrTable* vc, const double T_prev[12], const double T_now[12],
+                       double sensor_hz, int num_threads, int32_t* perm, uint16_t* chunk, double* poses, int* n_poses,
+                       int64_t* n_kept);
 void madicp_host_trig(const double* args, double* res, int n, int num_threads);
 void madicp_host_hot(int on);
 
@@ -80,6 +81,13 @@ struct BuildState {
   size_t raw_cap = 0;
   int* h_kept = nullptr;  // mapped: kept points of every scan, counted by the device's compaction (k_compact)
   int kept_check = 0;     // scans of the resident cloud whose h_kept the next build compares with the host's count
+  // vertical correction (vertical_correction.h): one table per distinct angle, kept while the lane lives.  The host
+  // copy of slot k is written once, before its upload is queued, and never again until every upload has run.
+  VcorrTable* d_vtab = nullptr;
+  VcorrTable* h_vtab = nullptr;        // pinned
+  std::vector<double> vtab_angle;      // angle of slot k
+  int* h_vc_err = nullptr;             // mapped: a corrected point's rotation angle fell outside its table
+  bool vc_check = false;               // the resident cloud was corrected: the next build checks h_vc_err
   int* d_perm = nullptr;
   unsigned short* d_chunk = nullptr;
   double* d_poses = nullptr;
@@ -96,6 +104,7 @@ struct BuildState {
   // (packed float64) or d_raw (anything else, each scan on a 16-byte boundary), back to back
   struct Staged {
     madicp_points_t d;
+    madicp_vcorr_t vc;
     std::shared_future<RootSums> root;  // the root's sums and the kept count, on a host thread since the scan was staged
   };
   std::vector<Staged> staged;
@@ -220,6 +229,9 @@ int ensure_state(void** slot, cudaStream_t stream, size_t n, size_t raw_bytes, B
     bs->d_raw = raw;
   }
   if (!rc) rc = host_alloc(bs, &bs->h_kept, size_t(kMaxBatch));
+  if (!rc) rc = dev_alloc(bs, &bs->d_vtab, size_t(kMaxBatch));
+  if (!rc) rc = host_alloc(bs, &bs->h_vtab, size_t(kMaxBatch));
+  if (!rc) rc = host_alloc(bs, &bs->h_vc_err, 1);
   if (!rc) rc = dev_alloc(bs, &bs->d_perm, cap);
   if (!rc) rc = dev_alloc(bs, &bs->d_chunk, cap);
   if (!rc) rc = dev_alloc(bs, &bs->d_poses, size_t(65536) * 12);
@@ -282,6 +294,9 @@ int mark_idle(BuildState* bs, cudaStream_t st) {
 // device one per ~10 ns), and the host has the cloud in hand while it is being copied up.  The same pass applies the
 // scan's range gate (records.hpp): the sums run over the kept points in record order, and their count is the offset
 // of the next scan in a forest.
+// A corrected scan (madicp_vcorr_t) is not summed here: its points are the device's corrected ones, and the host would
+// have to restate the correction per point (several ms per 100k points, on the critical path without look-ahead) --
+// the device computes the roots of a batch holding a corrected scan, and the host only counts (kept_count_host).
 template <class T, bool kPacked>
 int64_t root_sums_host(const madicp_points_t& d, double* S) {
   const RecReader<T> rd(d);
@@ -310,6 +325,39 @@ int64_t root_sums_host(const madicp_points_t& d, double* S) {
   const bool packed = !points_gated(d) && d.stride == 3 * e && d.offset[0] == 0 && d.offset[1] == e && d.offset[2] == 2 * e;
   if (d.is_f32) return packed ? root_sums_host<float, true>(d, S) : root_sums_host<float, false>(d, S);
   return packed ? root_sums_host<double, true>(d, S) : root_sums_host<double, false>(d, S);
+}
+// the number of records the scan's range gate keeps (the same predicate), without the sums
+int64_t kept_count_host(const madicp_points_t& d) {
+  if (!points_gated(d)) return d.n;
+  int64_t kept = 0;
+  auto run = [&](auto zero) {
+    using T = decltype(zero);
+    const RecReader<T> rd(d);
+    for (int64_t i = 0; i < d.n; ++i) {
+      T x, y, z;
+      rd.xyz(i, x, y, z);
+      kept += rd.keep(x, y, z) ? 1 : 0;
+    }
+  };
+  if (d.is_f32) run(0.0f);
+  else run(0.0);
+  return kept;
+}
+// the root's sums and the kept count of a scan (root_sums_host), or the count alone for a corrected scan
+int64_t root_host(const madicp_points_t& d, const madicp_vcorr_t& vc, double* S) {
+  return vc.enabled ? kept_count_host(d) : root_sums_host(d, S);
+}
+// the host's table of an enabled correction, or nullptr
+const VcorrTable* vcorr_table(const madicp_vcorr_t& v, VcorrTable* t) {
+  if (!v.enabled) return nullptr;
+  vcorr_table_fill(v.angle, t);
+  return t;
+}
+std::string vcorr_out_of_table(const char* fn, double angle) {
+  char buf[64];
+  snprintf(buf, sizeof(buf), "%.17g", angle);
+  return std::string(fn) + ": a point's rotation angle lies outside the table of the vertical correction (angle " + buf +
+         "): its sin / cos cannot be reproduced exactly";
 }
 
 // A few resident host threads for work that is handed over and collected later (the roots' sums of staged clouds).
@@ -456,6 +504,10 @@ int build_forest(madicp_ctx* c, BuildState* bs, cudaStream_t st, int n_trees, co
     CK(cudaStreamSynchronize(st));  // the level's one host round trip: libm for the eigen-decomposition
     const auto ts1 = now();
     t_sync += us(ts0, ts1);
+    if (depth == 0 && bs->vc_check && *bs->h_vc_err) {
+      set_error("madtree_gpu_build: a point's rotation angle lies outside the table of the vertical correction");
+      return MADICP_ERR_STATE;
+    }
     if (depth == 0)
       for (int b = 0; b < check_kept; ++b)
         if (bs->h_kept[b] != offs[b + 1] - offs[b]) {
@@ -573,13 +625,55 @@ void madicp_gpu_build_release(madicp_ctx* c) {
 namespace {
 
 size_t align16(size_t x) { return (x + 15) & ~size_t(15); }
-// a packed float64 cloud without a gate is copied straight into the point buffer; everything else goes through d_raw
-bool is_direct(const madicp_points_t& d) {
-  return !d.is_f32 && d.stride == 24 && d.offset[0] == 0 && d.offset[1] == 8 && d.offset[2] == 16 && !points_gated(d);
+// a packed float64 cloud without a gate or a correction is copied straight into the point buffer; everything else goes
+// through d_raw
+bool is_direct(const madicp_points_t& d, const madicp_vcorr_t& vc) {
+  return !d.is_f32 && d.stride == 24 && d.offset[0] == 0 && d.offset[1] == 8 && d.offset[2] == 16 && !points_gated(d) &&
+         !vc.enabled;
 }
-// layout of one scan for the device (RecSrc, gpu_tree_kernels.cuh); raw: its byte offset in d_raw, first: its first record
-RecSrc rec_src(const madicp_points_t& d, size_t raw, int first) {
+bool vtab_cached(const BuildState* bs, double angle) {
+  for (double a : bs->vtab_angle)
+    if (std::memcmp(&a, &angle, sizeof(double)) == 0) return true;
+  return false;
+}
+// Room for the tables of the corrections vc[0..count) before a launch assigns its slots: when the angles not cached yet
+// would not fit, the lane waits for `st` (the uploads and the kernels reading the tables) and starts over.
+int vtab_room(BuildState* bs, cudaStream_t st, const madicp_vcorr_t* vc, int count) {
+  size_t fresh = 0;
+  for (int b = 0; b < count; ++b) {
+    if (!vc[b].enabled || vtab_cached(bs, vc[b].angle)) continue;
+    bool seen = false;  // (an angle new to the cache, counted once)
+    for (int e = 0; e < b && !seen; ++e)
+      seen = vc[e].enabled && std::memcmp(&vc[e].angle, &vc[b].angle, sizeof(double)) == 0;
+    fresh += seen ? 0 : 1;
+  }
+  if (bs->vtab_angle.size() + fresh <= size_t(kMaxBatch)) return MADICP_OK;
+  CK(cudaStreamSynchronize(st));
+  bs->vtab_angle.clear();
+  return MADICP_OK;
+}
+// The device table of an enabled correction's angle (bs->d_vtab[*slot]), uploaded on `st` at its first use; *slot = -1
+// without a correction.  Call vtab_room first.
+int vtab_slot(BuildState* bs, cudaStream_t st, const madicp_vcorr_t& vc, int* slot) {
+  *slot = -1;
+  if (!vc.enabled) return MADICP_OK;
+  for (size_t k = 0; k < bs->vtab_angle.size(); ++k)
+    if (std::memcmp(&bs->vtab_angle[k], &vc.angle, sizeof(double)) == 0) {
+      *slot = int(k);
+      return MADICP_OK;
+    }
+  const int k = int(bs->vtab_angle.size());
+  vcorr_table_fill(vc.angle, bs->h_vtab + k);
+  CK(cudaMemcpyAsync(bs->d_vtab + k, bs->h_vtab + k, sizeof(VcorrTable), cudaMemcpyHostToDevice, st));
+  bs->vtab_angle.push_back(vc.angle);
+  *slot = k;
+  return MADICP_OK;
+}
+// layout of one scan for the device (RecSrc, gpu_tree_kernels.cuh); raw: its byte offset in d_raw, first: its first
+// record, vc: its correction's table slot (vtab_slot)
+RecSrc rec_src(const madicp_points_t& d, size_t raw, int first, int vc) {
   RecSrc s{};
+  s.vc = (signed char) vc;
   s.raw = (long long) raw;
   s.first = first;
   s.stride = int(d.stride);
@@ -598,30 +692,36 @@ RecSrc rec_src(const madicp_points_t& d, size_t raw, int first) {
   return s;
 }
 // Order-preserving compaction of the gated records of B (d_raw) into P[0]; the kept count of every scan goes to
-// bs->h_kept.
-int launch_compaction(madicp_ctx* c, BuildState* bs, cudaStream_t st, const RecBatch& B) {
+// bs->h_kept.  vc: some scan of B is corrected.
+int launch_compaction(madicp_ctx* c, BuildState* bs, cudaStream_t st, const RecBatch& B, bool vc) {
   const char* raw = static_cast<const char*>(bs->d_raw);
   const int tiles = (B.n_rec + kTile - 1) / kTile;
   k_gate_flags<<<blocks(B.n_rec), kBlock, 0, st>>>(B, raw, bs->flag);
   k_scan_tiles<<<tiles, kTile, 0, st>>>(bs->flag, B.n_rec, bs->G, bs->tile);
   k_scan_tile_sums<<<1, 1024, 0, st>>>(bs->tile, tiles);
-  k_compact<<<blocks(std::max(B.n_rec, B.count)), kBlock, 0, st>>>(B, raw, bs->flag, bs->G, bs->tile, bs->P[0], bs->h_kept);
+  auto k = vc ? k_compact<true> : k_compact<false>;
+  k<<<blocks(std::max(B.n_rec, B.count)), kBlock, 0, st>>>(B, raw, bs->flag, bs->G, bs->tile, bs->P[0], bs->h_kept, bs->d_vtab,
+                                                           bs->h_vc_err);
   c->launches += 4;
   CK(cudaGetLastError());
   return MADICP_OK;
 }
 
-// The batch build behind madtree_gpu_build_batch and madtree_gpu_build_batch_points (descriptors validated).
-int build_batch(madicp_ctx* c, const madicp_points_t* d, int count, double b_max, double b_min, madtree_gpu** out,
-                const char* fn) {
-  bool direct = true, gated = false;
+// The batch build behind madtree_gpu_build_batch and madtree_gpu_build_batch_points[_ex] (descriptors and corrections
+// validated; vcorrs nullable).
+int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* vcorrs, int count, double b_max, double b_min,
+                madtree_gpu** out, const char* fn) {
+  bool direct = true, gated = false, corrected = false;
+  madicp_vcorr_t vc[kMaxBatch];
   int first[kMaxBatch + 1];
   size_t raw_off[kMaxBatch + 1];
   first[0] = 0;
   raw_off[0] = 0;
   for (int b = 0; b < count; ++b) {
-    direct = direct && is_direct(d[b]);
+    vc[b] = vcorr_of(vcorrs ? vcorrs + b : nullptr);
+    direct = direct && is_direct(d[b], vc[b]);
     gated = gated || points_gated(d[b]);
+    corrected = corrected || vc[b].enabled;
     if (int64_t(first[b]) + d[b].n > (int64_t(1) << 26)) {
       set_error(std::string(fn) + ": more than 2^26 points in the batch");
       return MADICP_ERR_INVALID;
@@ -644,7 +744,7 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, int count, double b_max
   // scans uploaded ahead of time (madicp_stage_cloud / _points): the longest prefix of this batch staged in this order
   int n_staged = 0;
   if (!bs->staged.empty() && bs->staged_raw == !direct)
-    while (n_staged < count && n_staged < int(bs->staged.size()) && same_points(bs->staged[size_t(n_staged)].d, d[n_staged]))
+    while (n_staged < count && n_staged < int(bs->staged.size()) && same_points(bs->staged[size_t(n_staged)].d, bs->staged[size_t(n_staged)].vc, d[n_staged], vc[n_staged]))
       ++n_staged;
   std::vector<std::shared_future<RootSums>> early;
   for (int b = 0; b < n_staged; ++b) early.push_back(bs->staged[size_t(b)].root);
@@ -658,25 +758,34 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, int count, double b_max
   bs->n_resident = 0;  // the concatenated clouds are not "the resident cloud" of madtree_gpu_build_resident
   bs->has_root_S = false;
   bs->kept_check = 0;
+  bs->vc_check = corrected;
   if (!direct) {
     RecBatch B;
     B.count = count;
     B.n_rec = n_rec;
-    for (int b = 0; b < count; ++b) B.s[b] = rec_src(d[b], raw_off[b], first[b]);
+    if (corrected) CK(cudaMemsetAsync(bs->h_vc_err, 0, sizeof(int), st));
+    if (int e = vtab_room(bs, st, vc, count)) return e;
+    for (int b = 0; b < count; ++b) {
+      int slot = -1;
+      if (int e = vtab_slot(bs, st, vc[b], &slot)) return e;
+      B.s[b] = rec_src(d[b], raw_off[b], first[b], slot);
+    }
     if (gated) {
-      if (int e = launch_compaction(c, bs, st, B)) return e;
+      if (int e = launch_compaction(c, bs, st, B, corrected)) return e;
     } else {
-      k_ingest<<<blocks(n_rec), kBlock, 0, st>>>(B, raw, nullptr, nullptr, bs->d_poses, n_rec, bs->P[0]);
+      auto k = corrected ? k_ingest<true> : k_ingest<false>;
+      k<<<blocks(n_rec), kBlock, 0, st>>>(B, raw, nullptr, nullptr, bs->d_poses, n_rec, bs->P[0], bs->d_vtab, bs->h_vc_err);
       c->launches++;
     }
   }
   const auto ta1 = std::chrono::steady_clock::now();
-  // the roots' sums and the kept counts on the host, one scan per host thread, while the scans are being copied up
+  // the roots' sums and the kept counts on the host, one scan per host thread, while the scans are being copied up; a
+  // batch holding a corrected scan has its roots summed on the device (root_host)
   std::vector<double> S(size_t(count) * 9);
   std::vector<int64_t> kept(static_cast<size_t>(count));
   if (count > n_staged) madicp_host_for(count - n_staged, bs->threads, [&](int k) {
     const int b = n_staged + k;
-    kept[size_t(b)] = root_sums_host(d[b], S.data() + size_t(b) * 9);
+    kept[size_t(b)] = root_host(d[b], vc[b], S.data() + size_t(b) * 9);
   });
   for (int b = 0; b < n_staged; ++b) {
     const RootSums& r = early[size_t(b)].get();
@@ -693,7 +802,7 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, int count, double b_max
     offs[b + 1] = offs[b] + int(kept[size_t(b)]);
   }
   const auto tb0 = std::chrono::steady_clock::now();
-  rc = build_forest(c, bs, st, count, offs, b_max, b_min, S.data(), gated ? count : 0, out);
+  rc = build_forest(c, bs, st, count, offs, b_max, b_min, corrected ? nullptr : S.data(), gated ? count : 0, out);
   if (getenv("MADICP_BUILD_TIMING"))
     fprintf(stderr, "%s: %d scans (%d staged), copies enqueued %.0f us, roots' sums on the host %.0f us, forest build %.0f us\n",
             fn, count, n_staged, std::chrono::duration<double, std::micro>(ta1 - ta0).count(),
@@ -702,12 +811,12 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, int count, double b_max
   return rc;
 }
 
-// The early upload behind madicp_stage_cloud and madicp_stage_points (descriptor validated).
-int stage(madicp_ctx* c, const madicp_points_t& d, int64_t reserve_points) {
+// The early upload behind madicp_stage_cloud and madicp_stage_points[_ex] (descriptor and correction validated).
+int stage(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int64_t reserve_points) {
   CK(cudaSetDevice(c->device));
   BuildState* bs = static_cast<BuildState*>(c->build_state);
   if (bs && bs->stage_closed) return MADICP_OK;
-  const bool raw = !is_direct(d);
+  const bool raw = !is_direct(d, vc);
   const size_t bytes = size_t(d.n) * size_t(d.stride);
   if (!bs || bs->staged.empty()) {
     const int64_t res = std::max(reserve_points, d.n);
@@ -722,6 +831,7 @@ int stage(madicp_ctx* c, const madicp_points_t& d, int64_t reserve_points) {
     bs->n_resident = 0;  // the cloud madicp_ingest left is about to be overwritten
     bs->has_root_S = false;
     bs->kept_check = 0;
+    bs->vc_check = false;
   }
   const size_t at = align16(bs->staged_bytes);
   if (bs->staged_raw != raw || size_t(bs->staged_points + d.n) > bs->cap || (raw && at + bytes > bs->raw_cap) ||
@@ -731,21 +841,21 @@ int stage(madicp_ctx* c, const madicp_points_t& d, int64_t reserve_points) {
   }
   if (raw) CK(cudaMemcpyAsync(static_cast<char*>(bs->d_raw) + at, d.data, points_bytes(d), cudaMemcpyHostToDevice, bs->copy_stream));
   else CK(cudaMemcpyAsync(bs->P[0] + size_t(bs->staged_points) * 3, d.data, bytes, cudaMemcpyHostToDevice, bs->copy_stream));
-  // the root's sums (root_sums_host) start now too, on a background thread: the caller is about to wait for the device
-  auto sums = background().submit([d]() {
+  // the root's sums (root_host) start now too, on a background thread: the caller is about to wait for the device
+  auto sums = background().submit([d, vc]() {
     RootSums r;
-    r.kept = root_sums_host(d, r.S.data());
+    r.kept = root_host(d, vc, r.S.data());
     return r;
   });
-  bs->staged.push_back({d, std::move(sums)});
+  bs->staged.push_back({d, vc, std::move(sums)});
   bs->staged_points += d.n;
   if (raw) bs->staged_bytes = at + bytes;
   return MADICP_OK;
 }
 
-// The ingest behind madicp_ingest and madicp_ingest_points (descriptor validated).
-int ingest(madicp_ctx* c, const madicp_points_t& d, int deskew, const double T_prev[12], const double T_now[12],
-           double sensor_hz, int num_threads, int64_t* n_kept, double* points_out, const char* fn) {
+// The ingest behind madicp_ingest and madicp_ingest_points[_ex] (descriptor and correction validated).
+int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int deskew, const double T_prev[12],
+           const double T_now[12], double sensor_hz, int num_threads, int64_t* n_kept, double* points_out, const char* fn) {
   CK(cudaSetDevice(c->device));
   BuildState* bs = nullptr;
   const int64_t n = d.n;
@@ -756,34 +866,45 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, int deskew, const double T_p
   cudaStream_t st = c->stream;
   bs->n_resident = 0;
   bs->kept_check = 0;
+  bs->vc_check = vc.enabled != 0;
   // the raw scan goes up while the host works out the order (deskew) or the root's sums
   CK(cudaMemcpyAsync(bs->d_raw, d.data, points_bytes(d), cudaMemcpyHostToDevice, st));
   const char* raw = static_cast<const char*>(bs->d_raw);
+  int slot = -1;
+  if (vc.enabled) CK(cudaMemsetAsync(bs->h_vc_err, 0, sizeof(int), st));
+  if (int e = vtab_room(bs, st, &vc, 1)) return e;
+  if (int e = vtab_slot(bs, st, vc, &slot)) return e;
   RecBatch B;
   B.count = 1;
   B.n_rec = int(n);
-  B.s[0] = rec_src(d, 0, 0);
+  B.s[0] = rec_src(d, 0, 0, slot);
   int64_t kept = n;
   if (deskew) {
     CK(cudaStreamSynchronize(st));  // h_perm / h_chunk / h_poses of the previous scan have been consumed
     int n_poses = 0;
-    rc = madicp_deskew_plan(d, T_prev, T_now, sensor_hz, num_threads, bs->h_perm, bs->h_chunk, bs->h_poses, &n_poses, &kept);
+    VcorrTable table;  // (the azimuths are those of the corrected points)
+    rc = madicp_deskew_plan(d, vcorr_table(vc, &table), T_prev, T_now, sensor_hz, num_threads, bs->h_perm, bs->h_chunk, bs->h_poses, &n_poses,
+                            &kept);
+    if (rc == MADICP_ERR_STATE) set_error(vcorr_out_of_table(fn, vc.angle));
     if (rc) return rc;
     if (kept > 0) {
       CK(cudaMemcpyAsync(bs->d_perm, bs->h_perm, size_t(kept) * sizeof(int), cudaMemcpyHostToDevice, st));
       CK(cudaMemcpyAsync(bs->d_chunk, bs->h_chunk, size_t(kept) * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
       CK(cudaMemcpyAsync(bs->d_poses, bs->h_poses, size_t(n_poses) * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
-      k_ingest<<<blocks(kept), kBlock, 0, st>>>(B, raw, bs->d_perm, bs->d_chunk, bs->d_poses, int(kept), bs->P[0]);
+      auto k = vc.enabled ? k_ingest<true> : k_ingest<false>;
+      k<<<blocks(kept), kBlock, 0, st>>>(B, raw, bs->d_perm, bs->d_chunk, bs->d_poses, int(kept), bs->P[0], bs->d_vtab,
+                                         bs->h_vc_err);
       c->launches++;
     }
   } else if (points_gated(d)) {
-    if (int e = launch_compaction(c, bs, st, B)) return e;
-    kept = root_sums_host(d, bs->root_S);
+    if (int e = launch_compaction(c, bs, st, B, vc.enabled)) return e;
+    kept = root_host(d, vc, bs->root_S);
     bs->kept_check = 1;
   } else {
-    k_ingest<<<blocks(n), kBlock, 0, st>>>(B, raw, nullptr, nullptr, bs->d_poses, int(n), bs->P[0]);
+    auto k = vc.enabled ? k_ingest<true> : k_ingest<false>;
+    k<<<blocks(n), kBlock, 0, st>>>(B, raw, nullptr, nullptr, bs->d_poses, int(n), bs->P[0], bs->d_vtab, bs->h_vc_err);
     c->launches++;
-    root_sums_host(d, bs->root_S);
+    kept = root_host(d, vc, bs->root_S);
   }
   CK(cudaGetLastError());
   if (kept == 0) {
@@ -792,11 +913,17 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, int deskew, const double T_p
     return MADICP_ERR_INVALID;
   }
   bs->n_resident = kept;
-  bs->has_root_S = !deskew;  // (a deskewed cloud exists on the device only: its root sums run there)
+  bs->has_root_S = !deskew && !vc.enabled;  // (a deskewed or corrected cloud exists on the device only: its root sums run
+                                            // there)
   if (n_kept) *n_kept = kept;
   if (points_out) {
     CK(cudaMemcpyAsync(points_out, bs->P[0], size_t(kept) * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
+    if (bs->vc_check && *bs->h_vc_err) {
+      set_error(vcorr_out_of_table(fn, vc.angle));
+      bs->n_resident = 0;
+      return MADICP_ERR_STATE;
+    }
     if (bs->kept_check && bs->h_kept[0] != kept) {
       set_error(std::string(fn) + ": the device kept " + std::to_string(bs->h_kept[0]) + " points, the host " +
                 std::to_string(kept));
@@ -827,21 +954,35 @@ int madtree_gpu_build_batch(madicp_ctx_t* c, const void* const* clouds, const in
     }
     d[b] = packed_points(clouds[b], n_points[b], is_f32);
   }
-  return build_batch(c, d, count, b_max, b_min, out, "madtree_gpu_build_batch");
+  return build_batch(c, d, nullptr, count, b_max, b_min, out, "madtree_gpu_build_batch");
   MADICP_CATCH("madtree_gpu_build_batch")
 }
 
-int madtree_gpu_build_batch_points(madicp_ctx_t* c, const madicp_points_t* descs, int count, double b_max, double b_min,
-                                   madtree_gpu_t** out) {
+namespace {
+int build_batch_points(madicp_ctx_t* c, const madicp_points_t* descs, const madicp_vcorr_t* vcorrs, int count, double b_max,
+                       double b_min, madtree_gpu_t** out, const char* fn) {
   if (!c || !descs || !out || count < 1 || count > kMaxBatch) {
-    set_error("madtree_gpu_build_batch_points: bad arguments (1..64 scans)");
+    set_error(std::string(fn) + ": bad arguments (1..64 scans)");
     return MADICP_ERR_INVALID;
   }
-  for (int b = 0; b < count; ++b)
-    if (int e = check_points(descs + b, "madtree_gpu_build_batch_points")) return e;
+  for (int b = 0; b < count; ++b) {
+    if (int e = check_points(descs + b, fn)) return e;
+    if (int e = check_vcorr(vcorrs ? vcorrs + b : nullptr, fn)) return e;
+  }
   MADICP_TRY
-  return build_batch(c, descs, count, b_max, b_min, out, "madtree_gpu_build_batch_points");
-  MADICP_CATCH("madtree_gpu_build_batch_points")
+  return build_batch(c, descs, vcorrs, count, b_max, b_min, out, fn);
+  MADICP_CATCH(fn)
+}
+}  // namespace
+
+int madtree_gpu_build_batch_points(madicp_ctx_t* c, const madicp_points_t* descs, int count, double b_max, double b_min,
+                                   madtree_gpu_t** out) {
+  return build_batch_points(c, descs, nullptr, count, b_max, b_min, out, "madtree_gpu_build_batch_points");
+}
+
+int madtree_gpu_build_batch_points_ex(madicp_ctx_t* c, const madicp_points_t* descs, const madicp_vcorr_t* vcorrs, int count,
+                                      double b_max, double b_min, madtree_gpu_t** out) {
+  return build_batch_points(c, descs, vcorrs, count, b_max, b_min, out, "madtree_gpu_build_batch_points");
 }
 
 int madicp_stage_cloud(madicp_ctx_t* c, const void* cloud, int64_t n, int is_f32, int64_t reserve_points) {
@@ -850,19 +991,24 @@ int madicp_stage_cloud(madicp_ctx_t* c, const void* cloud, int64_t n, int is_f32
     return MADICP_ERR_INVALID;
   }
   MADICP_TRY
-  return stage(c, packed_points(cloud, n, is_f32), reserve_points);
+  return stage(c, packed_points(cloud, n, is_f32), madicp_vcorr_t{}, reserve_points);
   MADICP_CATCH("madicp_stage_cloud")
 }
 
-int madicp_stage_points(madicp_ctx_t* c, const madicp_points_t* desc, int64_t reserve_points) {
+int madicp_stage_points_ex(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int64_t reserve_points) {
   if (!c || reserve_points > (int64_t(1) << 26)) {
     set_error("madicp_stage_points: bad arguments");
     return MADICP_ERR_INVALID;
   }
   if (int e = check_points(desc, "madicp_stage_points")) return e;
+  if (int e = check_vcorr(vcorr, "madicp_stage_points")) return e;
   MADICP_TRY
-  return stage(c, *desc, reserve_points);
+  return stage(c, *desc, vcorr_of(vcorr), reserve_points);
   MADICP_CATCH("madicp_stage_points")
+}
+
+int madicp_stage_points(madicp_ctx_t* c, const madicp_points_t* desc, int64_t reserve_points) {
+  return madicp_stage_points_ex(c, desc, nullptr, reserve_points);
 }
 
 int madicp_stage_discard(madicp_ctx_t* c) {
@@ -895,6 +1041,7 @@ int madtree_gpu_build(madicp_ctx_t* c, const double* points_xyz, int64_t n, doub
   bs->n_resident = n;
   bs->kept_check = 0;
   root_sums_host(packed_points(points_xyz, n, 0), bs->root_S);
+  bs->vc_check = false;
   bs->has_root_S = true;
   return build_resident(c, bs, c->stream, n, b_max, b_min, bs->root_S, out);
   MADICP_CATCH("madtree_gpu_build")
@@ -945,21 +1092,29 @@ int madicp_ingest(madicp_ctx_t* c, const void* xyz, int64_t n, int is_f32, int d
     return MADICP_ERR_INVALID;
   }
   MADICP_TRY
-  return ingest(c, packed_points(xyz, n, is_f32), deskew, T_prev, T_now, sensor_hz, num_threads, nullptr, points_out,
-                "madicp_ingest");
+  return ingest(c, packed_points(xyz, n, is_f32), madicp_vcorr_t{}, deskew, T_prev, T_now, sensor_hz, num_threads, nullptr,
+                points_out, "madicp_ingest");
   MADICP_CATCH("madicp_ingest")
 }
 
-int madicp_ingest_points(madicp_ctx_t* c, const madicp_points_t* desc, int deskew, const double T_prev[12],
-                         const double T_now[12], double sensor_hz, int num_threads, int64_t* n_kept, double* points_out) {
+int madicp_ingest_points_ex(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int deskew,
+                            const double T_prev[12], const double T_now[12], double sensor_hz, int num_threads,
+                            int64_t* n_kept, double* points_out) {
   if (!c || (deskew && (!T_prev || !T_now || !(sensor_hz > 0.0)))) {
     set_error("madicp_ingest_points: bad arguments");
     return MADICP_ERR_INVALID;
   }
   if (int e = check_points(desc, "madicp_ingest_points")) return e;
+  if (int e = check_vcorr(vcorr, "madicp_ingest_points")) return e;
   MADICP_TRY
-  return ingest(c, *desc, deskew, T_prev, T_now, sensor_hz, num_threads, n_kept, points_out, "madicp_ingest_points");
+  return ingest(c, *desc, vcorr_of(vcorr), deskew, T_prev, T_now, sensor_hz, num_threads, n_kept, points_out,
+                "madicp_ingest_points");
   MADICP_CATCH("madicp_ingest_points")
+}
+
+int madicp_ingest_points(madicp_ctx_t* c, const madicp_points_t* desc, int deskew, const double T_prev[12],
+                         const double T_now[12], double sensor_hz, int num_threads, int64_t* n_kept, double* points_out) {
+  return madicp_ingest_points_ex(c, desc, nullptr, deskew, T_prev, T_now, sensor_hz, num_threads, n_kept, points_out);
 }
 
 int64_t madicp_debug_range_mask(const madicp_points_t* desc, uint8_t* keep) {
@@ -981,6 +1136,31 @@ int64_t madicp_debug_range_mask(const madicp_points_t* desc, uint8_t* keep) {
   };
   if (desc->is_f32) run(0.0f);
   else run(0.0);
+  return kept;
+}
+
+int64_t madicp_debug_correct_points(const madicp_points_t* desc, const madicp_vcorr_t* vcorr, double* out) {
+  if (int e = check_points(desc, "madicp_debug_correct_points")) return e;
+  if (int e = check_vcorr(vcorr, "madicp_debug_correct_points")) return e;
+  if (!out) {
+    set_error("madicp_debug_correct_points: null output");
+    return MADICP_ERR_INVALID;
+  }
+  VcorrTable table;
+  const VcorrTable* vt = vcorr_table(vcorr_of(vcorr), &table);
+  int64_t kept = 0;
+  bool bad = false;
+  auto run = [&](auto zero) {
+    const RecReader<decltype(zero)> rd(*desc, vt);
+    for (int64_t i = 0; i < desc->n; ++i)
+      if (rd.kept_point(i, out[3 * kept], out[3 * kept + 1], out[3 * kept + 2], bad)) ++kept;
+  };
+  if (desc->is_f32) run(0.0f);
+  else run(0.0);
+  if (bad) {
+    set_error(vcorr_out_of_table("madicp_debug_correct_points", vcorr->angle));
+    return MADICP_ERR_STATE;
+  }
   return kept;
 }
 

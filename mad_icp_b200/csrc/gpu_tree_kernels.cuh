@@ -23,6 +23,7 @@
 #include "arith.h"
 #include "eig3.h"
 #include "range_gate.h"
+#include "vertical_correction.h"
 
 namespace madicp {
 namespace gtb {
@@ -855,6 +856,7 @@ struct RecSrc {
   int off[3];          // byte offsets of x, y, z: from `vbase` when vec > 0, from the record start otherwise
   int vbase;           // start of the first 16-byte chunk holding x, y, z
   unsigned char is_f32, vec, mode, drop_nan;  // vec: 128-bit loads per record (0: one load per field)
+  signed char vc;      // the scan's vertical-correction table (an index into the launch's tables), -1: none
   double lo, hi;       // the gate's bounds, already rounded to the field type
 };
 struct RecBatch {
@@ -877,10 +879,10 @@ __device__ __forceinline__ int rec_scan(const RecBatch& B, int r) {  // scan of 
   }
   return lo;
 }
-// record r of the batch -> float64 x, y, z; returns whether the scan's range gate keeps it (range_gate.h)
-__device__ __forceinline__ bool read_record(const RecBatch& B, const char* __restrict__ raw, int r, double& x, double& y,
+// record r of the batch (s: its scan) -> float64 x, y, z as stored; returns whether the scan's range gate keeps it
+// (range_gate.h)
+__device__ __forceinline__ bool read_record(const RecSrc& s, const char* __restrict__ raw, int r, double& x, double& y,
                                             double& z) {
-  const RecSrc& s = B.s[rec_scan(B, r)];
   const char* rec = raw + s.raw + (long long)(r - s.first) * s.stride;
   if (s.is_f32) {
     float fx, fy, fz;
@@ -912,6 +914,13 @@ __device__ __forceinline__ bool read_record(const RecBatch& B, const char* __res
   }
   return range_keep<double>(x, y, z, s.lo, s.hi, s.mode, s.drop_nan);
 }
+// The scan's vertical correction (vertical_correction.h) of a kept point: the reader masks first and corrects the
+// kept points, so the gate above decides on the raw values and the correction applies to the value that is written.
+// A rotation angle outside the table raises *err (mapped host memory, checked at the caller's next host sync).
+__device__ __forceinline__ void correct_record(const RecSrc& s, const VcorrTable* __restrict__ vtab, int* err, double& x,
+                                               double& y, double& z) {
+  if (s.vc >= 0 && !vcorr_apply(vtab[s.vc], x, y, z)) *err = 1;
+}
 
 // Order-preserving compaction of the gated records (no deskew): flags -> the tile scan above (k_scan_tiles +
 // k_scan_tile_sums: G[i] + tile[i >> 10] = kept records before i) -> every kept record converted and written at its
@@ -922,12 +931,15 @@ k_gate_flags(const __grid_constant__ RecBatch B, const char* __restrict__ raw, u
   const int i = blockIdx.x * kBlock + threadIdx.x;
   if (i >= B.n_rec) return;
   double x, y, z;
-  flag[i] = read_record(B, raw, i, x, y, z) ? 1 : 0;
+  flag[i] = read_record(B.s[rec_scan(B, i)], raw, i, x, y, z) ? 1 : 0;
 }
-// kept (mapped host memory): kept points of every scan, for the build to compare with the host's count
+// kept (mapped host memory): kept points of every scan, for the build to compare with the host's count; vtab / vc_err:
+// see correct_record.  kVc: some scan of the batch is corrected (without, the kernel is the uncorrected one exactly)
+template <bool kVc>
 __global__ void __launch_bounds__(kBlock)
 k_compact(const __grid_constant__ RecBatch B, const char* __restrict__ raw, const unsigned char* __restrict__ flag,
-          const int* __restrict__ G, const int* __restrict__ tile_off, double* __restrict__ out, int* __restrict__ kept) {
+          const int* __restrict__ G, const int* __restrict__ tile_off, double* __restrict__ out, int* __restrict__ kept,
+          const VcorrTable* __restrict__ vtab, int* vc_err) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
   const int n = B.n_rec;
   auto rank = [&](int r) {  // kept records before r
@@ -936,7 +948,9 @@ k_compact(const __grid_constant__ RecBatch B, const char* __restrict__ raw, cons
   if (i < B.count) kept[i] = rank(i + 1 < B.count ? B.s[i + 1].first : n) - rank(B.s[i].first);
   if (i >= n || !flag[i]) return;
   double x, y, z;
-  read_record(B, raw, i, x, y, z);
+  const RecSrc& s = B.s[rec_scan(B, i)];
+  read_record(s, raw, i, x, y, z);
+  if (kVc) correct_record(s, vtab, vc_err, x, y, z);
   const size_t o = size_t(rank(i));
   out[3 * o] = x;
   out[3 * o + 1] = y;
@@ -946,15 +960,21 @@ k_compact(const __grid_constant__ RecBatch B, const char* __restrict__ raw, cons
 // Ingest (odometry/pipeline.cpp:79-123 + the float32 -> float64 conversion of the readers): out[i] = T[chunk[i]] *
 // record(perm[i]), with the reference's operand order (Isometry * point = R p + t, dot3 rows) and no FMA.
 // perm == nullptr: identity; chunk == nullptr: no transform (conversion only).  The gate is not applied here: perm
-// holds kept records only (madicp_deskew_plan), and without perm the batch has no gate.
+// holds kept records only (madicp_deskew_plan), and without perm the batch has no gate.  The vertical correction
+// (correct_record) applies to the gathered point, before the chunk's transform, as the reader's cloud is corrected
+// before the pipeline deskews it.  kVc: as in k_compact.
+template <bool kVc>
 __global__ void __launch_bounds__(kBlock)
 k_ingest(const __grid_constant__ RecBatch B, const char* __restrict__ raw, const int* __restrict__ perm,
          const unsigned short* __restrict__ chunk, const double* __restrict__ poses /* n_chunks x 12 */, int n,
-         double* __restrict__ out) {
+         double* __restrict__ out, const VcorrTable* __restrict__ vtab, int* vc_err) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
   if (i >= n) return;
   double x, y, z;
-  read_record(B, raw, perm ? perm[i] : i, x, y, z);
+  const int r = perm ? perm[i] : i;
+  const RecSrc& s = B.s[rec_scan(B, r)];
+  read_record(s, raw, r, x, y, z);
+  if (kVc) correct_record(s, vtab, vc_err, x, y, z);
   if (chunk) {
     const double* X = poses + size_t(chunk[i]) * 12;
     double ox, oy, oz;

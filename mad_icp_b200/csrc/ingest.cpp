@@ -234,11 +234,14 @@ extern "C" int madicp_deskew(double* points_xyz, int64_t n, const double T_prev[
 // the chunk poses (sin/cos inside the exponential map) -- and nothing that touches the points' values: the gather,
 // the float -> double conversion and the rigid transform run on the device.
 // The records are read through their descriptor and the range gate (records.hpp) is applied in the azimuth pass: the
-// sort sees the kept points in record order, exactly the cloud the reader would have handed over.
+// sort sees the kept points in record order, exactly the cloud the reader would have handed over.  With a vertical
+// correction (vc != nullptr, vertical_correction.h) the azimuths are those of the corrected points, as the reader
+// corrects before the pipeline deskews; MADICP_ERR_STATE (no message) when a rotation angle falls outside the table.
 // perm[i] = record index of the kept point at sorted position i; chunk[i] = its pose; poses: (*n_poses) x 12
 // row-major; *n_kept = number of kept points (entries of perm / chunk).
-int madicp_deskew_plan(const madicp_points_t& pts, const double T_prev[12], const double T_now[12], double sensor_hz,
-                       int num_threads, int32_t* perm, uint16_t* chunk, double* poses, int* n_poses, int64_t* n_kept) {
+int madicp_deskew_plan(const madicp_points_t& pts, const madicp::VcorrTable* vc, const double T_prev[12],
+                       const double T_now[12], double sensor_hz, int num_threads, int32_t* perm, uint16_t* chunk,
+                       double* poses, int* n_poses, int64_t* n_kept) {
   const int64_t n_rec = pts.n;
   if (!pts.data || !T_prev || !T_now || n_rec <= 0 || n_rec > (int64_t(1) << 30) || !(sensor_hz > 0.0)) {
     madicp::set_error("madicp_ingest: bad arguments");
@@ -257,24 +260,27 @@ int madicp_deskew_plan(const madicp_points_t& pts, const double T_prev[12], cons
   const double resolution = 2 * M_PI / double(kChunks), delta = ts / double(kChunks - 1);
   madicp_host::HotScope hot;
   RawVec<Item> items(static_cast<size_t>(n_rec));
-  auto azimuths = [&](auto zero) {  // (pad = 1: the record survives the gate)
+  auto azimuths = [&](auto zero) {  // (pad = 1: the record survives the gate; 2: ... but its correction failed)
     using T = decltype(zero);
-    const madicp::RecReader<T> rd(pts);
+    const madicp::RecReader<T> rd(pts, vc);
     for_chunks(threads, size_t(n_rec), 8192, [&](size_t c0, size_t c1) {
       for (size_t i = c0; i < c1; ++i) {
-        T x, y, z;
-        rd.xyz(int64_t(i), x, y, z);
-        items[i] = Item{std::atan2(double(y), double(x)), int32_t(i), rd.keep(x, y, z) ? 1 : 0};
+        double x = 0, y = 0, z = 0;
+        bool bad = false;
+        const bool kept = rd.kept_point(int64_t(i), x, y, z, bad);
+        items[i] = Item{std::atan2(y, x), int32_t(i), bad ? 2 : (kept ? 1 : 0)};
       }
     });
   };
   if (pts.is_f32) azimuths(0.0f);
   else azimuths(0.0);
   size_t un = size_t(n_rec);
-  if (madicp::points_gated(pts)) {  // the kept records, in record order
+  if (madicp::points_gated(pts) || vc) {  // the kept records, in record order
     un = 0;
-    for (size_t i = 0; i < size_t(n_rec); ++i)
+    for (size_t i = 0; i < size_t(n_rec); ++i) {
+      if (items[i].pad == 2) return MADICP_ERR_STATE;
       if (items[i].pad) items[un++] = items[i];
+    }
   }
   *n_kept = int64_t(un);
   *n_poses = 0;

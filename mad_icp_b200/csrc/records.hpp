@@ -1,5 +1,6 @@
 // records.hpp -- host side of madicp_points_t (include/madicp_b200.h): validation, field reads, the range gate
-// (range_gate.h) with its bounds rounded to the field type.  Shared by gpu_tree.cu and ingest.cpp.
+// (range_gate.h) with its bounds rounded to the field type, and the optional vertical-angle correction
+// (madicp_vcorr_t, vertical_correction.h).  Shared by gpu_tree.cu, ingest.cpp and the facade.
 #pragma once
 #include <algorithm>
 #include <cmath>
@@ -9,6 +10,7 @@
 
 #include "../../include/madicp_b200.h"
 #include "range_gate.h"
+#include "vertical_correction.h"
 
 namespace madicp {
 void set_error(const std::string& msg);
@@ -33,7 +35,19 @@ inline size_t points_bytes(const madicp_points_t& d) {
   const int64_t end = std::max(d.offset[0], std::max(d.offset[1], d.offset[2])) + e;
   return size_t((d.n - 1) * d.stride + end);
 }
-inline bool same_points(const madicp_points_t& a, const madicp_points_t& b) {
+// the correction of a nullable madicp_vcorr_t: disabled, or enabled with its angle (the reserved field ignored)
+inline madicp_vcorr_t vcorr_of(const madicp_vcorr_t* v) {
+  madicp_vcorr_t o{};
+  if (v && v->enabled) {
+    o.angle = v->angle;
+    o.enabled = 1;
+  }
+  return o;
+}
+// the same scan as far as the device is concerned: equal descriptors and equal corrections (angles equal bit for bit)
+inline bool same_points(const madicp_points_t& a, const madicp_vcorr_t& va, const madicp_points_t& b,
+                        const madicp_vcorr_t& vb) {
+  if (va.enabled != vb.enabled || (va.enabled && std::memcmp(&va.angle, &vb.angle, sizeof(double)) != 0)) return false;
   return a.data == b.data && a.n == b.n && a.stride == b.stride && a.offset[0] == b.offset[0] && a.offset[1] == b.offset[1] &&
          a.offset[2] == b.offset[2] && (a.is_f32 != 0) == (b.is_f32 != 0) && a.min_range == b.min_range &&
          a.max_range == b.max_range && a.range_mode == b.range_mode && (a.drop_nan != 0) == (b.drop_nan != 0);
@@ -60,8 +74,16 @@ inline int check_points(const madicp_points_t* d, const char* fn) {
   if (d->range_mode < kGateNone || d->range_mode > kGateStrict) return bad("range_mode must be 0, 1 or 2");
   return MADICP_OK;
 }
+// MADICP_OK, or MADICP_ERR_INVALID with a message naming `fn`: an enabled correction needs a finite angle
+inline int check_vcorr(const madicp_vcorr_t* v, const char* fn) {
+  if (v && v->enabled && !std::isfinite(v->angle)) {
+    set_error(std::string(fn) + ": the vertical correction angle must be finite");
+    return MADICP_ERR_INVALID;
+  }
+  return MADICP_OK;
+}
 
-// The gate of one descriptor in field type T
+// The gate of one descriptor in field type T, and the correction (nullable table) of its kept points
 template <class T>
 struct RecReader {
   const char* base;
@@ -70,9 +92,11 @@ struct RecReader {
   T lo, hi;
   int mode, drop_nan;
   bool gated;
-  explicit RecReader(const madicp_points_t& d)
+  const VcorrTable* vc;
+  explicit RecReader(const madicp_points_t& d, const VcorrTable* vc_table = nullptr)
       : base(static_cast<const char*>(d.data)), stride(d.stride), off{d.offset[0], d.offset[1], d.offset[2]},
-        lo(T(d.min_range)), hi(T(d.max_range)), mode(d.range_mode), drop_nan(d.drop_nan), gated(points_gated(d)) {}
+        lo(T(d.min_range)), hi(T(d.max_range)), mode(d.range_mode), drop_nan(d.drop_nan), gated(points_gated(d)),
+        vc(vc_table) {}
   void xyz(int64_t i, T& x, T& y, T& z) const {
     const char* r = base + i * stride;
     std::memcpy(&x, r + off[0], sizeof(T));
@@ -80,6 +104,16 @@ struct RecReader {
     std::memcpy(&z, r + off[2], sizeof(T));
   }
   bool keep(T x, T y, T z) const { return !gated || range_keep<T>(x, y, z, lo, hi, mode, drop_nan); }
+  // Record i: whether the gate keeps it and, when it does, its point as float64, corrected.  `bad` is set when the
+  // correction's angle falls outside the table (the point is then not the reader's: the caller fails).
+  bool kept_point(int64_t i, double& x, double& y, double& z, bool& bad) const {
+    T fx, fy, fz;
+    xyz(i, fx, fy, fz);
+    if (!keep(fx, fy, fz)) return false;
+    x = double(fx); y = double(fy); z = double(fz);
+    if (vc && !vcorr_apply(*vc, x, y, z)) bad = true;
+    return true;
+  }
 };
 
 }  // namespace madicp

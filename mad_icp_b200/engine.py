@@ -9,7 +9,7 @@ import numpy as np
 
 from . import _capi as capi
 from ._capi import MadIcpError, as_b, as_d, as_i, check, pose12
-from .records import describe
+from .records import VERTICAL_ANGLE_OFFSET, describe, vcorr
 
 
 class FlatTree:
@@ -213,33 +213,46 @@ class Registrar:
                                        Tp, Tn, sensor_hz, num_threads, as_d(out)), "madicp_ingest")
         return out
 
-    # ---- raw sensor records (records.describe: strided x/y/z + the readers' range gate), read in place
+    # ---- raw sensor records (records.describe: strided x/y/z + the readers' range gate), read in place; with
+    # apply_correction=True the kept points get KITTI's vertical-angle correction (records.vcorr)
     def ingest_records(self, records, min_range=0.0, max_range=math.inf, inclusive=True, drop_nan=False, deskew=False,
-                       T_prev=None, T_now=None, sensor_hz=10.0, num_threads=1, want_points=False):
-        """Records -> device-resident float64 cloud of the kept points (madicp_ingest_points).  Returns the kept points
-        (want_points) or their number."""
+                       T_prev=None, T_now=None, sensor_hz=10.0, num_threads=1, want_points=False, apply_correction=False,
+                       vertical_angle_offset=VERTICAL_ANGLE_OFFSET):
+        """Records -> device-resident float64 cloud of the kept points (madicp_ingest_points_ex).  Returns the kept
+        points (want_points) or their number."""
         d = describe(records, min_range, max_range, inclusive, drop_nan)
+        v = vcorr(apply_correction, vertical_angle_offset)
         out = np.empty((d.n, 3)) if want_points else None
         kept = C.c_int64(0)
         Tp = as_d(pose12(T_prev)) if T_prev is not None else None
         Tn = as_d(pose12(T_now)) if T_now is not None else None
-        check(capi.lib().madicp_ingest_points(self._h, C.byref(d), int(deskew), Tp, Tn, sensor_hz, num_threads,
-                                              C.byref(kept), as_d(out)), "madicp_ingest_points")
+        check(capi.lib().madicp_ingest_points_ex(self._h, C.byref(d), C.byref(v) if v else None, int(deskew), Tp, Tn,
+                                                 sensor_hz, num_threads, C.byref(kept), as_d(out)), "madicp_ingest_points")
         return out[:kept.value].copy() if want_points else kept.value
 
-    def stage_records(self, records, reserve_points=0, **gate):
-        """Early upload of the records of a scan of the NEXT build_trees_records call (madicp_stage_points); pass the
-        same array and gate there, unchanged."""
+    def stage_records(self, records, reserve_points=0, apply_correction=False, vertical_angle_offset=VERTICAL_ANGLE_OFFSET,
+                      **gate):
+        """Early upload of the records of a scan of the NEXT build_trees_records call (madicp_stage_points_ex); pass the
+        same array, gate and correction there, unchanged."""
         d = describe(records, **gate)
+        v = vcorr(apply_correction, vertical_angle_offset)
         self._staged_keepalive.append(records)
-        check(capi.lib().madicp_stage_points(self._h, C.byref(d), int(reserve_points)), "madicp_stage_points")
+        check(capi.lib().madicp_stage_points_ex(self._h, C.byref(d), C.byref(v) if v else None, int(reserve_points)),
+              "madicp_stage_points")
 
-    def build_trees_records(self, records_list, b_max=0.2, b_min=0.1, **gate):
-        """Several scans of records at once: one forest build, a DeviceTree per scan (madtree_gpu_build_batch_points)."""
+    def build_trees_records(self, records_list, b_max=0.2, b_min=0.1, apply_correction=False,
+                            vertical_angle_offset=VERTICAL_ANGLE_OFFSET, **gate):
+        """Several scans of records at once: one forest build, a DeviceTree per scan (madtree_gpu_build_batch_points_ex).
+        apply_correction: one flag for all scans, or a sequence with one flag per scan."""
         k = len(records_list)
         descs = (capi.Points * k)(*[describe(r, **gate) for r in records_list])
+        flags = list(apply_correction) if isinstance(apply_correction, (list, tuple)) else [apply_correction] * k
+        if len(flags) != k:
+            raise ValueError("build_trees_records: one apply_correction flag per scan")
+        vcs = (capi.Vcorr * k)(*[vcorr(f, vertical_angle_offset) or capi.Vcorr() for f in flags])
         out = (C.c_void_p * k)()
-        check(capi.lib().madtree_gpu_build_batch_points(self._h, descs, k, b_max, b_min, out), "madtree_gpu_build_batch_points")
+        check(capi.lib().madtree_gpu_build_batch_points_ex(self._h, descs, vcs, k, b_max, b_min, out),
+              "madtree_gpu_build_batch_points")
         self._staged_keepalive.clear()
         return [DeviceTree(C.c_void_p(out[i]), self) for i in range(k)]
 

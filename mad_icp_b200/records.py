@@ -9,15 +9,21 @@ The dataset readers of the reference filter every scan with numpy before it reac
 (read in place, never copied on the host) and apply the same filter on the way in, with numpy's arithmetic: the
 kept points and their order are the reader's, bit for bit.  A Python float bound is compared in the field type, as
 numpy compares it.
+
+KITTI's reader can also rotate every kept point by a small vertical angle (`apply_correction`,
+apps/utils/kitti_reader.py:72-79, 90-91, a scipy rotation about p x e_z).  `apply_correction=True` does the same on
+the device, bit for bit with scipy 1.18 (`correct_vertical_angle` is the host restatement).
 """
 import ctypes as C
 import math
 
 import numpy as np
 
-from ._capi import Points
+from ._capi import Points, Vcorr
 
 RANGE_NONE, RANGE_INCLUSIVE, RANGE_STRICT = 0, 1, 2
+# KittiReader.vertical_angle_offset: the reader's own expression, so the default is its value bit for bit
+VERTICAL_ANGLE_OFFSET = float(np.radians(0.205))
 
 _POINTFIELD_TYPES = {7: np.dtype("<f4"), 8: np.dtype("<f8")}  # sensor_msgs/PointField FLOAT32, FLOAT64
 
@@ -111,6 +117,16 @@ def layout(records, min_range=0.0, max_range=math.inf, inclusive=True, drop_nan=
             d.range_mode, d.drop_nan)
 
 
+def vcorr(apply_correction=False, vertical_angle_offset=VERTICAL_ANGLE_OFFSET):
+    """madicp_vcorr_t of the reader's `apply_correction` / `vertical_angle_offset`, or None without a correction."""
+    if not apply_correction:
+        return None
+    v = Vcorr()
+    v.angle = float(vertical_angle_offset)
+    v.enabled = 1
+    return v
+
+
 def range_mask(records, **gate):
     """The gate on the host (madicp_debug_range_mask): uint8 keep flag per record."""
     from . import _capi
@@ -120,4 +136,17 @@ def range_mask(records, **gate):
     return keep[:d.n]
 
 
-__all__ = ["pointcloud2_dtype", "describe", "layout", "range_mask", "RANGE_NONE", "RANGE_INCLUSIVE", "RANGE_STRICT"]
+def correct_vertical_angle(records, vertical_angle_offset=VERTICAL_ANGLE_OFFSET, **gate):
+    """The kept points of `records` (describe's gate keywords), corrected like KittiReader.apply_rotation_correction,
+    on the host with the restatement the device applies (madicp_debug_correct_points): an M x 3 float64 array."""
+    from . import _capi
+    d = describe(records, **gate)
+    v = vcorr(True, vertical_angle_offset)
+    out = np.empty((max(int(d.n), 1), 3))
+    kept = _capi.check(_capi.lib().madicp_debug_correct_points(C.byref(d), C.byref(v), _capi.as_d(out)),
+                       "madicp_debug_correct_points")
+    return out[:kept]
+
+
+__all__ = ["pointcloud2_dtype", "describe", "layout", "range_mask", "vcorr", "correct_vertical_angle",
+           "VERTICAL_ANGLE_OFFSET", "RANGE_NONE", "RANGE_INCLUSIVE", "RANGE_STRICT"]

@@ -4,6 +4,8 @@ no range gate at the source) is laid out two ways:
   kitti   float32 N x 4 records (16 bytes), gate 0.7 <= r <= 120 (the KITTI config)
   ouster  48-byte PointCloud2 records, x/y/z float32 at 16/20/24, NaN rows for missing returns, NaN drop + gate
           0 < r < 50 (the vbr_os0 config; its reader hands float64 to compute)
+  kitti+correction  the kitti layout with the KITTI config's apply_correction: the reader's scipy rotation of the kept
+          points (kitti_reader.py:72-79, 90-91) + compute, against computeRecords(apply_correction=True)
 and run four ways: reader + compute, reader + prefetch, computeRecords, prefetchRecords (look-ahead batches of 16).
 Reports host wall time per scan (reader included), scans/s and H2D bytes per scan, plus the GPU name and power limit.
 Usage: python scripts/records_bench.py [n_scans=1000] [out.json]"""
@@ -15,6 +17,8 @@ import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
+
+from scipy.spatial.transform import Rotation
 
 from mad_icp_b200 import synth
 
@@ -59,6 +63,14 @@ def read_kitti(buf):  # kitti_reader.py:82-88
     return cloud[(norms >= 0.7) & (norms <= 120.0)]
 
 
+def read_kitti_corrected(buf):  # kitti_reader.py:72-79, 82-91 with apply_correction
+    points = read_kitti(buf)
+    rotation_vectors = np.cross(points, np.array([0., 0., 1.]))
+    norms = np.linalg.norm(rotation_vectors, axis=1).reshape(-1, 1)
+    rotation_vectors_normalized = rotation_vectors / norms
+    return Rotation.from_rotvec(np.radians(0.205) * rotation_vectors_normalized).apply(points)
+
+
 def read_ouster(buf):  # point_cloud2.py:77-87, 96
     s = np.frombuffer(buf, OUSTER)
     pts = np.column_stack([s["x"], s["y"], s["z"]])
@@ -72,6 +84,8 @@ LAYOUTS = {
               dict(min_range=0.7, max_range=120.0, inclusive=True, drop_nan=False)),
     "ouster": (ouster, read_ouster, lambda b: np.frombuffer(b, OUSTER),
                dict(min_range=0.0, max_range=50.0, inclusive=False, drop_nan=True)),
+    "kitti+correction": (kitti, read_kitti_corrected, lambda b: np.frombuffer(b, np.float32).reshape(-1, 4)[:, :3],
+                         dict(min_range=0.7, max_range=120.0, inclusive=True, drop_nan=False, apply_correction=True)),
 }
 kw = dict(sensor_hz=10.0, deskew=False, b_max=0.2, rho_ker=0.1, p_th=0.8, b_min=0.1, b_ratio=0.02, num_keyframes=16,
           num_threads=min(16, os.cpu_count() or 1), realtime=False)
@@ -92,7 +106,7 @@ def run(layout, records, prefetch):
                 for k in range(i, min(i + 16, len(bufs))):
                     p.prefetchRecords(view(bufs[k]), **gate)
             p.computeRecords(0.1 * i, a, **gate)
-            h2d += a.shape[0] * (16 if layout == "kitti" else 48) - (4 if layout == "kitti" else 20)
+            h2d += a.shape[0] * (48 if layout == "ouster" else 16) - (20 if layout == "ouster" else 4)
         else:
             pts = reader(b)
             if prefetch and i >= 1 and p.prefetched() == 0:

@@ -248,6 +248,27 @@ int madicp_stage_points_ex(madicp_ctx_t* ctx, const madicp_points_t* desc, const
 int madtree_gpu_build_batch_points_ex(madicp_ctx_t* ctx, const madicp_points_t* descs, const madicp_vcorr_t* vcorrs,
                                       int count, double b_max, double b_min, madtree_gpu_t** out);
 
+/* Look-ahead for deskewed scans.  What Pipeline::deskew decides from the points alone -- the range gate, the
+ * correction, the azimuths, the sort permutation (ties included) and the chunk of every sorted position -- does not
+ * depend on the poses, so it can be worked out, and uploaded with the records, while earlier scans register; only the
+ * <= 1024 chunk poses need T_prev / T_now.
+ * madicp_plan_points hands a future scan over: its records start going up to the device at once, and the pose-free
+ * half of the deskew runs on a host thread of the context (at most num_threads of them at a time; the shared host pool
+ * is left to the tree builds), after which its permutation and chunks go up too.  The records must stay valid and
+ * unchanged until the plan is consumed or freed.  Invalid descriptors and corrections fail here, as in
+ * madicp_ingest_points_ex; what depends on the points (a gate that keeps nothing, a rotation angle outside the table)
+ * fails the madicp_ingest_plan that consumes the plan.
+ * madicp_ingest_plan consumes the plan, whatever the outcome (do not use or free it afterwards): the same result as
+ * madicp_ingest_points_ex(desc, vcorr, deskew, T_prev, T_now, sensor_hz, ...) on the plan's scan, bit for bit, without
+ * a host synchronisation (unless points_out is given).  Plans of one context may be consumed in any order.
+ * madicp_plan_free gives a plan up; it returns once nothing reads the caller's records any more. */
+typedef struct madicp_plan madicp_plan_t;
+int madicp_plan_points(madicp_ctx_t* ctx, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int num_threads,
+                       madicp_plan_t** out);
+int madicp_ingest_plan(madicp_ctx_t* ctx, madicp_plan_t* plan, int deskew, const double T_prev[12], const double T_now[12],
+                       double sensor_hz, int64_t* n_kept, double* points_out);
+void madicp_plan_free(madicp_plan_t* plan);
+
 /* K1 only -- MADtree::bestMatchingLeafFast (tools/mad_tree.cpp:144-152) of X*mean for every moving
  * leaf against every active keyframe.  out_ordinals: K_active x L int32 on the host (row k = k-th
  * active slot in ascending slot order); values are getLeafs ordinals of the matched leaf. */

@@ -50,6 +50,16 @@ int64_t madicp_debug_range_mask(const madicp_points_t* desc, uint8_t* keep);
  * madicp_debug_range_mask; MADICP_ERR_STATE when a point's rotation angle falls outside the table.  No device work. */
 int64_t madicp_debug_correct_points(const madicp_points_t* desc, const madicp_vcorr_t* vcorr, double* out);
 
+/* The deskew plan of madicp_ingest_points_ex on the host: split != 0 runs its pose-independent order half (azimuths,
+ * sort, chunk of every sorted position) on the calling thread alone and then its pose half (the chunk poses), as a
+ * look-ahead plan does (madicp_plan_points / madicp_ingest_plan); split == 0 runs both as the ingest does, on
+ * num_threads threads.  perm / chunk receive *n_kept entries (room for desc->n), poses *n_poses x 12 (room for 1024).
+ * MADICP_ERR_STATE when a corrected point's rotation angle falls outside the table; a gate that keeps nothing gives
+ * *n_kept = 0.  No device work. */
+int madicp_debug_deskew_plan(const madicp_points_t* desc, const madicp_vcorr_t* vcorr, const double T_prev[12],
+                             const double T_now[12], double sensor_hz, int split, int num_threads, int32_t* perm,
+                             uint16_t* chunk, double* poses, int* n_poses, int64_t* n_kept);
+
 #ifdef __cplusplus
 }
 #endif

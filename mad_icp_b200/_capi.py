@@ -84,6 +84,11 @@ SYMBOLS = {
     "madicp_stage_points_ex": (C.c_int, [vp, pts_p, vc_p, C.c_int64]),
     "madtree_gpu_build_batch_points_ex": (C.c_int, [vp, pts_p, vc_p, C.c_int, C.c_double, C.c_double, C.POINTER(vp)]),
     "madicp_debug_correct_points": (C.c_int64, [pts_p, vc_p, dp]),
+    "madicp_plan_points": (C.c_int, [vp, pts_p, vc_p, C.c_int, C.POINTER(vp)]),
+    "madicp_ingest_plan": (C.c_int, [vp, vp, C.c_int, dp, dp, C.c_double, C.POINTER(C.c_int64), dp]),
+    "madicp_plan_free": (None, [vp]),
+    "madicp_debug_deskew_plan": (C.c_int, [pts_p, vc_p, dp, dp, C.c_double, C.c_int, C.c_int, ip,
+                                           C.POINTER(C.c_uint16), dp, C.POINTER(C.c_int), C.POINTER(C.c_int64)]),
     "madicp_register_fetch_weight": (C.c_int, [vp, dp, dp, dp, bp, C.POINTER(C.c_int), dp]),
     "madicp_register_partial_async": (C.c_int, [vp, C.c_int, dp]),
     "madicp_calibrate": (C.c_int, [vp, dp]),

@@ -77,6 +77,7 @@ struct madicp_ctx {
   cudaEvent_t tree_free_ev = nullptr;    // recorded on the context's stream at every madtree_gpu_free
   std::mutex tree_mu;                    // ... builders on other host threads allocate from it too
   void* build_state = nullptr;           // gpu_tree.cu: working memory of the device build (lazily created)
+  void* plan_state = nullptr;            // gpu_tree.cu: buffers and threads of look-ahead plans (lazily created)
   long long* d_dbg_cta = nullptr;  // MADICP_MAX_ITERS x grid item-phase cycles when debug timing is on
   madicp::IcpParams P{0.2, 0.31622776601683794, 0.02};
   double* d_moving = nullptr;               // raw L x 3 means as uploaded / gathered

@@ -92,6 +92,9 @@ struct VelocityEstimator {
 // the build's latency is that of its dependent-add chains, which a batch runs side by side -- and compute() then
 // consumes them in FIFO order.  Possible because a scan's tree depends on the pose estimates only when the scan is
 // deskewed (pipeline.cpp:137-141).  No threads: the batch is built by the thread that calls compute().
+// A deskewed scan queues a plan instead (madicp_plan_points, pushPlan): its records go up and the pose-free half of its
+// deskew (gate, correction, azimuth sort, chunks) runs on a library thread at once; compute() then consumes it with
+// the latest poses (madicp_ingest_plan) and builds its tree alone -- the tree depends on the poses of the scan before.
 class Lookahead {
  public:
   struct Job {
@@ -105,20 +108,43 @@ class Lookahead {
     std::shared_ptr<void> keepalive;
     size_t n = 0;
     madtree_gpu_t* tree = nullptr;
+    madicp_plan_t* plan = nullptr;  // a deskewed scan's look-ahead plan (pushPlan)
     const void* data() const { return ext ? ext : (is_f32 ? static_cast<const void*>(f32.data()) : static_cast<const void*>(f64.data())); }
   };
   Lookahead(madicp_ctx_t* ctx, double b_max, double b_min, int batch) : ctx_(ctx), b_max_(b_max), b_min_(b_min), batch_(batch) {}
   ~Lookahead() {
     madicp_stage_discard(ctx_);  // uploads and background sums may still be reading the queued clouds
-    for (auto& j : fifo_)
+    for (auto& j : fifo_) {
       if (j.tree) madtree_gpu_free(j.tree);
+      if (j.plan) madicp_plan_free(j.plan);  // (returns once nothing reads the scan's buffer)
+    }
   }
   void push(Job&& j) {
     fifo_.push_back(std::move(j));
     stageQueued();
   }
+  // a deskewed scan: planned at once, over its records or its packed cloud, with at most num_threads plans' order
+  // halves running at a time
+  void pushPlan(Job&& j, int num_threads) {
+    fifo_.push_back(std::move(j));
+    Job& q = fifo_.back();  // (planned where its private copy, if any, will stay)
+    const madicp_points_t d = q.records ? q.pts : madicp::packed_points(q.data(), int64_t(q.n), q.is_f32 ? 1 : 0);
+    const int rc = madicp_plan_points(ctx_, &d, q.records ? &q.vc : nullptr, num_threads, &q.plan);
+    if (rc < 0) {
+      const std::string msg = "madicp_plan_points failed (" + std::to_string(rc) + "): " + madicp_last_error();
+      fifo_.pop_back();
+      throw Error(msg);
+    }
+  }
   bool empty() const { return fifo_.empty(); }
   size_t size() const { return fifo_.size(); }
+  bool frontIsPlan() const { return !fifo_.empty() && fifo_.front().plan; }
+  // the oldest queued scan, a planned one (the caller consumes the plan)
+  Job popPlan() {
+    Job j = std::move(fifo_.front());
+    fifo_.pop_front();
+    return j;
+  }
   // tree of the oldest prefetched scan
   madtree_gpu_t* pop() {
     if (!fifo_.front().tree) buildBatch();
@@ -132,7 +158,9 @@ class Lookahead {
  private:
   // scans that can share one batch call: packed clouds of one element type, or records (each with its own correction:
   // the batch call takes one per scan)
-  static bool sameKind(const Job& a, const Job& b) { return a.records == b.records && (a.records || a.is_f32 == b.is_f32); }
+  static bool sameKind(const Job& a, const Job& b) {
+    return !a.plan && !b.plan && a.records == b.records && (a.records || a.is_f32 == b.is_f32);
+  }
   // Builds the trees of the longest run of queued scans of the front's kind, up to the batch size.  A scan whose tree
   // cannot be built (records the range gate leaves empty) fails the batch call as a whole: the run is then halved until
   // the batch no longer contains it, and once the front scan fails on its own it is dropped from the queue and its
@@ -189,7 +217,7 @@ class Lookahead {
   void stageQueued() {
     while (staged_ < size_t(batch_) && built_ + staged_ < fifo_.size()) {
       const Job& j = fifo_[built_ + staged_];
-      if (!sameKind(j, fifo_[built_])) break;
+      if (j.plan || !sameKind(j, fifo_[built_])) break;
       if (j.records)
         check(madicp_stage_points_ex(ctx_, &j.pts, &j.vc, int64_t(batch_) * int64_t(j.n)), "madicp_stage_points");
       else
@@ -305,12 +333,14 @@ class Pipeline {
   int lastIcpIterations() const { return last_iters_; }  // rounds the realtime budget allowed for the last scan
   // Hands a FUTURE scan over for a look-ahead (batched) tree build (see Lookahead).  compute() then consumes the
   // prefetched scans in the order they were handed over and ignores its own cloud argument for them.  Returns false (and does
-  // nothing) when look-ahead is not possible: host-built trees, or deskewing (the scan needs the latest poses).
+  // nothing) when look-ahead is not possible: host-built trees, or deskewing without deskew_ahead (the scan needs the
+  // latest poses).  deskew_ahead on a deskewing pipeline: the scan is planned instead -- uploaded, gated, corrected and
+  // sorted by azimuth ahead of time; compute() applies the chunk poses and builds its tree (no effect without deskew).
   // keepalive: when given, the buffer is read in place (no copy) and the handle is dropped once compute() has consumed
   // the scan; without it the cloud is copied.
   bool prefetch(const void* xyz, size_t n, bool is_f32, std::shared_ptr<void> keepalive = nullptr,
-                const madicp_points_t* records = nullptr, const madicp_vcorr_t* vc = nullptr) {
-    if (!gpu_build_ || deskew_ || !xyz || n == 0) return false;
+                const madicp_points_t* records = nullptr, const madicp_vcorr_t* vc = nullptr, bool deskew_ahead = false) {
+    if (!gpu_build_ || (deskew_ && !deskew_ahead) || !xyz || n == 0) return false;
     const auto p0 = clk();
     struct Tick {  // (the hand-over runs on the thread that launches the registrations: its cost is part of the scan's)
       Pipeline* p; std::chrono::steady_clock::time_point t0;
@@ -342,11 +372,13 @@ class Pipeline {
     } else {
       j.f64.assign(static_cast<const double*>(xyz), static_cast<const double*>(xyz) + 3 * n);
     }
-    lookahead_->push(std::move(j));
+    if (deskew_) lookahead_->pushPlan(std::move(j), num_threads_);
+    else lookahead_->push(std::move(j));
     return true;
   }
-  bool prefetchRecords(const madicp_points_t& pts, std::shared_ptr<void> keepalive, const madicp_vcorr_t* vc = nullptr) {
-    return prefetch(pts.data, pts.n > 0 ? size_t(pts.n) : 0, pts.is_f32 != 0, std::move(keepalive), &pts, vc);
+  bool prefetchRecords(const madicp_points_t& pts, std::shared_ptr<void> keepalive, const madicp_vcorr_t* vc = nullptr,
+                       bool deskew_ahead = false) {
+    return prefetch(pts.data, pts.n > 0 ? size_t(pts.n) : 0, pts.is_f32 != 0, std::move(keepalive), &pts, vc, deskew_ahead);
   }
   size_t prefetched() { return lookahead_ ? lookahead_->size() : 0; }
 
@@ -354,11 +386,16 @@ class Pipeline {
   // the scan's MAD-tree: ingest (+ deskew, pipeline.cpp:137-138) and build, on the device or on the host
   std::unique_ptr<MADtree> makeTree(const void* xyz, size_t n, bool is_f32, const madicp_points_t* records,
                                     const madicp_vcorr_t* vc) {
-    if (lookahead_ && !lookahead_->empty())  // built ahead of time by a worker lane
-      return std::unique_ptr<MADtree>(new MADtree(icp_.context(), lookahead_->pop(), b_max_));
     const bool dsk = deskew_ && is_initialized_ && trajectory_.size() > 1;
     const double* Ta = dsk ? trajectory_[trajectory_.size() - 2].m : nullptr;
     const double* Tb = dsk ? trajectory_[trajectory_.size() - 1].m : nullptr;
+    if (lookahead_ && lookahead_->frontIsPlan()) {  // planned ahead of time: the chunk poses, the ingest, the tree
+      const Lookahead::Job j = lookahead_->popPlan();  // (a failure leaves the scans after it queued)
+      check(madicp_ingest_plan(icp_.context(), j.plan, dsk ? 1 : 0, Ta, Tb, sensor_hz_, nullptr, nullptr), "madicp_ingest_plan");
+      return std::unique_ptr<MADtree>(new MADtree(icp_.context(), b_max_, b_min_));
+    }
+    if (lookahead_ && !lookahead_->empty())  // built ahead of time by a worker lane
+      return std::unique_ptr<MADtree>(new MADtree(icp_.context(), lookahead_->pop(), b_max_));
     if (gpu_build_ && records) {
       check(madicp_ingest_points_ex(icp_.context(), records, vc, dsk ? 1 : 0, Ta, Tb, sensor_hz_,
                                     std::max(1 << max_parallel_levels_, 1), nullptr, nullptr), "madicp_ingest_points");

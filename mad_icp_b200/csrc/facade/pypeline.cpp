@@ -74,7 +74,7 @@ PYBIND11_MODULE(pypeline, m) {
       .def_static("_deskewOnly", [](const py::object& cloud, const NpArr& a, const NpArr& b, double sensor_hz, int num_threads) {
         return mb::Pipeline::deskewOnly(cloud_arg(cloud), pose_from_numpy(a), pose_from_numpy(b), sensor_hz, num_threads);
       }, py::arg("cloud"), py::arg("T_prev"), py::arg("T_now"), py::arg("sensor_hz"), py::arg("num_threads") = 1)
-      .def("prefetch", [](mb::Pipeline& p, const py::object& cloud) {
+      .def("prefetch", [](mb::Pipeline& p, const py::object& cloud, bool deskew_ahead) {
         // the array is read in place when the batch is built (inside a later compute()): a reference keeps it alive
         // until then (it is dropped there, on the calling thread, with the GIL held)
         auto hold = [](const py::object& o) {
@@ -83,17 +83,17 @@ PYBIND11_MODULE(pypeline, m) {
         };
         if (py::isinstance<mb::ContainerType>(cloud)) {
           const mb::ContainerType& v = cloud.cast<const mb::ContainerType&>();
-          return p.prefetch(v.empty() ? nullptr : v[0].data(), v.size(), false, hold(cloud));
+          return p.prefetch(v.empty() ? nullptr : v[0].data(), v.size(), false, hold(cloud), nullptr, nullptr, deskew_ahead);
         }
         if (py::isinstance<py::array>(cloud) && py::array::ensure(cloud).dtype().is(py::dtype::of<float>())) {
           const auto a = cloud.cast<py::array_t<float, py::array::c_style | py::array::forcecast>>();
           if (a.ndim() != 2 || a.shape(1) != 3) throw py::cast_error();
-          return p.prefetch(a.data(), size_t(a.shape(0)), true, hold(a));
+          return p.prefetch(a.data(), size_t(a.shape(0)), true, hold(a), nullptr, nullptr, deskew_ahead);
         }
         const NpArr a = cloud.cast<NpArr>();
         if (a.ndim() != 2 || a.shape(1) != 3) throw py::cast_error();
-        return p.prefetch(a.data(), size_t(a.shape(0)), false, hold(a));
-      }, py::arg("cloud"))
+        return p.prefetch(a.data(), size_t(a.shape(0)), false, hold(a), nullptr, nullptr, deskew_ahead);
+      }, py::arg("cloud"), py::arg("deskew_ahead") = false)
       // additions (not in the reference): raw sensor records, filtered on the way in like the dataset readers do
       // (mad_icp_b200/records.py describes the array; it is read in place); apply_correction: KITTI's vertical-angle
       // correction of the kept points, as KittiReader applies it
@@ -104,15 +104,19 @@ PYBIND11_MODULE(pypeline, m) {
       }, py::arg("stamp"), py::arg("records"), py::arg("min_range") = 0.0,
          py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false,
          py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle)
+      // deskew_ahead (prefetch, prefetchRecords): on a deskewing pipeline the scan is planned ahead -- uploaded, gated,
+      // corrected and sorted by azimuth while earlier scans register -- and compute applies its chunk poses
       .def("prefetchRecords", [](mb::Pipeline& p, const py::object& records, double min_range, double max_range,
-                                 bool inclusive, bool drop_nan, bool apply_correction, double vertical_angle_offset) {
+                                 bool inclusive, bool drop_nan, bool apply_correction, double vertical_angle_offset,
+                                 bool deskew_ahead) {
         const madicp_points_t d = records_arg(records, min_range, max_range, inclusive, drop_nan);
         const madicp_vcorr_t v = vcorr_arg(apply_correction, vertical_angle_offset);
         py::object* ref = new py::object(records);  // dropped once the scan's tree is built (see prefetch)
-        return p.prefetchRecords(d, std::shared_ptr<void>(ref, [](void* q) { delete static_cast<py::object*>(q); }), &v);
+        return p.prefetchRecords(d, std::shared_ptr<void>(ref, [](void* q) { delete static_cast<py::object*>(q); }), &v,
+                                 deskew_ahead);
       }, py::arg("records"), py::arg("min_range") = 0.0,
          py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false,
-         py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle)
+         py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle, py::arg("deskew_ahead") = false)
       .def("prefetched", &mb::Pipeline::prefetched)
       .def("lastIcpIterations", &mb::Pipeline::lastIcpIterations)
       .def("gpuBuild", &mb::Pipeline::gpuBuild)

@@ -15,6 +15,7 @@
 #include <condition_variable>
 #include <deque>
 #include <future>
+#include <memory>
 #include <mutex>
 #include <functional>
 #include <cstdio>
@@ -36,6 +37,9 @@ void madicp_host_for(int n, int num_threads, const std::function<void(int)>& fn)
 int madicp_deskew_plan(const madicp_points_t& pts, const VcorrTable* vc, const double T_prev[12], const double T_now[12],
                        double sensor_hz, int num_threads, int32_t* perm, uint16_t* chunk, double* poses, int* n_poses,
                        int64_t* n_kept);
+int madicp_deskew_order(const madicp_points_t& pts, const VcorrTable* vc, int num_threads, int32_t* perm, uint16_t* chunk,
+                        int* n_chunks, int64_t* n_kept);
+void madicp_deskew_poses(const double T_prev[12], const double T_now[12], double sensor_hz, int n_chunks, double* poses);
 void madicp_host_trig(const double* args, double* res, int n, int num_threads);
 void madicp_host_hot(int on);
 
@@ -612,9 +616,16 @@ int build_resident(madicp_ctx* c, BuildState* bs, cudaStream_t st, int64_t n, do
   return build_forest(c, bs, st, 1, offs, b_max, b_min, root_S, bs->kept_check, out);
 }
 
+struct PlanLane;  // (look-ahead plans, below)
+void release_plan_lane(PlanLane* L);
+
 }  // namespace
 
 void madicp_gpu_build_release(madicp_ctx* c) {
+  if (c->plan_state) {  // (plans still held by the caller are the caller's to free first)
+    release_plan_lane(static_cast<PlanLane*>(c->plan_state));
+    c->plan_state = nullptr;
+  }
   BuildState* bs = static_cast<BuildState*>(c->build_state);
   if (!bs) return;
   release(bs);
@@ -691,10 +702,9 @@ RecSrc rec_src(const madicp_points_t& d, size_t raw, int first, int vc) {
   s.hi = d.is_f32 ? double(float(d.max_range)) : d.max_range;
   return s;
 }
-// Order-preserving compaction of the gated records of B (d_raw) into P[0]; the kept count of every scan goes to
-// bs->h_kept.  vc: some scan of B is corrected.
-int launch_compaction(madicp_ctx* c, BuildState* bs, cudaStream_t st, const RecBatch& B, bool vc) {
-  const char* raw = static_cast<const char*>(bs->d_raw);
+// Order-preserving compaction of the gated records of B (in `raw`: d_raw or a plan's copy) into P[0]; the kept count of
+// every scan goes to bs->h_kept.  vc: some scan of B is corrected.
+int launch_compaction(madicp_ctx* c, BuildState* bs, cudaStream_t st, const RecBatch& B, const char* raw, bool vc) {
   const int tiles = (B.n_rec + kTile - 1) / kTile;
   k_gate_flags<<<blocks(B.n_rec), kBlock, 0, st>>>(B, raw, bs->flag);
   k_scan_tiles<<<tiles, kTile, 0, st>>>(bs->flag, B.n_rec, bs->G, bs->tile);
@@ -771,7 +781,7 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* v
       B.s[b] = rec_src(d[b], raw_off[b], first[b], slot);
     }
     if (gated) {
-      if (int e = launch_compaction(c, bs, st, B, corrected)) return e;
+      if (int e = launch_compaction(c, bs, st, B, raw, corrected)) return e;
     } else {
       auto k = corrected ? k_ingest<true> : k_ingest<false>;
       k<<<blocks(n_rec), kBlock, 0, st>>>(B, raw, nullptr, nullptr, bs->d_poses, n_rec, bs->P[0], bs->d_vtab, bs->h_vc_err);
@@ -853,13 +863,241 @@ int stage(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int
   return MADICP_OK;
 }
 
-// The ingest behind madicp_ingest and madicp_ingest_points[_ex] (descriptor and correction validated).
+// ---- look-ahead plans of deskewed scans (madicp_plan_points / madicp_ingest_plan)
+//
+// A plan is one future scan whose pose-free deskew half (madicp_deskew_order: gate, correction, azimuths, sort, chunk
+// sweep) runs on a host thread of the context while earlier scans register, and whose records, permutation and chunk
+// numbers are uploaded on the plan lane's own stream.  Consuming it leaves the chunk poses (a few microseconds), one
+// k_ingest over the plan's buffers and the tree build.  The plan lane is separate from the build lane (BuildState):
+// the build lane may be re-allocated while plans are in flight, and its copy stream with it.
+
+// device and pinned buffers of one plan, recycled through the lane's cache (as device trees are)
+struct PlanBuf {
+  size_t cap = 0, raw_cap = 0;  // records, bytes
+  char* d_raw = nullptr;        // the records as uploaded
+  int32_t* d_perm = nullptr;
+  uint16_t* d_chunk = nullptr;
+  int32_t* h_perm = nullptr;  // pinned: what the order half writes
+  uint16_t* h_chunk = nullptr;
+  cudaEvent_t ready = nullptr;    // lane stream: records, perm and chunk are on the device
+  cudaEvent_t free_ev = nullptr;  // context stream: the last ingest that read the device buffers has run
+};
+void free_buf(PlanBuf* b) {
+  if (b->ready) cudaEventSynchronize(b->ready);
+  if (b->free_ev) cudaEventSynchronize(b->free_ev);
+  cudaFree(b->d_raw);
+  cudaFree(b->d_perm);
+  cudaFree(b->d_chunk);
+  cudaFreeHost(b->h_perm);
+  cudaFreeHost(b->h_chunk);
+  if (b->ready) cudaEventDestroy(b->ready);
+  if (b->free_ev) cudaEventDestroy(b->free_ev);
+  delete b;
+}
+
+struct PlanLane {
+  static constexpr int kRing = 8;                // chunk-pose tables in flight
+  static constexpr int kRingPoses = 2 * 1024;    // per table: the sweep makes at most 1024 chunks (+1 on rounding)
+  int device = 0;
+  cudaStream_t stream = nullptr;  // uploads of the plans
+  double* h_poses = nullptr;      // pinned ring of chunk-pose tables: kRing x kRingPoses x 12
+  cudaEvent_t ring_done[kRing] = {};
+  uint32_t ring_seq = 0;
+  std::mutex mu;  // everything below
+  std::condition_variable cv;
+  std::vector<PlanBuf*> cache;
+  struct Task {
+    int limit;  // at most this many order halves at a time (this one included)
+    std::function<void()> fn;
+  };
+  std::deque<Task> tasks;
+  int running = 0;
+  bool stop = false;
+  std::vector<std::thread> workers;
+
+  void submit(int limit, std::function<void()> fn) {
+    {
+      std::lock_guard<std::mutex> lk(mu);
+      tasks.push_back(Task{limit, std::move(fn)});
+      while (int(workers.size()) < limit) workers.emplace_back([this]() { loop(); });
+    }
+    cv.notify_all();
+  }
+  void loop() {
+    std::unique_lock<std::mutex> lk(mu);
+    for (;;) {
+      cv.wait(lk, [this]() { return stop || (!tasks.empty() && running < tasks.front().limit); });
+      if (stop) return;
+      Task t = std::move(tasks.front());
+      tasks.pop_front();
+      ++running;
+      lk.unlock();
+      t.fn();
+      lk.lock();
+      --running;
+      cv.notify_all();
+    }
+  }
+};
+
+void release_plan_lane(PlanLane* L) {
+  {
+    std::lock_guard<std::mutex> lk(L->mu);
+    L->stop = true;
+  }
+  L->cv.notify_all();
+  for (std::thread& t : L->workers) t.join();
+  for (PlanBuf* b : L->cache) free_buf(b);
+  if (L->stream) {
+    cudaStreamSynchronize(L->stream);
+    cudaStreamDestroy(L->stream);
+  }
+  for (cudaEvent_t e : L->ring_done)
+    if (e) cudaEventDestroy(e);
+  if (L->h_poses) cudaFreeHost(L->h_poses);
+  delete L;
+}
+
+int plan_lane(madicp_ctx* c, PlanLane** out) {
+  if (c->plan_state) {
+    *out = static_cast<PlanLane*>(c->plan_state);
+    return MADICP_OK;
+  }
+  PlanLane* L = new PlanLane;
+  L->device = c->device;
+  cudaError_t e = cudaStreamCreateWithFlags(&L->stream, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaHostAlloc(&L->h_poses, size_t(PlanLane::kRing) * PlanLane::kRingPoses * 12 * sizeof(double), 0);
+  for (int r = 0; r < PlanLane::kRing && e == cudaSuccess; ++r) e = cudaEventCreateWithFlags(&L->ring_done[r], cudaEventDisableTiming);
+  if (e != cudaSuccess) {
+    release_plan_lane(L);
+    set_error(std::string("madicp_plan_points: ") + cudaGetErrorString(e));
+    return MADICP_ERR_CUDA;
+  }
+  c->plan_state = L;
+  *out = L;
+  return MADICP_OK;
+}
+
+// a cached buffer that holds n records of `bytes` bytes, or a new one
+int plan_buf(PlanLane* L, size_t n, size_t bytes, PlanBuf** out) {
+  {
+    std::lock_guard<std::mutex> lk(L->mu);
+    for (size_t i = 0; i < L->cache.size(); ++i)
+      if (L->cache[i]->cap >= n && L->cache[i]->raw_cap >= bytes) {
+        *out = L->cache[i];
+        L->cache.erase(L->cache.begin() + long(i));
+        return MADICP_OK;
+      }
+  }
+  PlanBuf* b = new PlanBuf;
+  b->cap = size_t(1) << 17;
+  while (b->cap < n) b->cap <<= 1;
+  b->raw_cap = size_t(1) << 21;
+  while (b->raw_cap < bytes) b->raw_cap <<= 1;
+  cudaError_t e = cudaMalloc(&b->d_raw, b->raw_cap);
+  if (e == cudaSuccess) e = cudaMalloc(&b->d_perm, b->cap * sizeof(int32_t));
+  if (e == cudaSuccess) e = cudaMalloc(&b->d_chunk, b->cap * sizeof(uint16_t));
+  if (e == cudaSuccess) e = cudaHostAlloc(&b->h_perm, b->cap * sizeof(int32_t), 0);
+  if (e == cudaSuccess) e = cudaHostAlloc(&b->h_chunk, b->cap * sizeof(uint16_t), 0);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->ready, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->free_ev, cudaEventDisableTiming);
+  if (e != cudaSuccess) {
+    free_buf(b);
+    set_error(std::string("madicp_plan_points: ") + cudaGetErrorString(e));
+    return MADICP_ERR_CUDA;
+  }
+  *out = b;
+  return MADICP_OK;
+}
+void return_buf(PlanLane* L, PlanBuf* b) {
+  std::lock_guard<std::mutex> lk(L->mu);
+  L->cache.push_back(b);
+}
+
+}  // namespace
+
+struct madicp_plan {
+  madicp_ctx* ctx = nullptr;
+  PlanLane* lane = nullptr;
+  madicp_points_t d{};
+  madicp_vcorr_t vc{};
+  PlanBuf* buf = nullptr;
+  std::promise<void> done_p;
+  std::future<void> done;  // the order half has run and its uploads are queued
+  // the order half's outcome (valid once `done` is ready)
+  int rc = MADICP_OK;
+  std::string err;  // message of rc (none for MADICP_ERR_STATE: the caller names the angle)
+  int64_t kept = 0;
+  int n_chunks = 0;
+};
+
+namespace {
+
+// The order half of a plan, on one of the lane's threads: the permutation and chunks into the pinned arrays, then
+// their uploads behind the records on the lane's stream, then `ready`.
+void plan_order(madicp_plan* p) {
+  PlanBuf* b = p->buf;
+  cudaStream_t st = p->lane->stream;
+  int rc = MADICP_OK;
+  std::string err;
+  auto cuda = [&](cudaError_t e, const char* what) {
+    if (e != cudaSuccess && rc != MADICP_ERR_CUDA) {
+      rc = MADICP_ERR_CUDA;
+      err = std::string("madicp_plan_points: ") + what + ": " + cudaGetErrorString(e);
+    }
+  };
+  cuda(cudaSetDevice(p->lane->device), "cudaSetDevice");
+  cuda(cudaEventSynchronize(b->ready), "cudaEventSynchronize");  // the buffer's last uploads from h_perm / h_chunk have run
+  if (!rc) {
+    VcorrTable table;
+    rc = madicp_deskew_order(p->d, vcorr_table(p->vc, &table), 1, b->h_perm, b->h_chunk, &p->n_chunks, &p->kept);
+    if (rc && rc != MADICP_ERR_STATE) err = madicp_last_error();
+  }
+  if (!rc && p->kept > 0) {
+    cuda(cudaMemcpyAsync(b->d_perm, b->h_perm, size_t(p->kept) * sizeof(int32_t), cudaMemcpyHostToDevice, st), "perm upload");
+    cuda(cudaMemcpyAsync(b->d_chunk, b->h_chunk, size_t(p->kept) * sizeof(uint16_t), cudaMemcpyHostToDevice, st), "chunk upload");
+  }
+  cuda(cudaEventRecord(b->ready, st), "cudaEventRecord");  // (after the records' upload too, whatever the outcome)
+  p->rc = rc;
+  p->err = err;
+  p->done_p.set_value();
+}
+
+// Gives a plan up: waits for its order half and (wait_uploads) its uploads, the buffer returns to the lane's cache.
+void plan_release(madicp_plan* p, bool wait_uploads) {
+  p->done.wait();
+  if (wait_uploads) cudaEventSynchronize(p->buf->ready);
+  return_buf(p->lane, p->buf);
+  delete p;
+}
+
+// The chunk poses of a consumed plan: computed into the next table of the lane's pinned ring and copied to d_poses on
+// `st` -- no synchronisation unless the ring wrapped around a copy that has not run yet.
+int stage_chunk_poses(PlanLane* L, cudaStream_t st, const double T_prev[12], const double T_now[12], double sensor_hz,
+                      int n_chunks, double* d_poses) {
+  if (n_chunks > PlanLane::kRingPoses) {
+    set_error("madicp_ingest_plan: internal error (chunk count)");
+    return MADICP_ERR_STATE;
+  }
+  const int r = int(L->ring_seq % PlanLane::kRing);
+  CK(cudaEventSynchronize(L->ring_done[r]));
+  double* h = L->h_poses + size_t(r) * PlanLane::kRingPoses * 12;
+  madicp_deskew_poses(T_prev, T_now, sensor_hz, n_chunks, h);
+  CK(cudaMemcpyAsync(d_poses, h, size_t(n_chunks) * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(L->ring_done[r], st));
+  L->ring_seq++;
+  return MADICP_OK;
+}
+
+// The ingest behind madicp_ingest, madicp_ingest_points[_ex] and madicp_ingest_plan (descriptor and correction
+// validated).  plan (nullable): the scan's records are already on their way up, with its deskew order (madicp_plan_points).
 int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int deskew, const double T_prev[12],
-           const double T_now[12], double sensor_hz, int num_threads, int64_t* n_kept, double* points_out, const char* fn) {
+           const double T_now[12], double sensor_hz, int num_threads, madicp_plan* plan, int64_t* n_kept, double* points_out,
+           const char* fn) {
   CK(cudaSetDevice(c->device));
   BuildState* bs = nullptr;
   const int64_t n = d.n;
-  const size_t bytes = size_t(n) * size_t(d.stride);
+  const size_t bytes = plan ? 0 : size_t(n) * size_t(d.stride);
   int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
   if (!rc) rc = ensure_state(c, size_t(n), bytes, &bs);
   if (rc) return rc;
@@ -867,9 +1105,13 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
   bs->n_resident = 0;
   bs->kept_check = 0;
   bs->vc_check = vc.enabled != 0;
-  // the raw scan goes up while the host works out the order (deskew) or the root's sums
-  CK(cudaMemcpyAsync(bs->d_raw, d.data, points_bytes(d), cudaMemcpyHostToDevice, st));
   const char* raw = static_cast<const char*>(bs->d_raw);
+  if (plan) {  // the records, the permutation and the chunks went up on the plan lane's stream
+    CK(cudaStreamWaitEvent(st, plan->buf->ready, 0));
+    raw = plan->buf->d_raw;
+  } else {  // the raw scan goes up while the host works out the order (deskew) or the root's sums
+    CK(cudaMemcpyAsync(bs->d_raw, d.data, points_bytes(d), cudaMemcpyHostToDevice, st));
+  }
   int slot = -1;
   if (vc.enabled) CK(cudaMemsetAsync(bs->h_vc_err, 0, sizeof(int), st));
   if (int e = vtab_room(bs, st, &vc, 1)) return e;
@@ -879,7 +1121,19 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
   B.n_rec = int(n);
   B.s[0] = rec_src(d, 0, 0, slot);
   int64_t kept = n;
-  if (deskew) {
+  if (deskew && plan) {  // only the chunk poses are left
+    if (plan->rc == MADICP_ERR_STATE) set_error(vcorr_out_of_table(fn, vc.angle));
+    else if (plan->rc) set_error(plan->err);
+    if (plan->rc) return plan->rc;
+    kept = plan->kept;
+    if (kept > 0) {
+      if (int e = stage_chunk_poses(plan->lane, st, T_prev, T_now, sensor_hz, plan->n_chunks, bs->d_poses)) return e;
+      auto k = vc.enabled ? k_ingest<true> : k_ingest<false>;
+      k<<<blocks(kept), kBlock, 0, st>>>(B, raw, plan->buf->d_perm, plan->buf->d_chunk, bs->d_poses, int(kept), bs->P[0],
+                                         bs->d_vtab, bs->h_vc_err);
+      c->launches++;
+    }
+  } else if (deskew) {
     CK(cudaStreamSynchronize(st));  // h_perm / h_chunk / h_poses of the previous scan have been consumed
     int n_poses = 0;
     VcorrTable table;  // (the azimuths are those of the corrected points)
@@ -897,7 +1151,7 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
       c->launches++;
     }
   } else if (points_gated(d)) {
-    if (int e = launch_compaction(c, bs, st, B, vc.enabled)) return e;
+    if (int e = launch_compaction(c, bs, st, B, raw, vc.enabled)) return e;
     kept = root_host(d, vc, bs->root_S);
     bs->kept_check = 1;
   } else {
@@ -907,6 +1161,7 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
     kept = root_host(d, vc, bs->root_S);
   }
   CK(cudaGetLastError());
+  if (plan) CK(cudaEventRecord(plan->buf->free_ev, st));  // (the plan's buffers may be reused once this has run)
   if (kept == 0) {
     bs->kept_check = 0;
     set_error(std::string(fn) + ": no point inside the range gate");
@@ -1093,7 +1348,7 @@ int madicp_ingest(madicp_ctx_t* c, const void* xyz, int64_t n, int is_f32, int d
   }
   MADICP_TRY
   return ingest(c, packed_points(xyz, n, is_f32), madicp_vcorr_t{}, deskew, T_prev, T_now, sensor_hz, num_threads, nullptr,
-                points_out, "madicp_ingest");
+                nullptr, points_out, "madicp_ingest");
   MADICP_CATCH("madicp_ingest")
 }
 
@@ -1107,7 +1362,7 @@ int madicp_ingest_points_ex(madicp_ctx_t* c, const madicp_points_t* desc, const 
   if (int e = check_points(desc, "madicp_ingest_points")) return e;
   if (int e = check_vcorr(vcorr, "madicp_ingest_points")) return e;
   MADICP_TRY
-  return ingest(c, *desc, vcorr_of(vcorr), deskew, T_prev, T_now, sensor_hz, num_threads, n_kept, points_out,
+  return ingest(c, *desc, vcorr_of(vcorr), deskew, T_prev, T_now, sensor_hz, num_threads, nullptr, n_kept, points_out,
                 "madicp_ingest_points");
   MADICP_CATCH("madicp_ingest_points")
 }
@@ -1115,6 +1370,79 @@ int madicp_ingest_points_ex(madicp_ctx_t* c, const madicp_points_t* desc, const 
 int madicp_ingest_points(madicp_ctx_t* c, const madicp_points_t* desc, int deskew, const double T_prev[12],
                          const double T_now[12], double sensor_hz, int num_threads, int64_t* n_kept, double* points_out) {
   return madicp_ingest_points_ex(c, desc, nullptr, deskew, T_prev, T_now, sensor_hz, num_threads, n_kept, points_out);
+}
+
+int madicp_plan_points(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int num_threads,
+                       madicp_plan_t** out) {
+  if (!c || !out) {
+    set_error("madicp_plan_points: bad arguments");
+    return MADICP_ERR_INVALID;
+  }
+  *out = nullptr;
+  if (int e = check_points(desc, "madicp_plan_points")) return e;
+  if (int e = check_vcorr(vcorr, "madicp_plan_points")) return e;
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  PlanLane* L = nullptr;
+  if (int e = plan_lane(c, &L)) return e;
+  PlanBuf* b = nullptr;
+  if (int e = plan_buf(L, size_t(desc->n), points_bytes(*desc), &b)) return e;
+  std::unique_ptr<madicp_plan> p(new madicp_plan);
+  p->ctx = c;
+  p->lane = L;
+  p->d = *desc;
+  p->vc = vcorr_of(vcorr);
+  p->buf = b;
+  p->done = p->done_p.get_future();
+  // the records go up now, once the last ingest that read this buffer has run
+  cudaError_t e = cudaStreamWaitEvent(L->stream, b->free_ev, 0);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(b->d_raw, desc->data, points_bytes(*desc), cudaMemcpyHostToDevice, L->stream);
+  if (e != cudaSuccess) {
+    return_buf(L, b);
+    set_error(std::string("madicp_plan_points: ") + cudaGetErrorString(e));
+    return MADICP_ERR_CUDA;
+  }
+  madicp_plan* q = p.get();
+  L->submit(std::max(1, std::min(num_threads, 64)), [q]() { plan_order(q); });
+  *out = p.release();
+  return MADICP_OK;
+  MADICP_CATCH("madicp_plan_points")
+}
+
+int madicp_ingest_plan(madicp_ctx_t* c, madicp_plan_t* plan, int deskew, const double T_prev[12], const double T_now[12],
+                       double sensor_hz, int64_t* n_kept, double* points_out) {
+  if (!plan) {
+    set_error("madicp_ingest_plan: null plan");
+    return MADICP_ERR_INVALID;
+  }
+  int rc = MADICP_OK;
+  if (!c || c != plan->ctx || (deskew && (!T_prev || !T_now || !(sensor_hz > 0.0)))) {
+    set_error("madicp_ingest_plan: bad arguments (the plan's context, and the poses and rate when deskewing)");
+    rc = MADICP_ERR_INVALID;
+  }
+  try {
+    plan->done.wait();
+    if (!rc && plan->rc == MADICP_ERR_CUDA) {  // (a CUDA failure of the order half: its uploads cannot be trusted)
+      set_error(plan->err);
+      rc = plan->rc;
+    }
+    if (!rc)
+      rc = ingest(c, plan->d, plan->vc, deskew, T_prev, T_now, sensor_hz, 0, plan, n_kept, points_out, "madicp_ingest_plan");
+  } catch (const std::bad_alloc&) {
+    set_error("madicp_ingest_plan: out of host memory");
+    rc = MADICP_ERR_NOMEM;
+  } catch (const std::exception& e) {
+    set_error(std::string("madicp_ingest_plan: ") + e.what());
+    rc = MADICP_ERR_INVALID;
+  }
+  plan_release(plan, rc != MADICP_OK);  // (a failed call returns once nothing reads the records any more)
+  return rc;
+}
+
+void madicp_plan_free(madicp_plan_t* plan) {
+  if (!plan) return;
+  cudaSetDevice(plan->ctx->device);
+  plan_release(plan, true);
 }
 
 int64_t madicp_debug_range_mask(const madicp_points_t* desc, uint8_t* keep) {

@@ -114,6 +114,33 @@ class DeviceTree:
         return out
 
 
+class DeskewPlan:
+    """A future scan handed over for a deskewed look-ahead (`Registrar.plan_records`): its records are on their way to
+    the device and its pose-free deskew order is worked out on a host thread.  `Registrar.ingest_plan` consumes it;
+    dropping it unconsumed frees it.  It keeps its records alive."""
+
+    def __init__(self, handle, registrar, records):
+        self._h, self._reg, self._records = handle, registrar, records  # the registrar must outlive the plan
+
+    def _take(self):
+        h, self._h = self._h, None
+        if not h:
+            raise ValueError("the plan has been consumed or freed")
+        return h
+
+    def free(self):
+        h = getattr(self, "_h", None)
+        if h and getattr(self._reg, "_h", None):
+            self._h = None
+            try:
+                capi.lib().madicp_plan_free(h)
+            except TypeError:  # interpreter shutdown
+                pass
+        self._records = None
+
+    __del__ = free
+
+
 class Registrar:
     """One GPU's registration context (reference: class MADicp + Pipeline's keyframe deque)."""
 
@@ -255,6 +282,34 @@ class Registrar:
               "madtree_gpu_build_batch_points")
         self._staged_keepalive.clear()
         return [DeviceTree(C.c_void_p(out[i]), self) for i in range(k)]
+
+    def plan_records(self, records, min_range=0.0, max_range=math.inf, inclusive=True, drop_nan=False, num_threads=1,
+                     apply_correction=False, vertical_angle_offset=VERTICAL_ANGLE_OFFSET):
+        """Hands a future scan over for a deskewed look-ahead (madicp_plan_points): the records start going up at once
+        and the pose-free half of the deskew runs on a host thread (at most num_threads at a time).  Returns a
+        DeskewPlan for ingest_plan; the array is read in place and must stay unchanged until then."""
+        d = describe(records, min_range, max_range, inclusive, drop_nan)
+        v = vcorr(apply_correction, vertical_angle_offset)
+        h = C.c_void_p()
+        check(capi.lib().madicp_plan_points(self._h, C.byref(d), C.byref(v) if v else None, int(num_threads), C.byref(h)),
+              "madicp_plan_points")
+        return DeskewPlan(h, self, records)
+
+    def ingest_plan(self, plan, deskew=False, T_prev=None, T_now=None, sensor_hz=10.0, want_points=False):
+        """Consumes a DeskewPlan (madicp_ingest_plan): the same device-resident cloud as ingest_records on its scan with
+        the same deskew arguments.  Returns the kept points (want_points) or their number."""
+        h = plan._take()
+        n = plan._records.shape[0]
+        out = np.empty((n, 3)) if want_points else None
+        kept = C.c_int64(0)
+        Tp = as_d(pose12(T_prev)) if T_prev is not None else None
+        Tn = as_d(pose12(T_now)) if T_now is not None else None
+        try:
+            check(capi.lib().madicp_ingest_plan(self._h, h, int(deskew), Tp, Tn, sensor_hz, C.byref(kept), as_d(out)),
+                  "madicp_ingest_plan")
+        finally:
+            plan._records = None
+        return out[:kept.value].copy() if want_points else kept.value
 
     def set_moving_tree(self, tree):
         check(capi.lib().madicp_set_moving_tree(self._h, tree._h), "madicp_set_moving_tree")

@@ -7,8 +7,15 @@ no range gate at the source) is laid out two ways:
   kitti+correction  the kitti layout with the KITTI config's apply_correction: the reader's scipy rotation of the kept
           points (kitti_reader.py:72-79, 90-91) + compute, against computeRecords(apply_correction=True)
 and run four ways: reader + compute, reader + prefetch, computeRecords, prefetchRecords (look-ahead batches of 16).
+Two deskewed layouts (the mulran / vbr_os1 configs deskew) run three ways: reader + compute, computeRecords, and
+prefetchRecords(deskew_ahead=True) (look-ahead plans, 16 at a time):
+  kitti+deskew   the kitti layout, deskewed at 10 Hz
+  ouster+deskew  the ouster layout with vbr_os1's strict gate 1.3 < r < 120, deskewed at 20 Hz
 Reports host wall time per scan (reader included), scans/s and H2D bytes per scan, plus the GPU name and power limit.
-Usage: python scripts/records_bench.py [n_scans=1000] [out.json]"""
+With MADICP_PIPELINE_TIMING set every pipeline prints its per-phase means to stderr when it is destroyed.
+Usage: python scripts/records_bench.py [n_scans=1000] [out.json] [layouts=all, comma-separated] [ways=all: any of
+reader,records,prefetch]"""
+import hashlib
 import json
 import os
 import subprocess
@@ -23,7 +30,7 @@ from scipy.spatial.transform import Rotation
 from mad_icp_b200 import synth
 
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 1000
-out_path = sys.argv[2] if len(sys.argv) > 2 else None
+out_path = sys.argv[2] if len(sys.argv) > 2 and sys.argv[2] != "-" else None
 scene = synth.StreetScene(seed=7, x_min=-45.0, x_max=60.0 + 0.8 * n)
 OUSTER = np.dtype({"names": ["x", "y", "z", "intensity", "t", "reflectivity"],
                    "formats": ["<f4", "<f4", "<f4", "<f4", "<u4", "<u2"], "offsets": [16, 20, 24, 28, 32, 40], "itemsize": 48})
@@ -71,29 +78,38 @@ def read_kitti_corrected(buf):  # kitti_reader.py:72-79, 82-91 with apply_correc
     return Rotation.from_rotvec(np.radians(0.205) * rotation_vectors_normalized).apply(points)
 
 
-def read_ouster(buf):  # point_cloud2.py:77-87, 96
+def read_ouster(buf, lo=0.0, hi=50.0):  # point_cloud2.py:77-87, 96
     s = np.frombuffer(buf, OUSTER)
     pts = np.column_stack([s["x"], s["y"], s["z"]])
     pts = pts[~np.any(np.isnan(pts), axis=1)]
     norms = np.linalg.norm(pts, axis=1)
-    return pts[(norms > 0.0) & (norms < 50.0)].astype(np.float64)
+    return pts[(norms > lo) & (norms < hi)].astype(np.float64)
 
 
+# name: (buffers, reader, records view, gate, pipeline settings)
 LAYOUTS = {
     "kitti": (kitti, read_kitti, lambda b: np.frombuffer(b, np.float32).reshape(-1, 4)[:, :3],
-              dict(min_range=0.7, max_range=120.0, inclusive=True, drop_nan=False)),
+              dict(min_range=0.7, max_range=120.0, inclusive=True, drop_nan=False), {}),
     "ouster": (ouster, read_ouster, lambda b: np.frombuffer(b, OUSTER),
-               dict(min_range=0.0, max_range=50.0, inclusive=False, drop_nan=True)),
+               dict(min_range=0.0, max_range=50.0, inclusive=False, drop_nan=True), {}),
     "kitti+correction": (kitti, read_kitti_corrected, lambda b: np.frombuffer(b, np.float32).reshape(-1, 4)[:, :3],
-                         dict(min_range=0.7, max_range=120.0, inclusive=True, drop_nan=False, apply_correction=True)),
+                         dict(min_range=0.7, max_range=120.0, inclusive=True, drop_nan=False, apply_correction=True), {}),
+    "kitti+deskew": (kitti, read_kitti, lambda b: np.frombuffer(b, np.float32).reshape(-1, 4)[:, :3],
+                     dict(min_range=0.7, max_range=120.0, inclusive=True, drop_nan=False), dict(deskew=True)),
+    "ouster+deskew": (ouster, lambda b: read_ouster(b, 1.3, 120.0), lambda b: np.frombuffer(b, OUSTER),
+                      dict(min_range=1.3, max_range=120.0, inclusive=False, drop_nan=True),
+                      dict(deskew=True, sensor_hz=20.0)),
 }
 kw = dict(sensor_hz=10.0, deskew=False, b_max=0.2, rho_ker=0.1, p_th=0.8, b_min=0.1, b_ratio=0.02, num_keyframes=16,
           num_threads=min(16, os.cpu_count() or 1), realtime=False)
 
 
 def run(layout, records, prefetch):
-    bufs, reader, view, gate = LAYOUTS[layout]
-    p = Pipeline(**kw)
+    bufs, reader, view, gate, settings = LAYOUTS[layout]
+    cfg = dict(kw, **settings)
+    ahead = dict(deskew_ahead=True) if cfg["deskew"] else {}  # (a deskewed pipeline plans its look-ahead scans)
+    p = Pipeline(**cfg)
+    sys.stderr.write(f"[{layout} {'records' if records else 'reader+compute'}{' +prefetch' if prefetch else ''}] ")
     h2d = 0
     poses = []
     t0 = None
@@ -104,18 +120,20 @@ def run(layout, records, prefetch):
             a = view(b)
             if prefetch and i >= 1 and p.prefetched() == 0:
                 for k in range(i, min(i + 16, len(bufs))):
-                    p.prefetchRecords(view(bufs[k]), **gate)
-            p.computeRecords(0.1 * i, a, **gate)
-            h2d += a.shape[0] * (48 if layout == "ouster" else 16) - (20 if layout == "ouster" else 4)
+                    assert p.prefetchRecords(view(bufs[k]), **gate, **ahead)
+            p.computeRecords(i / cfg["sensor_hz"], a, **gate)
+            h2d += a.shape[0] * (48 if layout.startswith("ouster") else 16) - (20 if layout.startswith("ouster") else 4)
         else:
             pts = reader(b)
             if prefetch and i >= 1 and p.prefetched() == 0:
                 for k in range(i, min(i + 16, len(bufs))):
                     p.prefetch(reader(bufs[k]))
-            p.compute(0.1 * i, pts)
+            p.compute(i / cfg["sensor_hz"], pts)
             h2d += pts.nbytes
         poses.append(p.currentPose())
     dt = time.perf_counter() - t0
+    del p  # (prints its phases now, with MADICP_PIPELINE_TIMING)
+    sys.stderr.flush()
     return dict(ms_per_scan=1e3 * dt / (len(bufs) - 1), scans_per_s=(len(bufs) - 1) / dt, h2d_bytes_per_scan=h2d / len(bufs),
                 poses=np.array(poses))
 
@@ -129,18 +147,24 @@ def gpu_info():
         return f"unknown ({e})"
 
 
+layouts = sys.argv[3].split(",") if len(sys.argv) > 3 and sys.argv[3] != "all" else list(LAYOUTS)
+ways = sys.argv[4].split(",") if len(sys.argv) > 4 else ["reader", "records", "prefetch"]
 result = dict(gpu=gpu_info(), n_scans=n, runs={})
 print("GPU:", result["gpu"])
-for layout in LAYOUTS:
+for layout in layouts:
     base = None
+    deskew = LAYOUTS[layout][4].get("deskew", False)
     for prefetch in (False, True):
         for records in (False, True):
+            if (prefetch and ("prefetch" not in ways or (deskew and not records)) or
+                    (not prefetch and ("records" if records else "reader") not in ways)):
+                continue  # (deskewed: look-ahead plans take records)
             name = f"{layout} {'records' if records else 'reader+compute'}{' +prefetch' if prefetch else ''}"
             r = run(layout, records, prefetch)
             if base is None:
                 base = r["poses"]
             same = bool((r["poses"] == base).all())
-            r.pop("poses")
+            r["poses_sha256"] = hashlib.sha256(np.ascontiguousarray(r.pop("poses")).tobytes()).hexdigest()
             r["poses_equal_reader_compute"] = same
             result["runs"][name] = r
             print(f"{name:34s} {r['ms_per_scan']:7.3f} ms/scan  {r['scans_per_s']:7.1f} scans/s  "

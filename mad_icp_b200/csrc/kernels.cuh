@@ -351,14 +351,16 @@ __device__ __forceinline__ int descend(const ModelView& M, int k, double qx, dou
 //   * The gate `|ml - f.mean| > ball` decides a flag (matched_) and a discontinuous contribution, so
 //     it is evaluated exactly as the reference does (FP64, no FMA); the square root is only taken
 //     when d^2 is within 1e-14 (relative) of ball^2, where the comparison of squares could disagree
-//     with the comparison of rounded roots.
+//     with the comparison of rounded roots.  The square keeps the radius's sign (b_ratio < 0 can make it negative):
+//     a negative radius then rejects every pair, d^2 = 0 included, as `norm > ball` does; a NaN radius accepts
+//     every pair; fabs folds into the multiply as a source modifier.
 //   * e, J and the products are continuous in their inputs; they use FMA (tolerance on H/b is
 //     1e-12 relative, an FMA moves a term by <= 1 ulp).
 __device__ __forceinline__ bool linearize_one(const double* __restrict__ X, double rho, const Moving4& m, double mlx,
                                               double mly, double mlz, const Rec& f, double ww, double* v) {
   const double ex = mlx - f.mx, ey = mly - f.my, ez = mlz - f.mz;
   const double d2 = dot3(ex, ey, ez, ex, ey, ez);
-  const double b2 = m.ball * m.ball;
+  const double b2 = m.ball * fabs(m.ball);
   if (d2 > b2 * (1.0 + 1e-14)) return false;
   if (!(d2 < b2 * (1.0 - 1e-14)) && sqrt(d2) > m.ball) return false;
   const double e = fma(ez, f.dz, fma(ey, f.dy, ex * f.dx));

@@ -133,7 +133,9 @@ def case_parameter_sweep(M, b_max, b_min, rho_ker, b_ratio):
     return out
 
 
-SWEEP = [(0.1, 0.05, 0.05, 0.01), (0.4, 0.2, 0.3, 0.05), (0.2, 0.1, 1e-3, 0.0)]
+# the last: a negative ratio makes every gate radius negative (|mean| > 4 m for every leaf of the case), and the
+# reference's `norm > ball` then rejects every pair
+SWEEP = [(0.1, 0.05, 0.05, 0.01), (0.4, 0.2, 0.3, 0.05), (0.2, 0.1, 1e-3, 0.0), (0.2, 0.1, 0.1, -0.05)]
 CASES = {f"tree_build[{b}]": (case_tree_build, dict(b_max=b)) for b in (0.2, 1e-5)}
 CASES["lidar_scan_and_async_levels"] = (case_lidar_scan_and_async_levels, {})
 CASES["degenerate_clouds"] = (case_degenerate_clouds, {})
@@ -209,4 +211,11 @@ def test_deskew_is_the_references(M, pinned):
 
 @pytest.mark.parametrize("b_max,b_min,rho_ker,b_ratio", SWEEP)
 def test_parameter_sweep_is_the_references(M, pinned, b_max, b_min, rho_ker, b_ratio):
-    _run(M, pinned, "parameter_sweep[%g-%g-%g-%g]" % (b_max, b_min, rho_ker, b_ratio))
+    out = _run(M, pinned, "parameter_sweep[%g-%g-%g-%g]" % (b_max, b_min, rho_ker, b_ratio))
+    icp = out["icp"]
+    if b_ratio < 0:  # the pinned digests are those of "nothing matched": H = b = 0, the pose never moves
+        assert not icp["matched"].any()
+        assert (icp["H_hist"] == 0).all() and (icp["b_hist"] == 0).all()
+        assert (icp["X"] == icp["X_hist"][0]).all()
+    else:
+        assert icp["matched"].mean() > 0.5

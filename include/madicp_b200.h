@@ -201,7 +201,7 @@ int madicp_ingest(madicp_ctx_t* ctx, const void* xyz, int64_t n, int is_f32, int
 #define MADICP_RANGE_INCLUSIVE 1
 #define MADICP_RANGE_STRICT 2
 typedef struct madicp_points {
-  const void* data; /* host memory: field c of record i at data + i * stride + offset[c] */
+  const void* data; /* host memory (device memory for the _dev calls): field c of record i at data + i * stride + offset[c] */
   int64_t n;        /* records */
   int64_t stride;   /* bytes from one record to the next */
   int32_t offset[3];
@@ -269,6 +269,33 @@ int madicp_ingest_plan(madicp_ctx_t* ctx, madicp_plan_t* plan, int deskew, const
                        double sensor_hz, int64_t* n_kept, double* points_out);
 void madicp_plan_free(madicp_plan_t* plan);
 
+/* ---------------- scans that already live on the device (a GPU driver, a simulator, a learned pre-processing step) ----
+ * The record entry points for a madicp_points_t whose `data` is device memory of the context's device (a CUDA tensor's
+ * storage, a CuPy array): the records are read in place, never copied to the host, with the same gate, correction and
+ * compaction as uploaded records -- the same kept cloud bit for bit, so the same trees and poses.
+ *   - desc->data must be device memory of the context's device, aligned to the field size (checked with
+ *     cudaPointerGetAttributes): host, managed or another device's memory is MADICP_ERR_INVALID, with a message.  Any
+ *     base address and stride is read (views with a storage offset included); 128-bit loads are used where the base is
+ *     16-byte aligned, one load per field elsewhere.
+ *   - producer_stream: the stream on which the records become ready (0: the legacy default stream).  Each call records
+ *     an event there and makes the context's stream wait on it; the caller does not synchronise.
+ *   - every call but madicp_plan_points_dev returns only after the library has finished reading the caller's records
+ *     (whatever the outcome); a plan reads them until it is consumed (madicp_ingest_plan) or freed, as host plans do.
+ *   - the host cannot count or sum device points: the kept counts come back from the device after the compaction (one
+ *     synchronisation) and the roots' sums run on the device.  A deskew copies the kept points (not the records) to the
+ *     host for the azimuth order, whose sort and libm calls stay there.
+ *   - there is no _dev staging call: there is no upload left to hide.
+ * points_out stays host memory. */
+int madicp_ingest_points_dev(madicp_ctx_t* ctx, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int deskew,
+                             const double T_prev[12], const double T_now[12], double sensor_hz, int num_threads,
+                             void* producer_stream, int64_t* n_kept, double* points_out);
+int madtree_gpu_build_batch_points_dev(madicp_ctx_t* ctx, const madicp_points_t* descs, const madicp_vcorr_t* vcorrs,
+                                       int count, double b_max, double b_min, void* producer_stream, madtree_gpu_t** out);
+/* The plan is consumed by madicp_ingest_plan (and freed by madicp_plan_free) like a host plan.  Its gate and correction
+ * run on the context's stream at once; an angle outside the table fails the madicp_ingest_plan that consumes it. */
+int madicp_plan_points_dev(madicp_ctx_t* ctx, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int num_threads,
+                           void* producer_stream, madicp_plan_t** out);
+
 /* K1 only -- MADtree::bestMatchingLeafFast (tools/mad_tree.cpp:144-152) of X*mean for every moving
  * leaf against every active keyframe.  out_ordinals: K_active x L int32 on the host (row k = k-th
  * active slot in ascending slot order); values are getLeafs ordinals of the matched leaf. */
@@ -327,6 +354,13 @@ int madicp_deskew(double* points_xyz, int64_t n, const double T_prev[12], const 
  * (leaf mean), normals n x 3, dists n. */
 int madicp_search_cloud(madicp_ctx_t* ctx, int slot, const double* queries_xyz, int64_t n, int32_t* ordinals,
                         double* points, double* normals, double* dists);
+/* The same with every pointer in device memory of the context's device: query i is x, y, z at queries + i * q_stride
+ * bytes, float32 (q_is_f32 != 0, widened to float64 exactly) or float64, read in place; the outputs (nullable, as above)
+ * are written in place.  The context's stream first waits for consumer_stream (where the queries are written and the
+ * outputs allocated; 0: the legacy default stream), and the results are ready on consumer_stream through an event wait:
+ * no host synchronisation. */
+int madicp_search_cloud_dev(madicp_ctx_t* ctx, int slot, const void* queries, int64_t n, int64_t q_stride, int q_is_f32,
+                            int32_t* ordinals, double* points, double* normals, double* dists, void* consumer_stream);
 
 /* Number of kernels this context has launched so far (bench.py's gpu_launches). */
 int64_t madicp_kernel_launches(const madicp_ctx_t* ctx);

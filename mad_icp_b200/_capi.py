@@ -87,6 +87,11 @@ SYMBOLS = {
     "madicp_plan_points": (C.c_int, [vp, pts_p, vc_p, C.c_int, C.POINTER(vp)]),
     "madicp_ingest_plan": (C.c_int, [vp, vp, C.c_int, dp, dp, C.c_double, C.POINTER(C.c_int64), dp]),
     "madicp_plan_free": (None, [vp]),
+    "madicp_ingest_points_dev": (C.c_int, [vp, pts_p, vc_p, C.c_int, dp, dp, C.c_double, C.c_int, vp, C.POINTER(C.c_int64),
+                                           dp]),
+    "madtree_gpu_build_batch_points_dev": (C.c_int, [vp, pts_p, vc_p, C.c_int, C.c_double, C.c_double, vp, C.POINTER(vp)]),
+    "madicp_plan_points_dev": (C.c_int, [vp, pts_p, vc_p, C.c_int, vp, C.POINTER(vp)]),
+    "madicp_search_cloud_dev": (C.c_int, [vp, C.c_int, vp, C.c_int64, C.c_int64, C.c_int, vp, vp, vp, vp, vp]),
     "madicp_debug_deskew_plan": (C.c_int, [pts_p, vc_p, dp, dp, C.c_double, C.c_int, C.c_int, ip,
                                            C.POINTER(C.c_uint16), dp, C.POINTER(C.c_int), C.POINTER(C.c_int64)]),
     "madicp_register_fetch_weight": (C.c_int, [vp, dp, dp, dp, bp, C.POINTER(C.c_int), dp]),

@@ -284,6 +284,7 @@ int madicp_create(madicp_ctx_t** out, int device, int max_keyframes) {
   CK(cudaMalloc(&c->d_comm, sizeof(CommBlock)));
   CK(cudaMemset(c->d_comm, 0, sizeof(CommBlock)));
   CK(cudaEventCreateWithFlags(&c->tree_free_ev, cudaEventDisableTiming));
+  CK(cudaEventCreateWithFlags(&c->xstream_ev, cudaEventDisableTiming));
   CK(cudaMalloc(&c->d_pool_lvl, size_t(max_keyframes) * (kMaxLevels + 1) * sizeof(int)));
   CK(cudaMalloc(&c->d_xform, size_t(madicp_ctx::kXformRing) * 12 * sizeof(double)));
   CK(cudaMallocHost(&c->h_xform, size_t(madicp_ctx::kXformRing) * 12 * sizeof(double)));
@@ -350,6 +351,7 @@ void madicp_destroy(madicp_ctx_t* c) {
     if (c->xform_done[i]) cudaEventDestroy(c->xform_done[i]);
   cudaFreeHost(c->h_matched);
   if (c->tree_free_ev) cudaEventDestroy(c->tree_free_ev);
+  if (c->xstream_ev) cudaEventDestroy(c->xstream_ev);
   cudaStreamDestroy(c->own_stream);
   delete c;
 }
@@ -606,6 +608,34 @@ int madicp_tree_alloc(madicp_ctx* c, size_t cap_nodes, madtree_gpu** out) {
   t->h_lvl.clear();
   t->full = nullptr;
   *out = t;
+  return MADICP_OK;
+}
+
+int madicp_check_device_ptr(madicp_ctx* c, const void* p, int align, const char* fn) {
+  cudaPointerAttributes a{};
+  const cudaError_t e = cudaPointerGetAttributes(&a, p);
+  cudaGetLastError();  // (an unknown pointer is an answer here, not a sticky error)
+  const char* why = nullptr;
+  if (e != cudaSuccess || a.type == cudaMemoryTypeUnregistered) why = "host memory";
+  else if (a.type == cudaMemoryTypeHost) why = "pinned host memory";
+  else if (a.type == cudaMemoryTypeManaged) why = "managed memory";
+  else if (a.device != c->device) why = "memory of another device";
+  if (why) {
+    set_error(std::string(fn) + ": the data must be device memory of the context's device " + std::to_string(c->device) +
+              ", not " + why + (a.type == cudaMemoryTypeDevice ? " (" + std::to_string(a.device) + ")" : std::string()));
+    return MADICP_ERR_INVALID;
+  }
+  if (reinterpret_cast<uintptr_t>(p) % uintptr_t(align)) {
+    set_error(std::string(fn) + ": the data is not aligned to its field size (" + std::to_string(align) + " bytes)");
+    return MADICP_ERR_INVALID;
+  }
+  return MADICP_OK;
+}
+
+int madicp_stream_wait(madicp_ctx* c, void* waiter, void* signaller) {
+  auto stream = [](void* s) { return s ? static_cast<cudaStream_t>(s) : cudaStreamLegacy; };
+  CK(cudaEventRecord(c->xstream_ev, stream(signaller)));
+  CK(cudaStreamWaitEvent(stream(waiter), c->xstream_ev, 0));
   return MADICP_OK;
 }
 
@@ -1072,7 +1102,8 @@ int madicp_search_cloud(madicp_ctx_t* c, int slot, const double* q, int64_t n, i
   double* d_d = d_q + size_t(n) * 9;
   int* d_o = c->d_cloud_o;
   CK(cudaMemcpyAsync(d_q, q, size_t(n) * 3 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  k_search_cloud<<<grid_for(c, n), kStepBlock, 0, c->stream>>>(make_view(c), slot_rank(c, slot), d_q, n, d_o,
+  k_search_cloud<<<grid_for(c, n), kStepBlock, 0, c->stream>>>(make_view(c), slot_rank(c, slot),
+                                                              reinterpret_cast<const char*>(d_q), n, 24, 0, d_o,
                                                               points ? d_p : nullptr, normals ? d_n : nullptr,
                                                               dists ? d_d : nullptr);
   c->launches++;
@@ -1083,6 +1114,29 @@ int madicp_search_cloud(madicp_ctx_t* c, int slot, const double* q, int64_t n, i
   if (dists) CK(cudaMemcpyAsync(dists, d_d, size_t(n) * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return MADICP_OK;
+}
+
+int madicp_search_cloud_dev(madicp_ctx_t* c, int slot, const void* queries, int64_t n, int64_t q_stride, int q_is_f32,
+                            int32_t* ordinals, double* points, double* normals, double* dists, void* consumer_stream) {
+  const int64_t e = q_is_f32 ? 4 : 8;
+  if (!c || !queries || n < 1 || slot < 0 || slot >= c->max_keyframes || c->slots[slot].n_nodes == 0 ||
+      q_stride < 3 * e || q_stride % e) {
+    set_error("madicp_search_cloud_dev: bad arguments (queries, n >= 1, a row stride holding x, y, z) or empty slot");
+    return MADICP_ERR_INVALID;
+  }
+  CK(cudaSetDevice(c->device));
+  const void* outs[4] = {ordinals, points, normals, dists};
+  if (int rc = madicp_check_device_ptr(c, queries, int(e), "madicp_search_cloud_dev")) return rc;
+  for (int k = 0; k < 4; ++k)
+    if (outs[k])
+      if (int rc = madicp_check_device_ptr(c, outs[k], k ? 8 : 4, "madicp_search_cloud_dev (output)")) return rc;
+  if (int rc = madicp_stream_wait(c, c->stream, consumer_stream)) return rc;  // queries written, outputs allocated there
+  k_search_cloud<<<grid_for(c, n), kStepBlock, 0, c->stream>>>(make_view(c), slot_rank(c, slot),
+                                                              static_cast<const char*>(queries), n, q_stride,
+                                                              q_is_f32 ? 1 : 0, ordinals, points, normals, dists);
+  c->launches++;
+  CK(cudaGetLastError());
+  return madicp_stream_wait(c, consumer_stream, c->stream);
 }
 
 // ------------------------------------------------------------------------------ multi-GPU

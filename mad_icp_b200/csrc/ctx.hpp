@@ -75,6 +75,7 @@ struct madicp_ctx {
   std::vector<madtree_gpu*> tree_cache;  // freed device trees keep their memory for the next scan
   std::vector<void*> tree_slabs;         // the allocations the trees are carved from
   cudaEvent_t tree_free_ev = nullptr;    // recorded on the context's stream at every madtree_gpu_free
+  cudaEvent_t xstream_ev = nullptr;      // hand-overs with a caller's stream (madicp_stream_wait)
   std::mutex tree_mu;                    // ... builders on other host threads allocate from it too
   void* build_state = nullptr;           // gpu_tree.cu: working memory of the device build (lazily created)
   void* plan_state = nullptr;            // gpu_tree.cu: buffers and threads of look-ahead plans (lazily created)
@@ -154,5 +155,11 @@ struct madicp_ctx {
 
 // capi.cu
 int madicp_tree_alloc(madicp_ctx* c, size_t cap_nodes, madtree_gpu** out);
+// MADICP_OK, or MADICP_ERR_INVALID with a message naming `fn`: p must be device memory (not host, managed or another
+// device's) of the context's device, aligned to `align` bytes
+int madicp_check_device_ptr(madicp_ctx* c, const void* p, int align, const char* fn);
+// `waiter` waits for everything enqueued on `signaller` so far (either one a caller's cudaStream_t, 0 being the legacy
+// default stream), through the context's hand-over event: no host synchronisation
+int madicp_stream_wait(madicp_ctx* c, void* waiter, void* signaller);
 // gpu_tree.cu
 void madicp_gpu_build_release(madicp_ctx* c);

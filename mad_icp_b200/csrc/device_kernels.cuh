@@ -288,13 +288,23 @@ __global__ void k_solve(const double* __restrict__ H, const double* __restrict__
   }
 }
 
-// MADtreeWrapper::searchCloud / searchCloudDist: arbitrary query points against one keyframe.
+// MADtreeWrapper::searchCloud / searchCloudDist: arbitrary query points against one keyframe.  Query i is x, y, z at
+// q + i * q_stride (bytes), float32 (q_is_f32) or float64, read in place; a float32 query is widened to float64 as the
+// host converts it.
 __global__ void __launch_bounds__(kStepBlock)
-k_search_cloud(const __grid_constant__ ModelView model, int root, const double* __restrict__ q, int64_t n,
-               int* __restrict__ ordinals, double* __restrict__ points, double* __restrict__ normals,
+k_search_cloud(const __grid_constant__ ModelView model, int root, const char* __restrict__ q, int64_t n, int64_t q_stride,
+               int q_is_f32, int* __restrict__ ordinals, double* __restrict__ points, double* __restrict__ normals,
                double* __restrict__ dists) {
   for (int64_t i = int64_t(blockIdx.x) * kStepBlock + threadIdx.x; i < n; i += int64_t(gridDim.x) * kStepBlock) {
-    const double qx = q[3 * i], qy = q[3 * i + 1], qz = q[3 * i + 2];
+    const char* r = q + i * q_stride;
+    double qx, qy, qz;
+    if (q_is_f32) {
+      const float* f = reinterpret_cast<const float*>(r);
+      qx = double(__ldg(f)); qy = double(__ldg(f + 1)); qz = double(__ldg(f + 2));
+    } else {
+      const double* d = reinterpret_cast<const double*>(r);
+      qx = __ldg(d); qy = __ldg(d + 1); qz = __ldg(d + 2);
+    }
     double ww;
     const Rec f = load_rec(model.recs + descend(model, root, qx, qy, qz, ww));
     if (ordinals) ordinals[i] = -1 - f.link;

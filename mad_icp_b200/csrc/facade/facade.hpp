@@ -343,6 +343,14 @@ class MADtreeWrapper {
                                 m.normals[0].data(), want_dist ? m.dists.data() : nullptr), "madicp_search_cloud");
     return m;
   }
+  // the same for n queries in device memory (x, y, z at q + i * stride bytes), written to device outputs, ready on `stream`
+  void searchCloudDev(const void* q, int64_t n, int64_t stride, bool is_f32, double* points, double* normals, double* dists,
+                      void* stream) {
+    if (!tree_) throw Error("MADtree.search: build the tree first");
+    if (n > 0)
+      check(madicp_search_cloud_dev(ctx_, 0, q, n, stride, is_f32 ? 1 : 0, nullptr, points, normals, dists, stream),
+            "madicp_search_cloud_dev");
+  }
 
  private:
   std::unique_ptr<MADtree> tree_;

@@ -19,6 +19,11 @@
 #include "facade.hpp"
 
 namespace madicp_b200 {
+// A scan whose records are device memory (a CUDA tensor, a CuPy array): read in place by the _dev entry points, after the
+// context's stream waits for `stream`, the stream they are written on (0: the legacy default stream)
+struct DevScan {
+  void* stream = nullptr;
+};
 namespace detail {
 
 using madicp_pose::Pose;
@@ -105,6 +110,8 @@ class Lookahead {
     bool records = false;             // raw sensor records (Pipeline::prefetchRecords): `pts` describes them, `vc` is
     madicp_points_t pts{};            // their vertical correction (disabled: none)
     madicp_vcorr_t vc{};
+    bool dev = false;                 // records in device memory, ready on `stream` (DevScan): never staged
+    void* stream = nullptr;
     std::shared_ptr<void> keepalive;
     size_t n = 0;
     madtree_gpu_t* tree = nullptr;
@@ -129,7 +136,8 @@ class Lookahead {
     fifo_.push_back(std::move(j));
     Job& q = fifo_.back();  // (planned where its private copy, if any, will stay)
     const madicp_points_t d = q.records ? q.pts : madicp::packed_points(q.data(), int64_t(q.n), q.is_f32 ? 1 : 0);
-    const int rc = madicp_plan_points(ctx_, &d, q.records ? &q.vc : nullptr, num_threads, &q.plan);
+    const int rc = q.dev ? madicp_plan_points_dev(ctx_, &d, &q.vc, num_threads, q.stream, &q.plan)
+                         : madicp_plan_points(ctx_, &d, q.records ? &q.vc : nullptr, num_threads, &q.plan);
     if (rc < 0) {
       const std::string msg = "madicp_plan_points failed (" + std::to_string(rc) + "): " + madicp_last_error();
       fifo_.pop_back();
@@ -157,9 +165,10 @@ class Lookahead {
 
  private:
   // scans that can share one batch call: packed clouds of one element type, or records (each with its own correction:
-  // the batch call takes one per scan)
+  // the batch call takes one per scan) -- host records, or device records ready on one stream
   static bool sameKind(const Job& a, const Job& b) {
-    return !a.plan && !b.plan && a.records == b.records && (a.records || a.is_f32 == b.is_f32);
+    return !a.plan && !b.plan && a.records == b.records && (a.records || a.is_f32 == b.is_f32) && a.dev == b.dev &&
+           (!a.dev || a.stream == b.stream);
   }
   // Builds the trees of the longest run of queued scans of the front's kind, up to the batch size.  A scan whose tree
   // cannot be built (records the range gate leaves empty) fails the batch call as a whole: the run is then halved until
@@ -185,10 +194,12 @@ class Lookahead {
         vc.push_back(fifo_[i].vc);
       }
       out.assign(k, nullptr);
-      const int rc = front.records
-                         ? madtree_gpu_build_batch_points_ex(ctx_, pts.data(), vc.data(), int(k), b_max_, b_min_, out.data())
-                         : madtree_gpu_build_batch(ctx_, ptr.data(), n.data(), front.is_f32 ? 1 : 0, int(k), b_max_, b_min_,
-                                                   out.data());
+      const int rc =
+          front.dev ? madtree_gpu_build_batch_points_dev(ctx_, pts.data(), vc.data(), int(k), b_max_, b_min_, front.stream,
+                                                         out.data())
+          : front.records ? madtree_gpu_build_batch_points_ex(ctx_, pts.data(), vc.data(), int(k), b_max_, b_min_, out.data())
+                          : madtree_gpu_build_batch(ctx_, ptr.data(), n.data(), front.is_f32 ? 1 : 0, int(k), b_max_, b_min_,
+                                                    out.data());
       if (rc >= 0) break;
       const std::string msg = std::string(front.records ? "madtree_gpu_build_batch_points" : "madtree_gpu_build_batch") +
                               " failed (" + std::to_string(rc) + "): " + madicp_last_error();
@@ -217,7 +228,7 @@ class Lookahead {
   void stageQueued() {
     while (staged_ < size_t(batch_) && built_ + staged_ < fifo_.size()) {
       const Job& j = fifo_[built_ + staged_];
-      if (j.plan || !sameKind(j, fifo_[built_])) break;
+      if (j.plan || j.dev || !sameKind(j, fifo_[built_])) break;
       if (j.records)
         check(madicp_stage_points_ex(ctx_, &j.pts, &j.vc, int64_t(batch_) * int64_t(j.n)), "madicp_stage_points");
       else
@@ -319,15 +330,18 @@ class Pipeline {
   // the same result as compute() on the reader's filtered array -- corrected by `vc` (nullable: none) like KITTI's
   // reader with apply_correction.  MADICP_GPU_BUILD=0: the kept points are packed (and corrected) on the host with the
   // same restatement, then the host path runs.
-  void computeRecords(double stamp, const madicp_points_t& pts, const madicp_vcorr_t* vc = nullptr) {
+  // dev (nullable): the records are device memory, read in place (host-built trees, MADICP_GPU_BUILD=0, need host records:
+  // the caller copies them over first)
+  void computeRecords(double stamp, const madicp_points_t& pts, const madicp_vcorr_t* vc = nullptr, const DevScan* dev = nullptr) {
     check(madicp::check_vcorr(vc, "Pipeline.computeRecords"), "Pipeline.computeRecords");
+    if (dev && !gpu_build_) throw Error("Pipeline.computeRecords: device records need device-built trees (MADICP_GPU_BUILD)");
     if (!gpu_build_) {
       compute(stamp, packRecords(pts, vc));
       return;
     }
     if (!pts.data || pts.n <= 0) throw Error("Pipeline.computeRecords: empty scan");
     const madicp_vcorr_t v = madicp::vcorr_of(vc);
-    computeRaw(stamp, pts.data, size_t(pts.n), pts.is_f32 != 0, &pts, &v);
+    computeRaw(stamp, pts.data, size_t(pts.n), pts.is_f32 != 0, &pts, &v, dev);
   }
   bool gpuBuild() const { return gpu_build_; }
   int lastIcpIterations() const { return last_iters_; }  // rounds the realtime budget allowed for the last scan
@@ -338,8 +352,11 @@ class Pipeline {
   // sorted by azimuth ahead of time; compute() applies the chunk poses and builds its tree (no effect without deskew).
   // keepalive: when given, the buffer is read in place (no copy) and the handle is dropped once compute() has consumed
   // the scan; without it the cloud is copied.
+  // dev (nullable, records only): the records are device memory (DevScan), kept alive until their tree is built or their
+  // plan consumed.
   bool prefetch(const void* xyz, size_t n, bool is_f32, std::shared_ptr<void> keepalive = nullptr,
-                const madicp_points_t* records = nullptr, const madicp_vcorr_t* vc = nullptr, bool deskew_ahead = false) {
+                const madicp_points_t* records = nullptr, const madicp_vcorr_t* vc = nullptr, bool deskew_ahead = false,
+                const DevScan* dev = nullptr) {
     if (!gpu_build_ || (deskew_ && !deskew_ahead) || !xyz || n == 0) return false;
     const auto p0 = clk();
     struct Tick {  // (the hand-over runs on the thread that launches the registrations: its cost is part of the scan's)
@@ -363,6 +380,8 @@ class Pipeline {
       j.records = true;
       j.pts = *records;
       j.vc = madicp::vcorr_of(vc);
+      j.dev = dev != nullptr;
+      j.stream = dev ? dev->stream : nullptr;
     }
     if (keepalive) {
       j.ext = xyz;
@@ -377,15 +396,16 @@ class Pipeline {
     return true;
   }
   bool prefetchRecords(const madicp_points_t& pts, std::shared_ptr<void> keepalive, const madicp_vcorr_t* vc = nullptr,
-                       bool deskew_ahead = false) {
-    return prefetch(pts.data, pts.n > 0 ? size_t(pts.n) : 0, pts.is_f32 != 0, std::move(keepalive), &pts, vc, deskew_ahead);
+                       bool deskew_ahead = false, const DevScan* dev = nullptr) {
+    return prefetch(pts.data, pts.n > 0 ? size_t(pts.n) : 0, pts.is_f32 != 0, std::move(keepalive), &pts, vc, deskew_ahead,
+                    dev);
   }
   size_t prefetched() { return lookahead_ ? lookahead_->size() : 0; }
 
  private:
   // the scan's MAD-tree: ingest (+ deskew, pipeline.cpp:137-138) and build, on the device or on the host
   std::unique_ptr<MADtree> makeTree(const void* xyz, size_t n, bool is_f32, const madicp_points_t* records,
-                                    const madicp_vcorr_t* vc) {
+                                    const madicp_vcorr_t* vc, const DevScan* dev) {
     const bool dsk = deskew_ && is_initialized_ && trajectory_.size() > 1;
     const double* Ta = dsk ? trajectory_[trajectory_.size() - 2].m : nullptr;
     const double* Tb = dsk ? trajectory_[trajectory_.size() - 1].m : nullptr;
@@ -396,6 +416,12 @@ class Pipeline {
     }
     if (lookahead_ && !lookahead_->empty())  // built ahead of time by a worker lane
       return std::unique_ptr<MADtree>(new MADtree(icp_.context(), lookahead_->pop(), b_max_));
+    if (gpu_build_ && records && dev) {
+      check(madicp_ingest_points_dev(icp_.context(), records, vc, dsk ? 1 : 0, Ta, Tb, sensor_hz_,
+                                     std::max(1 << max_parallel_levels_, 1), dev->stream, nullptr, nullptr),
+            "madicp_ingest_points_dev");
+      return std::unique_ptr<MADtree>(new MADtree(icp_.context(), b_max_, b_min_));
+    }
     if (gpu_build_ && records) {
       check(madicp_ingest_points_ex(icp_.context(), records, vc, dsk ? 1 : 0, Ta, Tb, sensor_hz_,
                                     std::max(1 << max_parallel_levels_, 1), nullptr, nullptr), "madicp_ingest_points");
@@ -417,7 +443,7 @@ class Pipeline {
   }
 
   void computeRaw(double stamp, const void* xyz, size_t n, bool is_f32, const madicp_points_t* records = nullptr,
-                  const madicp_vcorr_t* vc = nullptr) {
+                  const madicp_vcorr_t* vc = nullptr, const DevScan* dev = nullptr) {
     if (!xyz || n == 0) throw Error("Pipeline.compute: empty cloud");
     is_map_updated_ = false;
     if (!is_initialized_) {  // pipeline.cpp:267-284
@@ -425,7 +451,7 @@ class Pipeline {
       f->frame = int(seq_);
       f->to_map = frame_to_map_;
       f->stamp = stamp;
-      f->tree = makeTree(xyz, n, is_f32, records, vc);
+      f->tree = makeTree(xyz, n, is_f32, records, vc, dev);
       keyframes_.push_back(f);
       current_ = f;
       trajectory_.push_back(detail::poseIdentity());
@@ -436,7 +462,7 @@ class Pipeline {
     const auto c0 = clk();
     const auto c1 = c0;
     auto cur = std::make_shared<FrameB>();
-    cur->tree = makeTree(xyz, n, is_f32, records, vc);
+    cur->tree = makeTree(xyz, n, is_f32, records, vc, dev);
     const auto c2 = clk();
     double t[3], w[3];
     for (int a = 0; a < 3; ++a) {

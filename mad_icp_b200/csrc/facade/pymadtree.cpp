@@ -36,8 +36,13 @@ PYBIND11_MODULE(pymadtree, m) {
              return out;
            },
            py::arg("query_cloud"))
-      // array form of the same operator (SURVEY 8f next-4): (points N x 3, normals N x 3, dists N)
-      .def("searchCloudArrays", [](mb::MADtreeWrapper& t, const py::object& cloud) {
+      // array form of the same operator (SURVEY 8f next-4): (points N x 3, normals N x 3, dists N); device queries (a CUDA
+      // tensor, a CuPy array) are read in place and answered with float64 torch tensors on their device, ready on the
+      // caller's current stream (records.search_cloud_arrays_dev)
+      .def("searchCloudArrays", [](py::object self, const py::object& cloud) -> py::object {
+        if (py::hasattr(cloud, "__cuda_array_interface__"))
+          return py::module_::import("mad_icp_b200.records").attr("search_cloud_arrays_dev")(self.attr("_searchCloudDev"), cloud);
+        mb::MADtreeWrapper& t = self.cast<mb::MADtreeWrapper&>();
         auto r = t.searchCloud(cloud_arg(cloud), true);
         const size_t n = r.points.size();
         py::array_t<double> P({n, size_t(3)}), N({n, size_t(3)}), D(n);
@@ -47,5 +52,10 @@ PYBIND11_MODULE(pymadtree, m) {
           std::memcpy(D.mutable_data(), r.dists.data(), 8 * n);
         }
         return py::make_tuple(P, N, D);
+      })
+      .def("_searchCloudDev", [](mb::MADtreeWrapper& t, uintptr_t q, int64_t n, int64_t stride, bool is_f32, uintptr_t P,
+                                 uintptr_t N, uintptr_t D, uintptr_t stream) {
+        t.searchCloudDev(reinterpret_cast<const void*>(q), n, stride, is_f32, reinterpret_cast<double*>(P),
+                         reinterpret_cast<double*>(N), reinterpret_cast<double*>(D), reinterpret_cast<void*>(stream));
       });
 }

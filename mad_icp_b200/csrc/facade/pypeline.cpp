@@ -5,12 +5,20 @@
 #include "pipeline.hpp"
 #include "py_common.hpp"
 
-// records (2-D float array with >= 3 columns, or 1-D structured with x/y/z) -> madicp_points_t, by records.layout
+// an object exporting __cuda_array_interface__ (a CUDA tensor, a CuPy array): its records are device memory
+static bool on_device(const py::object& o) { return py::hasattr(o, "__cuda_array_interface__"); }
+// a device array copied to the host once (records.to_host), for host-built trees (MADICP_GPU_BUILD=0)
+static py::object to_host(const py::object& o) { return py::module_::import("mad_icp_b200.records").attr("to_host")(o); }
+
+// records (2-D float array with >= 3 columns, or 1-D structured with x/y/z; host or device memory) -> madicp_points_t, by
+// records.layout; dev receives the producer stream of device records (and is left alone for host records)
 static madicp_points_t records_arg(const py::object& records, double min_range, double max_range, bool inclusive,
-                                   bool drop_nan) {
+                                   bool drop_nan, mb::DevScan* dev = nullptr, bool* is_dev = nullptr) {
   const py::tuple t = py::module_::import("mad_icp_b200.records")
                           .attr("layout")(records, min_range, max_range, inclusive, drop_nan)
                           .cast<py::tuple>();
+  if (is_dev) *is_dev = t[11].cast<bool>();
+  if (dev && t[11].cast<bool>()) dev->stream = reinterpret_cast<void*>(t[12].cast<uintptr_t>());
   madicp_points_t d{};
   d.data = reinterpret_cast<const void*>(t[0].cast<uintptr_t>());
   d.n = t[1].cast<int64_t>();
@@ -54,8 +62,19 @@ PYBIND11_MODULE(pypeline, m) {
       .def("keyframeID", &mb::Pipeline::keyframeID)
       .def("modelLeaves", &mb::Pipeline::modelLeaves)
       .def("currentLeaves", &mb::Pipeline::currentLeaves)
-      .def("compute", [](mb::Pipeline& p, double stamp, const py::object& cloud) {
-        // read the points where they are: a bound VectorEigen3d by reference, a numpy array through its buffer
+      .def("compute", [](mb::Pipeline& p, double stamp, py::object cloud) {
+        // read the points where they are: a bound VectorEigen3d by reference, a numpy array through its buffer, a device
+        // array in place (as records without a gate)
+        if (on_device(cloud)) {
+          if (p.gpuBuild()) {
+            mb::DevScan dev;
+            madicp_points_t d = records_arg(cloud, 0.0, std::numeric_limits<double>::infinity(), true, false, &dev);
+            d.range_mode = MADICP_RANGE_NONE;
+            p.computeRecords(stamp, d, nullptr, &dev);
+            return;
+          }
+          cloud = to_host(cloud);
+        }
         if (py::isinstance<mb::ContainerType>(cloud)) {
           const mb::ContainerType& v = cloud.cast<const mb::ContainerType&>();
           p.compute(stamp, v.empty() ? nullptr : v[0].data(), v.size());
@@ -81,6 +100,13 @@ PYBIND11_MODULE(pypeline, m) {
           py::object* ref = new py::object(o);
           return std::shared_ptr<void>(ref, [](void* q) { delete static_cast<py::object*>(q); });
         };
+        if (on_device(cloud)) {  // (host-built trees: no look-ahead, as for host arrays)
+          if (!p.gpuBuild()) return false;
+          mb::DevScan dev;
+          madicp_points_t d = records_arg(cloud, 0.0, std::numeric_limits<double>::infinity(), true, false, &dev);
+          d.range_mode = MADICP_RANGE_NONE;
+          return p.prefetchRecords(d, hold(cloud), nullptr, deskew_ahead, &dev);
+        }
         if (py::isinstance<mb::ContainerType>(cloud)) {
           const mb::ContainerType& v = cloud.cast<const mb::ContainerType&>();
           return p.prefetch(v.empty() ? nullptr : v[0].data(), v.size(), false, hold(cloud), nullptr, nullptr, deskew_ahead);
@@ -100,7 +126,11 @@ PYBIND11_MODULE(pypeline, m) {
       .def("computeRecords", [](mb::Pipeline& p, double stamp, const py::object& records, double min_range, double max_range,
                                 bool inclusive, bool drop_nan, bool apply_correction, double vertical_angle_offset) {
         const madicp_vcorr_t v = vcorr_arg(apply_correction, vertical_angle_offset);
-        p.computeRecords(stamp, records_arg(records, min_range, max_range, inclusive, drop_nan), &v);
+        const py::object recs = (on_device(records) && !p.gpuBuild()) ? to_host(records) : records;
+        mb::DevScan dev;
+        bool is_dev = false;
+        const madicp_points_t d = records_arg(recs, min_range, max_range, inclusive, drop_nan, &dev, &is_dev);
+        p.computeRecords(stamp, d, &v, is_dev ? &dev : nullptr);
       }, py::arg("stamp"), py::arg("records"), py::arg("min_range") = 0.0,
          py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false,
          py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle)
@@ -109,11 +139,14 @@ PYBIND11_MODULE(pypeline, m) {
       .def("prefetchRecords", [](mb::Pipeline& p, const py::object& records, double min_range, double max_range,
                                  bool inclusive, bool drop_nan, bool apply_correction, double vertical_angle_offset,
                                  bool deskew_ahead) {
-        const madicp_points_t d = records_arg(records, min_range, max_range, inclusive, drop_nan);
+        if (on_device(records) && !p.gpuBuild()) return false;  // (host-built trees: no look-ahead)
+        mb::DevScan dev;
+        bool is_dev = false;
+        const madicp_points_t d = records_arg(records, min_range, max_range, inclusive, drop_nan, &dev, &is_dev);
         const madicp_vcorr_t v = vcorr_arg(apply_correction, vertical_angle_offset);
         py::object* ref = new py::object(records);  // dropped once the scan's tree is built (see prefetch)
         return p.prefetchRecords(d, std::shared_ptr<void>(ref, [](void* q) { delete static_cast<py::object*>(q); }), &v,
-                                 deskew_ahead);
+                                 deskew_ahead, is_dev ? &dev : nullptr);
       }, py::arg("records"), py::arg("min_range") = 0.0,
          py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false,
          py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle, py::arg("deskew_ahead") = false)

@@ -98,6 +98,7 @@ struct BuildState {
   int32_t* h_perm = nullptr;
   uint16_t* h_chunk = nullptr;
   double* h_poses = nullptr;
+  double* h_packed = nullptr;  // pinned, 3 x cap, at first use: a deskewed device scan's kept points for the host's order
   double* h_root = nullptr;  // pinned: the root's sums when the host computes them
   double root_S[9];          // ... of the cloud madicp_ingest left in P[0] (valid when has_root_S)
   bool has_root_S = false;
@@ -680,19 +681,21 @@ int vtab_slot(BuildState* bs, cudaStream_t st, const madicp_vcorr_t& vc, int* sl
   *slot = k;
   return MADICP_OK;
 }
-// layout of one scan for the device (RecSrc, gpu_tree_kernels.cuh); raw: its byte offset in d_raw, first: its first
-// record, vc: its correction's table slot (vtab_slot)
-RecSrc rec_src(const madicp_points_t& d, size_t raw, int first, int vc) {
+// layout of one scan for the device (RecSrc, gpu_tree_kernels.cuh); base: its first record on the device (in d_raw, a
+// plan's buffer or the caller's memory), first: its first record in the batch, vc: its correction's table slot
+// (vtab_slot)
+RecSrc rec_src(const madicp_points_t& d, const void* base, int first, int vc) {
   RecSrc s{};
   s.vc = (signed char) vc;
-  s.raw = (long long) raw;
+  s.base = static_cast<const char*>(base);
   s.first = first;
   s.stride = int(d.stride);
   const int e = d.is_f32 ? 4 : 8;
   const int lo = std::min(d.offset[0], std::min(d.offset[1], d.offset[2]));
   const int hi = std::max(d.offset[0], std::max(d.offset[1], d.offset[2])) + e;
   const int vbase = lo & ~15;
-  s.vec = (d.stride % 16 == 0) ? (hi - vbase <= 16 ? 1 : (hi - vbase <= 32 ? 2 : 0)) : 0;
+  const bool aligned = reinterpret_cast<uintptr_t>(base) % 16 == 0 && d.stride % 16 == 0;  // (a view of a tensor may not be)
+  s.vec = aligned ? (hi - vbase <= 16 ? 1 : (hi - vbase <= 32 ? 2 : 0)) : 0;
   s.vbase = s.vec ? vbase : 0;
   for (int c = 0; c < 3; ++c) s.off[c] = d.offset[c] - s.vbase;
   s.is_f32 = d.is_f32 ? 1 : 0;
@@ -702,25 +705,28 @@ RecSrc rec_src(const madicp_points_t& d, size_t raw, int first, int vc) {
   s.hi = d.is_f32 ? double(float(d.max_range)) : d.max_range;
   return s;
 }
-// Order-preserving compaction of the gated records of B (in `raw`: d_raw or a plan's copy) into P[0]; the kept count of
-// every scan goes to bs->h_kept.  vc: some scan of B is corrected.
-int launch_compaction(madicp_ctx* c, BuildState* bs, cudaStream_t st, const RecBatch& B, const char* raw, bool vc) {
+// Order-preserving compaction of the gated records of B into `out` (packed float64; bs->P[0] unless a deskew or a plan
+// needs the kept points elsewhere); the kept count of every scan goes to kept[] and a correction outside its table raises
+// *vc_err (both mapped host memory).  vc: some scan of B is corrected.
+int launch_compaction(madicp_ctx* c, BuildState* bs, cudaStream_t st, const RecBatch& B, double* out, int* kept, int* vc_err,
+                      bool vc) {
   const int tiles = (B.n_rec + kTile - 1) / kTile;
-  k_gate_flags<<<blocks(B.n_rec), kBlock, 0, st>>>(B, raw, bs->flag);
+  k_gate_flags<<<blocks(B.n_rec), kBlock, 0, st>>>(B, bs->flag);
   k_scan_tiles<<<tiles, kTile, 0, st>>>(bs->flag, B.n_rec, bs->G, bs->tile);
   k_scan_tile_sums<<<1, 1024, 0, st>>>(bs->tile, tiles);
   auto k = vc ? k_compact<true> : k_compact<false>;
-  k<<<blocks(std::max(B.n_rec, B.count)), kBlock, 0, st>>>(B, raw, bs->flag, bs->G, bs->tile, bs->P[0], bs->h_kept, bs->d_vtab,
-                                                           bs->h_vc_err);
+  k<<<blocks(std::max(B.n_rec, B.count)), kBlock, 0, st>>>(B, bs->flag, bs->G, bs->tile, out, kept, bs->d_vtab, vc_err);
   c->launches += 4;
   CK(cudaGetLastError());
   return MADICP_OK;
 }
 
-// The batch build behind madtree_gpu_build_batch and madtree_gpu_build_batch_points[_ex] (descriptors and corrections
-// validated; vcorrs nullable).
+// The batch build behind madtree_gpu_build_batch and madtree_gpu_build_batch_points[_ex|_dev] (descriptors and
+// corrections validated; vcorrs nullable).  dev: the scans are in device memory (the context's stream already waits for
+// their producer) and are read in place; the host cannot count or sum them, so the device's kept counts are read back
+// after the compaction and the roots are summed on the device.
 int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* vcorrs, int count, double b_max, double b_min,
-                madtree_gpu** out, const char* fn) {
+                madtree_gpu** out, const char* fn, bool dev = false) {
   bool direct = true, gated = false, corrected = false;
   madicp_vcorr_t vc[kMaxBatch];
   int first[kMaxBatch + 1];
@@ -743,7 +749,7 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* v
   CK(cudaSetDevice(c->device));
   BuildState* bs = static_cast<BuildState*>(c->build_state);
   cudaStream_t st = c->stream;
-  const size_t raw_bytes = direct ? 0 : raw_off[count];
+  const size_t raw_bytes = (direct || dev) ? 0 : raw_off[count];
   if (bs && (bs->cap < size_t(n_rec) || bs->raw_cap < raw_bytes)) {  // the lane is about to be re-allocated: early uploads are lost
     int e = drop_staged(bs, st);
     if (e) return e;
@@ -753,7 +759,7 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* v
   const auto ta0 = std::chrono::steady_clock::now();
   // scans uploaded ahead of time (madicp_stage_cloud / _points): the longest prefix of this batch staged in this order
   int n_staged = 0;
-  if (!bs->staged.empty() && bs->staged_raw == !direct)
+  if (!dev && !bs->staged.empty() && bs->staged_raw == !direct)
     while (n_staged < count && n_staged < int(bs->staged.size()) && same_points(bs->staged[size_t(n_staged)].d, bs->staged[size_t(n_staged)].vc, d[n_staged], vc[n_staged]))
       ++n_staged;
   std::vector<std::shared_future<RootSums>> early;
@@ -762,8 +768,10 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* v
   if (rc) return rc;
   char* raw = static_cast<char*>(bs->d_raw);
   for (int b = n_staged; b < count; ++b) {
-    if (direct) CK(cudaMemcpyAsync(bs->P[0] + size_t(first[b]) * 3, d[b].data, size_t(d[b].n) * 24, cudaMemcpyHostToDevice, st));
-    else CK(cudaMemcpyAsync(raw + raw_off[b], d[b].data, points_bytes(d[b]), cudaMemcpyHostToDevice, st));
+    if (direct)
+      CK(cudaMemcpyAsync(bs->P[0] + size_t(first[b]) * 3, d[b].data, size_t(d[b].n) * 24,
+                         dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+    else if (!dev) CK(cudaMemcpyAsync(raw + raw_off[b], d[b].data, points_bytes(d[b]), cudaMemcpyHostToDevice, st));
   }
   bs->n_resident = 0;  // the concatenated clouds are not "the resident cloud" of madtree_gpu_build_resident
   bs->has_root_S = false;
@@ -778,22 +786,26 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* v
     for (int b = 0; b < count; ++b) {
       int slot = -1;
       if (int e = vtab_slot(bs, st, vc[b], &slot)) return e;
-      B.s[b] = rec_src(d[b], raw_off[b], first[b], slot);
+      B.s[b] = rec_src(d[b], dev ? d[b].data : raw + raw_off[b], first[b], slot);
     }
-    if (gated) {
-      if (int e = launch_compaction(c, bs, st, B, raw, corrected)) return e;
+    if (gated || dev) {
+      if (int e = launch_compaction(c, bs, st, B, bs->P[0], bs->h_kept, bs->h_vc_err, corrected)) return e;
     } else {
       auto k = corrected ? k_ingest<true> : k_ingest<false>;
-      k<<<blocks(n_rec), kBlock, 0, st>>>(B, raw, nullptr, nullptr, bs->d_poses, n_rec, bs->P[0], bs->d_vtab, bs->h_vc_err);
+      k<<<blocks(n_rec), kBlock, 0, st>>>(B, nullptr, nullptr, bs->d_poses, n_rec, bs->P[0], bs->d_vtab, bs->h_vc_err);
       c->launches++;
     }
   }
   const auto ta1 = std::chrono::steady_clock::now();
   // the roots' sums and the kept counts on the host, one scan per host thread, while the scans are being copied up; a
-  // batch holding a corrected scan has its roots summed on the device (root_host)
+  // batch holding a corrected scan has its roots summed on the device (root_host), and so has a batch of device scans,
+  // whose kept counts are the compaction's
   std::vector<double> S(size_t(count) * 9);
   std::vector<int64_t> kept(static_cast<size_t>(count));
-  if (count > n_staged) madicp_host_for(count - n_staged, bs->threads, [&](int k) {
+  if (dev) {
+    if (!direct) CK(cudaStreamSynchronize(st));
+    for (int b = 0; b < count; ++b) kept[size_t(b)] = direct ? d[b].n : bs->h_kept[b];
+  } else if (count > n_staged) madicp_host_for(count - n_staged, bs->threads, [&](int k) {
     const int b = n_staged + k;
     kept[size_t(b)] = root_host(d[b], vc[b], S.data() + size_t(b) * 9);
   });
@@ -812,7 +824,8 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* v
     offs[b + 1] = offs[b] + int(kept[size_t(b)]);
   }
   const auto tb0 = std::chrono::steady_clock::now();
-  rc = build_forest(c, bs, st, count, offs, b_max, b_min, corrected ? nullptr : S.data(), gated ? count : 0, out);
+  rc = build_forest(c, bs, st, count, offs, b_max, b_min, (corrected || dev) ? nullptr : S.data(), (gated && !dev) ? count : 0,
+                    out);
   if (getenv("MADICP_BUILD_TIMING"))
     fprintf(stderr, "%s: %d scans (%d staged), copies enqueued %.0f us, roots' sums on the host %.0f us, forest build %.0f us\n",
             fn, count, n_staged, std::chrono::duration<double, std::micro>(ta1 - ta0).count(),
@@ -881,17 +894,26 @@ struct PlanBuf {
   uint16_t* h_chunk = nullptr;
   cudaEvent_t ready = nullptr;    // lane stream: records, perm and chunk are on the device
   cudaEvent_t free_ev = nullptr;  // context stream: the last ingest that read the device buffers has run
+  // a plan of device records (madicp_plan_points_dev): d_raw holds its kept points, compacted and corrected as packed
+  // float64 on the context's stream; the order half reads them back
+  int* h_cnt = nullptr;              // mapped: [0] kept points, [1] a correction fell outside its table
+  double* h_pts = nullptr;           // pinned, 3 x cap, at first use: the kept points for the order half
+  cudaEvent_t compacted = nullptr;   // context stream: the compaction has run
 };
 void free_buf(PlanBuf* b) {
   if (b->ready) cudaEventSynchronize(b->ready);
   if (b->free_ev) cudaEventSynchronize(b->free_ev);
+  if (b->compacted) cudaEventSynchronize(b->compacted);
   cudaFree(b->d_raw);
   cudaFree(b->d_perm);
   cudaFree(b->d_chunk);
   cudaFreeHost(b->h_perm);
   cudaFreeHost(b->h_chunk);
+  cudaFreeHost(b->h_cnt);
+  cudaFreeHost(b->h_pts);
   if (b->ready) cudaEventDestroy(b->ready);
   if (b->free_ev) cudaEventDestroy(b->free_ev);
+  if (b->compacted) cudaEventDestroy(b->compacted);
   delete b;
 }
 
@@ -1001,6 +1023,8 @@ int plan_buf(PlanLane* L, size_t n, size_t bytes, PlanBuf** out) {
   if (e == cudaSuccess) e = cudaHostAlloc(&b->h_chunk, b->cap * sizeof(uint16_t), 0);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->ready, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->free_ev, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaHostAlloc(&b->h_cnt, 2 * sizeof(int), cudaHostAllocMapped);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->compacted, cudaEventDisableTiming);
   if (e != cudaSuccess) {
     free_buf(b);
     set_error(std::string("madicp_plan_points: ") + cudaGetErrorString(e));
@@ -1021,6 +1045,7 @@ struct madicp_plan {
   PlanLane* lane = nullptr;
   madicp_points_t d{};
   madicp_vcorr_t vc{};
+  bool dev = false;  // device records: buf->d_raw holds the kept points (PlanBuf)
   PlanBuf* buf = nullptr;
   std::promise<void> done_p;
   std::future<void> done;  // the order half has run and its uploads are queued
@@ -1048,7 +1073,21 @@ void plan_order(madicp_plan* p) {
   };
   cuda(cudaSetDevice(p->lane->device), "cudaSetDevice");
   cuda(cudaEventSynchronize(b->ready), "cudaEventSynchronize");  // the buffer's last uploads from h_perm / h_chunk have run
-  if (!rc) {
+  if (p->dev) {  // the kept points, gated and corrected on the device, come back for the order: a packed, plain cloud
+    cuda(cudaEventSynchronize(b->compacted), "cudaEventSynchronize");
+    if (!rc && b->h_cnt[1]) rc = MADICP_ERR_STATE;
+    if (!rc) p->kept = b->h_cnt[0];
+    if (!rc && p->kept > 0) {
+      if (!b->h_pts) cuda(cudaHostAlloc(&b->h_pts, b->cap * 3 * sizeof(double), 0), "cudaHostAlloc");
+      if (!rc) cuda(cudaMemcpyAsync(b->h_pts, b->d_raw, size_t(p->kept) * 24, cudaMemcpyDeviceToHost, st), "kept points");
+      if (!rc) cuda(cudaEventRecord(b->ready, st), "cudaEventRecord");
+      if (!rc) cuda(cudaEventSynchronize(b->ready), "cudaEventSynchronize");
+      int64_t kept = 0;
+      if (!rc) rc = madicp_deskew_order(packed_points(b->h_pts, p->kept, 0), nullptr, 1, b->h_perm, b->h_chunk, &p->n_chunks,
+                                        &kept);
+      if (rc && rc != MADICP_ERR_CUDA) err = madicp_last_error();
+    }
+  } else if (!rc) {
     VcorrTable table;
     rc = madicp_deskew_order(p->d, vcorr_table(p->vc, &table), 1, b->h_perm, b->h_chunk, &p->n_chunks, &p->kept);
     if (rc && rc != MADICP_ERR_STATE) err = madicp_last_error();
@@ -1089,11 +1128,129 @@ int stage_chunk_poses(PlanLane* L, cudaStream_t st, const double T_prev[12], con
   return MADICP_OK;
 }
 
+// the `kept` packed float64 points at `pts` (device memory) as a one-scan batch for k_ingest: no gate, no correction
+RecBatch packed_batch(const double* pts, int64_t kept) {
+  RecBatch B;
+  B.count = 1;
+  B.n_rec = int(kept);
+  B.s[0] = rec_src(packed_points(pts, kept, 0), pts, 0, -1);
+  return B;
+}
+
+// The end of an ingest: the cloud of `kept` points in P[0] is the resident one (its root summed on the device), and
+// n_kept / points_out (host memory, synchronises) receive it.
+int ingest_done(BuildState* bs, cudaStream_t st, int64_t kept, int64_t* n_kept, double* points_out) {
+  CK(cudaGetLastError());
+  bs->n_resident = kept;
+  bs->has_root_S = false;
+  if (n_kept) *n_kept = kept;
+  if (points_out) {
+    CK(cudaMemcpyAsync(points_out, bs->P[0], size_t(kept) * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
+  return MADICP_OK;
+}
+
+// The ingest behind madicp_ingest_points_dev (descriptor, correction and device pointer validated; the context's stream
+// already waits for the producer).  The records are read in place: the gate, the correction and the compaction run as
+// for uploaded records, and the kept count comes back from the device (one synchronisation).  deskew: the kept points
+// are compacted into P[1], copied back for the host's order half (madicp_deskew_plan over a packed, plain cloud -- the
+// same points, so the same permutation and chunks), and gathered from there into P[0].
+int ingest_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int deskew, const double T_prev[12],
+               const double T_now[12], double sensor_hz, int num_threads, int64_t* n_kept, double* points_out,
+               const char* fn) {
+  BuildState* bs = nullptr;
+  int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
+  if (!rc) rc = ensure_state(c, size_t(d.n), 0, &bs);
+  if (rc) return rc;
+  cudaStream_t st = c->stream;
+  bs->n_resident = 0;
+  bs->kept_check = 0;
+  bs->vc_check = false;  // (an angle outside the table fails this call)
+  int64_t kept = d.n;
+  if (is_direct(d, vc) && !deskew) {
+    CK(cudaMemcpyAsync(bs->P[0], d.data, size_t(d.n) * 24, cudaMemcpyDeviceToDevice, st));
+  } else {
+    int slot = -1;
+    if (vc.enabled) CK(cudaMemsetAsync(bs->h_vc_err, 0, sizeof(int), st));
+    if (int e = vtab_room(bs, st, &vc, 1)) return e;
+    if (int e = vtab_slot(bs, st, vc, &slot)) return e;
+    RecBatch B;
+    B.count = 1;
+    B.n_rec = int(d.n);
+    B.s[0] = rec_src(d, d.data, 0, slot);
+    if (int e = launch_compaction(c, bs, st, B, deskew ? bs->P[1] : bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) return e;
+    CK(cudaStreamSynchronize(st));
+    if (vc.enabled && *bs->h_vc_err) {
+      set_error(vcorr_out_of_table(fn, vc.angle));
+      return MADICP_ERR_STATE;
+    }
+    kept = bs->h_kept[0];
+  }
+  if (kept == 0) {
+    set_error(std::string(fn) + ": no point inside the range gate");
+    return MADICP_ERR_INVALID;
+  }
+  if (deskew) {
+    if (!bs->h_packed)
+      if (int e = host_alloc(bs, &bs->h_packed, 3 * bs->cap)) return e;
+    CK(cudaMemcpyAsync(bs->h_packed, bs->P[1], size_t(kept) * 24, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    int n_poses = 0;
+    int64_t n_sorted = 0;
+    rc = madicp_deskew_plan(packed_points(bs->h_packed, kept, 0), nullptr, T_prev, T_now, sensor_hz, num_threads, bs->h_perm,
+                            bs->h_chunk, bs->h_poses, &n_poses, &n_sorted);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(bs->d_perm, bs->h_perm, size_t(kept) * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(bs->d_chunk, bs->h_chunk, size_t(kept) * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(bs->d_poses, bs->h_poses, size_t(n_poses) * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
+    k_ingest<false><<<blocks(kept), kBlock, 0, st>>>(packed_batch(bs->P[1], kept), bs->d_perm, bs->d_chunk, bs->d_poses,
+                                                     int(kept), bs->P[0], bs->d_vtab, bs->h_vc_err);
+    c->launches++;
+  }
+  return ingest_done(bs, st, kept, n_kept, points_out);
+}
+
+// madicp_ingest_plan of a plan of device records: its kept points (and, deskewing, their order) are on the device.
+int ingest_planned_dev(madicp_ctx* c, madicp_plan* plan, int deskew, const double T_prev[12], const double T_now[12],
+                       double sensor_hz, int64_t* n_kept, double* points_out, const char* fn) {
+  CK(cudaSetDevice(c->device));
+  if (plan->rc == MADICP_ERR_STATE) set_error(vcorr_out_of_table(fn, plan->vc.angle));
+  else if (plan->rc) set_error(plan->err);
+  if (plan->rc) return plan->rc;
+  if (plan->kept == 0) {
+    set_error(std::string(fn) + ": no point inside the range gate");
+    return MADICP_ERR_INVALID;
+  }
+  BuildState* bs = nullptr;
+  int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
+  if (!rc) rc = ensure_state(c, size_t(plan->d.n), 0, &bs);
+  if (rc) return rc;
+  cudaStream_t st = c->stream;
+  bs->n_resident = 0;
+  bs->kept_check = 0;
+  bs->vc_check = false;
+  const int64_t kept = plan->kept;
+  const double* pts = reinterpret_cast<const double*>(plan->buf->d_raw);
+  CK(cudaStreamWaitEvent(st, plan->buf->ready, 0));
+  if (deskew) {
+    if (int e = stage_chunk_poses(plan->lane, st, T_prev, T_now, sensor_hz, plan->n_chunks, bs->d_poses)) return e;
+    k_ingest<false><<<blocks(kept), kBlock, 0, st>>>(packed_batch(pts, kept), plan->buf->d_perm, plan->buf->d_chunk,
+                                                     bs->d_poses, int(kept), bs->P[0], bs->d_vtab, bs->h_vc_err);
+    c->launches++;
+  } else {
+    CK(cudaMemcpyAsync(bs->P[0], pts, size_t(kept) * 24, cudaMemcpyDeviceToDevice, st));
+  }
+  CK(cudaEventRecord(plan->buf->free_ev, st));  // (the plan's buffers may be reused once this has run)
+  return ingest_done(bs, st, kept, n_kept, points_out);
+}
+
 // The ingest behind madicp_ingest, madicp_ingest_points[_ex] and madicp_ingest_plan (descriptor and correction
 // validated).  plan (nullable): the scan's records are already on their way up, with its deskew order (madicp_plan_points).
 int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int deskew, const double T_prev[12],
            const double T_now[12], double sensor_hz, int num_threads, madicp_plan* plan, int64_t* n_kept, double* points_out,
            const char* fn) {
+  if (plan && plan->dev) return ingest_planned_dev(c, plan, deskew, T_prev, T_now, sensor_hz, n_kept, points_out, fn);
   CK(cudaSetDevice(c->device));
   BuildState* bs = nullptr;
   const int64_t n = d.n;
@@ -1119,7 +1276,7 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
   RecBatch B;
   B.count = 1;
   B.n_rec = int(n);
-  B.s[0] = rec_src(d, 0, 0, slot);
+  B.s[0] = rec_src(d, raw, 0, slot);
   int64_t kept = n;
   if (deskew && plan) {  // only the chunk poses are left
     if (plan->rc == MADICP_ERR_STATE) set_error(vcorr_out_of_table(fn, vc.angle));
@@ -1129,7 +1286,7 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
     if (kept > 0) {
       if (int e = stage_chunk_poses(plan->lane, st, T_prev, T_now, sensor_hz, plan->n_chunks, bs->d_poses)) return e;
       auto k = vc.enabled ? k_ingest<true> : k_ingest<false>;
-      k<<<blocks(kept), kBlock, 0, st>>>(B, raw, plan->buf->d_perm, plan->buf->d_chunk, bs->d_poses, int(kept), bs->P[0],
+      k<<<blocks(kept), kBlock, 0, st>>>(B, plan->buf->d_perm, plan->buf->d_chunk, bs->d_poses, int(kept), bs->P[0],
                                          bs->d_vtab, bs->h_vc_err);
       c->launches++;
     }
@@ -1146,17 +1303,17 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
       CK(cudaMemcpyAsync(bs->d_chunk, bs->h_chunk, size_t(kept) * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
       CK(cudaMemcpyAsync(bs->d_poses, bs->h_poses, size_t(n_poses) * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
       auto k = vc.enabled ? k_ingest<true> : k_ingest<false>;
-      k<<<blocks(kept), kBlock, 0, st>>>(B, raw, bs->d_perm, bs->d_chunk, bs->d_poses, int(kept), bs->P[0], bs->d_vtab,
+      k<<<blocks(kept), kBlock, 0, st>>>(B, bs->d_perm, bs->d_chunk, bs->d_poses, int(kept), bs->P[0], bs->d_vtab,
                                          bs->h_vc_err);
       c->launches++;
     }
   } else if (points_gated(d)) {
-    if (int e = launch_compaction(c, bs, st, B, raw, vc.enabled)) return e;
+    if (int e = launch_compaction(c, bs, st, B, bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) return e;
     kept = root_host(d, vc, bs->root_S);
     bs->kept_check = 1;
   } else {
     auto k = vc.enabled ? k_ingest<true> : k_ingest<false>;
-    k<<<blocks(n), kBlock, 0, st>>>(B, raw, nullptr, nullptr, bs->d_poses, int(n), bs->P[0], bs->d_vtab, bs->h_vc_err);
+    k<<<blocks(n), kBlock, 0, st>>>(B, nullptr, nullptr, bs->d_poses, int(n), bs->P[0], bs->d_vtab, bs->h_vc_err);
     c->launches++;
     kept = root_host(d, vc, bs->root_S);
   }
@@ -1238,6 +1395,27 @@ int madtree_gpu_build_batch_points(madicp_ctx_t* c, const madicp_points_t* descs
 int madtree_gpu_build_batch_points_ex(madicp_ctx_t* c, const madicp_points_t* descs, const madicp_vcorr_t* vcorrs, int count,
                                       double b_max, double b_min, madtree_gpu_t** out) {
   return build_batch_points(c, descs, vcorrs, count, b_max, b_min, out, "madtree_gpu_build_batch_points");
+}
+
+int madtree_gpu_build_batch_points_dev(madicp_ctx_t* c, const madicp_points_t* descs, const madicp_vcorr_t* vcorrs,
+                                       int count, double b_max, double b_min, void* producer_stream, madtree_gpu_t** out) {
+  const char* fn = "madtree_gpu_build_batch_points_dev";
+  if (!c || !descs || !out || count < 1 || count > kMaxBatch) {
+    set_error(std::string(fn) + ": bad arguments (1..64 scans)");
+    return MADICP_ERR_INVALID;
+  }
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  for (int b = 0; b < count; ++b) {
+    if (int e = check_points(descs + b, fn)) return e;
+    if (int e = check_vcorr(vcorrs ? vcorrs + b : nullptr, fn)) return e;
+    if (int e = madicp_check_device_ptr(c, descs[b].data, descs[b].is_f32 ? 4 : 8, fn)) return e;
+  }
+  if (int e = madicp_stream_wait(c, c->stream, producer_stream)) return e;
+  const int rc = build_batch(c, descs, vcorrs, count, b_max, b_min, out, fn, true);
+  if (rc) cudaStreamSynchronize(c->stream);  // (a failed call, too, returns once nothing reads the caller's records)
+  return rc;
+  MADICP_CATCH(fn)
 }
 
 int madicp_stage_cloud(madicp_ctx_t* c, const void* cloud, int64_t n, int is_f32, int64_t reserve_points) {
@@ -1372,6 +1550,26 @@ int madicp_ingest_points(madicp_ctx_t* c, const madicp_points_t* desc, int deske
   return madicp_ingest_points_ex(c, desc, nullptr, deskew, T_prev, T_now, sensor_hz, num_threads, n_kept, points_out);
 }
 
+int madicp_ingest_points_dev(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int deskew,
+                             const double T_prev[12], const double T_now[12], double sensor_hz, int num_threads,
+                             void* producer_stream, int64_t* n_kept, double* points_out) {
+  const char* fn = "madicp_ingest_points_dev";
+  if (!c || (deskew && (!T_prev || !T_now || !(sensor_hz > 0.0)))) {
+    set_error(std::string(fn) + ": bad arguments");
+    return MADICP_ERR_INVALID;
+  }
+  if (int e = check_points(desc, fn)) return e;
+  if (int e = check_vcorr(vcorr, fn)) return e;
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  if (int e = madicp_check_device_ptr(c, desc->data, desc->is_f32 ? 4 : 8, fn)) return e;
+  if (int e = madicp_stream_wait(c, c->stream, producer_stream)) return e;
+  const int rc = ingest_dev(c, *desc, vcorr_of(vcorr), deskew, T_prev, T_now, sensor_hz, num_threads, n_kept, points_out, fn);
+  CK(cudaStreamSynchronize(c->stream));  // returns once nothing reads the caller's records, whatever the outcome
+  return rc;
+  MADICP_CATCH(fn)
+}
+
 int madicp_plan_points(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int num_threads,
                        madicp_plan_t** out) {
   if (!c || !out) {
@@ -1407,6 +1605,68 @@ int madicp_plan_points(madicp_ctx_t* c, const madicp_points_t* desc, const madic
   *out = p.release();
   return MADICP_OK;
   MADICP_CATCH("madicp_plan_points")
+}
+
+namespace {
+// The device half of madicp_plan_points_dev, on the context's stream (whose build lane holds the scan scratch the
+// compaction needs): the scan's kept points, gated and corrected, into the plan buffer b as packed float64; b->compacted
+// follows.
+int plan_compact_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, void* producer, PlanBuf* b) {
+  BuildState* bs = static_cast<BuildState*>(c->build_state);
+  if (bs && bs->cap < size_t(d.n))  // the lane is about to be re-allocated: early uploads are lost
+    if (int e = drop_staged(bs, c->stream)) return e;
+  if (int e = ensure_state(c, size_t(d.n), 0, &bs)) return e;
+  cudaStream_t st = c->stream;
+  if (int e = madicp_stream_wait(c, st, producer)) return e;
+  int slot = -1;
+  if (int e = vtab_room(bs, st, &vc, 1)) return e;
+  if (int e = vtab_slot(bs, st, vc, &slot)) return e;
+  b->h_cnt[0] = b->h_cnt[1] = 0;  // (the buffer's last order half has read them)
+  RecBatch B;
+  B.count = 1;
+  B.n_rec = int(d.n);
+  B.s[0] = rec_src(d, d.data, 0, slot);
+  if (int e = launch_compaction(c, bs, st, B, reinterpret_cast<double*>(b->d_raw), b->h_cnt, b->h_cnt + 1, vc.enabled)) return e;
+  CK(cudaEventRecord(b->compacted, st));
+  return MADICP_OK;
+}
+}  // namespace
+
+int madicp_plan_points_dev(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int num_threads,
+                           void* producer_stream, madicp_plan_t** out) {
+  const char* fn = "madicp_plan_points_dev";
+  if (!c || !out) {
+    set_error(std::string(fn) + ": bad arguments");
+    return MADICP_ERR_INVALID;
+  }
+  *out = nullptr;
+  if (int e = check_points(desc, fn)) return e;
+  if (int e = check_vcorr(vcorr, fn)) return e;
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  if (int e = madicp_check_device_ptr(c, desc->data, desc->is_f32 ? 4 : 8, fn)) return e;
+  PlanLane* L = nullptr;
+  if (int e = plan_lane(c, &L)) return e;
+  PlanBuf* b = nullptr;
+  if (int e = plan_buf(L, size_t(desc->n), size_t(desc->n) * 24, &b)) return e;
+  std::unique_ptr<madicp_plan> p(new madicp_plan);
+  p->ctx = c;
+  p->lane = L;
+  p->d = *desc;
+  p->vc = vcorr_of(vcorr);
+  p->dev = true;
+  p->buf = b;
+  p->done = p->done_p.get_future();
+  if (int e = plan_compact_dev(c, *desc, p->vc, producer_stream, b)) {
+    cudaStreamSynchronize(c->stream);  // (nothing may still read the caller's records, nor write the buffer)
+    return_buf(L, b);
+    return e;
+  }
+  madicp_plan* q = p.get();
+  L->submit(std::max(1, std::min(num_threads, 64)), [q]() { plan_order(q); });
+  *out = p.release();
+  return MADICP_OK;
+  MADICP_CATCH(fn)
 }
 
 int madicp_ingest_plan(madicp_ctx_t* c, madicp_plan_t* plan, int deskew, const double T_prev[12], const double T_now[12],

@@ -844,13 +844,14 @@ k_records(Nodes N, int n_nodes, int n_points, const int* __restrict__ G, const i
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Raw records (madicp_points_t) as uploaded: the scans of a batch lie in the raw buffer one after the other, each
-// starting on a 16-byte boundary.  Their layouts travel as a __grid_constant__ kernel parameter (no copy, no host
-// buffer that a later call could overwrite while a copy is pending).  A record is read with the widest aligned loads
-// its stride allows: when the stride is a multiple of 16 and x, y, z lie within one (two) aligned 16-byte chunk(s),
-// one (two) 128-bit load(s) -- one per KITTI record, one per 48-byte Ouster record -- else one load per field.
+// Raw records (madicp_points_t), read where they lie: a scan uploaded from the host sits in the raw buffer on a 16-byte
+// boundary, a scan that already was on the device (the _dev entry points) is read in the caller's memory.  Their
+// layouts travel as a __grid_constant__ kernel parameter (no copy, no host buffer that a later call could overwrite
+// while a copy is pending).  A record is read with the widest aligned loads its base and stride allow: when the base
+// is 16-byte aligned, the stride a multiple of 16 and x, y, z lie within one (two) aligned 16-byte chunk(s), one (two)
+// 128-bit load(s) -- one per KITTI record, one per 48-byte Ouster record -- else one load per field.
 struct RecSrc {
-  long long raw;       // byte offset of the scan's first record in the raw buffer
+  const char* base;    // the scan's first record
   int first;           // index of that record in the batch's record sequence
   int stride;          // bytes
   int off[3];          // byte offsets of x, y, z: from `vbase` when vec > 0, from the record start otherwise
@@ -881,9 +882,8 @@ __device__ __forceinline__ int rec_scan(const RecBatch& B, int r) {  // scan of 
 }
 // record r of the batch (s: its scan) -> float64 x, y, z as stored; returns whether the scan's range gate keeps it
 // (range_gate.h)
-__device__ __forceinline__ bool read_record(const RecSrc& s, const char* __restrict__ raw, int r, double& x, double& y,
-                                            double& z) {
-  const char* rec = raw + s.raw + (long long)(r - s.first) * s.stride;
+__device__ __forceinline__ bool read_record(const RecSrc& s, int r, double& x, double& y, double& z) {
+  const char* rec = s.base + (long long)(r - s.first) * s.stride;
   if (s.is_f32) {
     float fx, fy, fz;
     if (s.vec) {
@@ -927,17 +927,17 @@ __device__ __forceinline__ void correct_record(const RecSrc& s, const VcorrTable
 // rank.  The scans of a batch lie back to back, so that rank is also the point's position in the forest.  No atomics
 // anywhere: the order is the records' order.
 __global__ void __launch_bounds__(kBlock)
-k_gate_flags(const __grid_constant__ RecBatch B, const char* __restrict__ raw, unsigned char* __restrict__ flag) {
+k_gate_flags(const __grid_constant__ RecBatch B, unsigned char* __restrict__ flag) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
   if (i >= B.n_rec) return;
   double x, y, z;
-  flag[i] = read_record(B.s[rec_scan(B, i)], raw, i, x, y, z) ? 1 : 0;
+  flag[i] = read_record(B.s[rec_scan(B, i)], i, x, y, z) ? 1 : 0;
 }
 // kept (mapped host memory): kept points of every scan, for the build to compare with the host's count; vtab / vc_err:
 // see correct_record.  kVc: some scan of the batch is corrected (without, the kernel is the uncorrected one exactly)
 template <bool kVc>
 __global__ void __launch_bounds__(kBlock)
-k_compact(const __grid_constant__ RecBatch B, const char* __restrict__ raw, const unsigned char* __restrict__ flag,
+k_compact(const __grid_constant__ RecBatch B, const unsigned char* __restrict__ flag,
           const int* __restrict__ G, const int* __restrict__ tile_off, double* __restrict__ out, int* __restrict__ kept,
           const VcorrTable* __restrict__ vtab, int* vc_err) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
@@ -949,7 +949,7 @@ k_compact(const __grid_constant__ RecBatch B, const char* __restrict__ raw, cons
   if (i >= n || !flag[i]) return;
   double x, y, z;
   const RecSrc& s = B.s[rec_scan(B, i)];
-  read_record(s, raw, i, x, y, z);
+  read_record(s, i, x, y, z);
   if (kVc) correct_record(s, vtab, vc_err, x, y, z);
   const size_t o = size_t(rank(i));
   out[3 * o] = x;
@@ -965,7 +965,7 @@ k_compact(const __grid_constant__ RecBatch B, const char* __restrict__ raw, cons
 // before the pipeline deskews it.  kVc: as in k_compact.
 template <bool kVc>
 __global__ void __launch_bounds__(kBlock)
-k_ingest(const __grid_constant__ RecBatch B, const char* __restrict__ raw, const int* __restrict__ perm,
+k_ingest(const __grid_constant__ RecBatch B, const int* __restrict__ perm,
          const unsigned short* __restrict__ chunk, const double* __restrict__ poses /* n_chunks x 12 */, int n,
          double* __restrict__ out, const VcorrTable* __restrict__ vtab, int* vc_err) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
@@ -973,7 +973,7 @@ k_ingest(const __grid_constant__ RecBatch B, const char* __restrict__ raw, const
   double x, y, z;
   const int r = perm ? perm[i] : i;
   const RecSrc& s = B.s[rec_scan(B, r)];
-  read_record(s, raw, r, x, y, z);
+  read_record(s, r, x, y, z);
   if (kVc) correct_record(s, vtab, vc_err, x, y, z);
   if (chunk) {
     const double* X = poses + size_t(chunk[i]) * 12;

@@ -245,16 +245,22 @@ class Registrar:
     def ingest_records(self, records, min_range=0.0, max_range=math.inf, inclusive=True, drop_nan=False, deskew=False,
                        T_prev=None, T_now=None, sensor_hz=10.0, num_threads=1, want_points=False, apply_correction=False,
                        vertical_angle_offset=VERTICAL_ANGLE_OFFSET):
-        """Records -> device-resident float64 cloud of the kept points (madicp_ingest_points_ex).  Returns the kept
-        points (want_points) or their number."""
+        """Records -> device-resident float64 cloud of the kept points (madicp_ingest_points_ex; a device array is read
+        in place, madicp_ingest_points_dev).  Returns the kept points (want_points) or their number."""
         d = describe(records, min_range, max_range, inclusive, drop_nan)
         v = vcorr(apply_correction, vertical_angle_offset)
         out = np.empty((d.n, 3)) if want_points else None
         kept = C.c_int64(0)
         Tp = as_d(pose12(T_prev)) if T_prev is not None else None
         Tn = as_d(pose12(T_now)) if T_now is not None else None
-        check(capi.lib().madicp_ingest_points_ex(self._h, C.byref(d), C.byref(v) if v else None, int(deskew), Tp, Tn,
-                                                 sensor_hz, num_threads, C.byref(kept), as_d(out)), "madicp_ingest_points")
+        if d.on_device:  # read in place on the device, after the producer's stream (records.describe)
+            check(capi.lib().madicp_ingest_points_dev(self._h, C.byref(d), C.byref(v) if v else None, int(deskew), Tp, Tn,
+                                                      sensor_hz, num_threads, d.stream, C.byref(kept), as_d(out)),
+                  "madicp_ingest_points_dev")
+        else:
+            check(capi.lib().madicp_ingest_points_ex(self._h, C.byref(d), C.byref(v) if v else None, int(deskew), Tp, Tn,
+                                                     sensor_hz, num_threads, C.byref(kept), as_d(out)),
+                  "madicp_ingest_points")
         return out[:kept.value].copy() if want_points else kept.value
 
     def stage_records(self, records, reserve_points=0, apply_correction=False, vertical_angle_offset=VERTICAL_ANGLE_OFFSET,
@@ -272,14 +278,21 @@ class Registrar:
         """Several scans of records at once: one forest build, a DeviceTree per scan (madtree_gpu_build_batch_points_ex).
         apply_correction: one flag for all scans, or a sequence with one flag per scan."""
         k = len(records_list)
-        descs = (capi.Points * k)(*[describe(r, **gate) for r in records_list])
+        ds = [describe(r, **gate) for r in records_list]
+        descs = (capi.Points * k)(*ds)
         flags = list(apply_correction) if isinstance(apply_correction, (list, tuple)) else [apply_correction] * k
         if len(flags) != k:
             raise ValueError("build_trees_records: one apply_correction flag per scan")
         vcs = (capi.Vcorr * k)(*[vcorr(f, vertical_angle_offset) or capi.Vcorr() for f in flags])
         out = (C.c_void_p * k)()
-        check(capi.lib().madtree_gpu_build_batch_points_ex(self._h, descs, vcs, k, b_max, b_min, out),
-              "madtree_gpu_build_batch_points")
+        if any(d.on_device for d in ds):  # device records, read in place (one producer stream: the first scan's)
+            if not all(d.on_device for d in ds):
+                raise ValueError("build_trees_records: all scans on the device, or all on the host")
+            check(capi.lib().madtree_gpu_build_batch_points_dev(self._h, descs, vcs, k, b_max, b_min, ds[0].stream, out),
+                  "madtree_gpu_build_batch_points_dev")
+        else:
+            check(capi.lib().madtree_gpu_build_batch_points_ex(self._h, descs, vcs, k, b_max, b_min, out),
+                  "madtree_gpu_build_batch_points")
         self._staged_keepalive.clear()
         return [DeviceTree(C.c_void_p(out[i]), self) for i in range(k)]
 
@@ -291,8 +304,12 @@ class Registrar:
         d = describe(records, min_range, max_range, inclusive, drop_nan)
         v = vcorr(apply_correction, vertical_angle_offset)
         h = C.c_void_p()
-        check(capi.lib().madicp_plan_points(self._h, C.byref(d), C.byref(v) if v else None, int(num_threads), C.byref(h)),
-              "madicp_plan_points")
+        if d.on_device:
+            check(capi.lib().madicp_plan_points_dev(self._h, C.byref(d), C.byref(v) if v else None, int(num_threads),
+                                                    d.stream, C.byref(h)), "madicp_plan_points_dev")
+        else:
+            check(capi.lib().madicp_plan_points(self._h, C.byref(d), C.byref(v) if v else None, int(num_threads),
+                                                C.byref(h)), "madicp_plan_points")
         return DeskewPlan(h, self, records)
 
     def ingest_plan(self, plan, deskew=False, T_prev=None, T_now=None, sensor_hz=10.0, want_points=False):

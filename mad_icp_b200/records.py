@@ -13,6 +13,10 @@ numpy compares it.
 KITTI's reader can also rotate every kept point by a small vertical angle (`apply_correction`,
 apps/utils/kitti_reader.py:72-79, 90-91, a scipy rotation about p x e_z).  `apply_correction=True` does the same on
 the device, bit for bit with scipy 1.18 (`correct_vertical_angle` is the host restatement).
+
+A scan that already lives on the GPU -- any object exporting `__cuda_array_interface__` (a torch CUDA tensor, a CuPy
+array) -- is described the same way and read in place on the device: no copy to the host and back, no synchronisation
+of its producer.  Its descriptor carries `on_device` and the producer `stream` (see `describe`).
 """
 import ctypes as C
 import math
@@ -59,18 +63,73 @@ def _float_type(dt):
     return dt.itemsize
 
 
-def describe(records, min_range=0.0, max_range=math.inf, inclusive=True, drop_nan=False):
+def _rows(n, s0, s1, e):
+    """byte stride and x/y/z offsets of the rows of a 2-D array of n rows whose columns lie s1 bytes apart"""
+    if s1 <= 0:
+        raise ValueError("records: columns must have a positive stride")
+    if n > 1 and s0 <= 0:
+        raise ValueError("records: rows must have a positive stride")
+    if n > 1 and s0 < 2 * s1 + e:
+        raise ValueError(f"records: x, y, z of a row must lie within the row stride ({s0} bytes; columns {s1} bytes "
+                         "apart): rows of a column-major (Fortran-order) or transposed array interleave -- pass "
+                         "np.ascontiguousarray(records) (a contiguous copy, e.g. tensor.contiguous(), on the device)")
+    return (s0 if n > 1 else max(s0, 2 * s1 + e)), [0, s1, 2 * s1]
+
+
+def _cuda_layout(cai):
+    """(pointer, rows, row stride, offsets, field size) of a __cuda_array_interface__ (v2 or v3)"""
+    shape = tuple(int(k) for k in cai["shape"])
+    e = {"<f4": 4, "<f8": 8}.get(cai["typestr"])
+    if len(shape) != 2 or shape[1] < 3 or e is None:
+        raise ValueError("records: a 2-D little-endian float32 / float64 device array with at least 3 columns")
+    if cai.get("mask") is not None:
+        raise ValueError("records: masked device arrays are not supported")
+    strides = cai.get("strides")
+    s0, s1 = (shape[1] * e, e) if strides is None else (int(strides[0]), int(strides[1]))
+    stride, offsets = _rows(shape[0], s0, s1, e)
+    return int(cai["data"][0]), shape[0], stride, offsets, e
+
+
+def _stream_handle(stream):
+    """a cudaStream_t as an int: an int handle, or an object with .cuda_stream (torch.cuda.Stream, cupy streams)"""
+    return int(getattr(stream, "cuda_stream", stream))
+
+
+def _producer_stream(records, cai, stream):
+    """The stream the device records are ready on: an explicit `stream`, else the interface's v3 `stream` entry, else
+    for a torch tensor torch's current stream on its device (torch exports v2, without a stream), else 0 (the legacy
+    default stream)."""
+    if stream is not None:
+        return _stream_handle(stream)
+    if int(cai.get("version", 0)) >= 3 and cai.get("stream") is not None:
+        return int(cai["stream"])  # (1: legacy default, 2: per-thread default, as the interface and the CUDA runtime number them)
+    if type(records).__module__.split(".")[0] == "torch":
+        import torch
+        if isinstance(records, torch.Tensor):
+            return torch.cuda.current_stream(records.device).cuda_stream
+    return 0
+
+
+def describe(records, min_range=0.0, max_range=math.inf, inclusive=True, drop_nan=False, stream=None):
     """madicp_points_t of `records` (read in place):
       - a 2-D float32 / float64 array with at least 3 columns (x, y, z = columns 0, 1, 2) and any row stride that holds
         a row's x, y, z (row-major layouts and views of them; not column-major), e.g.
         np.fromfile(f, np.float32).reshape(-1, 4);
-      - a 1-D structured array whose x, y, z fields share one float type, e.g. np.frombuffer(msg.data, dtype).
+      - a 1-D structured array whose x, y, z fields share one float type, e.g. np.frombuffer(msg.data, dtype);
+      - a 2-D device array exporting __cuda_array_interface__ (torch CUDA tensor, CuPy array), under the same rules as
+        the 2-D numpy array: the descriptor's `on_device` is True and its `stream` is the stream the records are ready
+        on -- `stream=` (an int handle or an object with .cuda_stream), else the interface's v3 stream, else for a torch
+        tensor torch's current stream on its device, else 0 (the legacy default stream).
     inclusive=True gates min_range <= r <= max_range (KITTI), False min_range < r < max_range (PointCloud2);
     drop_nan drops records with a NaN coordinate.  Returns the ctypes structure; the caller keeps `records` alive."""
     a = records
-    if not isinstance(a, np.ndarray):
-        raise TypeError("records: a numpy array (2-D float, or 1-D structured with x, y, z fields)")
-    if a.dtype.names:
+    cai = None if isinstance(a, np.ndarray) else getattr(a, "__cuda_array_interface__", None)
+    if cai is not None:
+        ptr, n, stride, offsets, e = _cuda_layout(cai)
+    elif not isinstance(a, np.ndarray):
+        raise TypeError("records: a numpy array (2-D float, or 1-D structured with x, y, z fields) or a device array "
+                        "exporting __cuda_array_interface__")
+    elif a.dtype.names:
         if a.ndim != 1 or not all(k in a.dtype.names for k in "xyz"):
             raise ValueError("records: a 1-D structured array needs fields x, y and z")
         types = {a.dtype.fields[k][0] for k in "xyz"}
@@ -83,22 +142,14 @@ def describe(records, min_range=0.0, max_range=math.inf, inclusive=True, drop_na
         e = _float_type(a.dtype)
         if a.ndim != 2 or a.shape[1] < 3 or e is None:
             raise ValueError("records: a 2-D little-endian float32 / float64 array with at least 3 columns")
-        s0, s1 = int(a.strides[0]), int(a.strides[1])
-        if s1 <= 0:
-            raise ValueError("records: columns must have a positive stride")
-        if a.shape[0] > 1 and s0 <= 0:
-            raise ValueError("records: rows must have a positive stride")
-        if a.shape[0] > 1 and s0 < 2 * s1 + e:
-            raise ValueError(f"records: x, y, z of a row must lie within the row stride ({s0} bytes; columns {s1} bytes "
-                             "apart): rows of a column-major (Fortran-order) or transposed array interleave -- pass "
-                             "np.ascontiguousarray(records)")
-        offsets = [0, s1, 2 * s1]
-        stride = s0 if a.shape[0] > 1 else max(s0, 2 * s1 + e)
+        stride, offsets = _rows(a.shape[0], int(a.strides[0]), int(a.strides[1]), e)
     if stride <= 0:
         raise ValueError("records: rows must have a positive stride")
     d = Points()
-    d.data = a.ctypes.data
-    d.n = a.shape[0]
+    if cai is not None:
+        d.data, d.n = ptr, n
+    else:
+        d.data, d.n = a.ctypes.data, a.shape[0]
     d.stride = stride
     d.offset[:] = offsets
     d.is_f32 = int(e == 4)
@@ -106,15 +157,46 @@ def describe(records, min_range=0.0, max_range=math.inf, inclusive=True, drop_na
     d.max_range = float(max_range)
     d.range_mode = RANGE_INCLUSIVE if inclusive else RANGE_STRICT
     d.drop_nan = int(bool(drop_nan))
+    d.on_device = cai is not None
+    d.stream = _producer_stream(records, cai, stream) if cai is not None else None
     return d
 
 
-def layout(records, min_range=0.0, max_range=math.inf, inclusive=True, drop_nan=False):
+def layout(records, min_range=0.0, max_range=math.inf, inclusive=True, drop_nan=False, stream=None):
     """describe() as a plain tuple (data, n, stride, off_x, off_y, off_z, is_f32, min_range, max_range, range_mode,
-    drop_nan): what the pybind Pipeline reads."""
-    d = describe(records, min_range, max_range, inclusive, drop_nan)
+    drop_nan, on_device, stream): what the pybind Pipeline reads (stream: 0 for host records)."""
+    d = describe(records, min_range, max_range, inclusive, drop_nan, stream)
     return (int(d.data or 0), d.n, d.stride, d.offset[0], d.offset[1], d.offset[2], d.is_f32, d.min_range, d.max_range,
-            d.range_mode, d.drop_nan)
+            d.range_mode, d.drop_nan, d.on_device, d.stream or 0)
+
+
+def to_host(records):
+    """A device array copied to the host once, as a numpy array (for host-built trees, MADICP_GPU_BUILD=0)."""
+    if hasattr(records, "cpu"):  # torch
+        return records.detach().cpu().numpy()
+    if hasattr(records, "get"):  # CuPy
+        return records.get()
+    raise TypeError("records: cannot copy this device array to the host (a torch tensor or a CuPy array is needed)")
+
+
+def search_cloud_arrays_dev(search_dev, queries):
+    """MADtree.searchCloudArrays of device queries: (points N x 3, normals N x 3, dists N) as float64 torch tensors on the
+    queries' device, written by the search kernel in place and ready on the caller's current stream (no host sync).
+    search_dev: MADtree._searchCloudDev."""
+    import torch
+    d = describe(queries)
+    e = 4 if d.is_f32 else 8
+    if list(d.offset) != [0, e, 2 * e]:
+        raise ValueError("queries: x, y, z must be adjacent columns -- pass a contiguous copy")
+    dev = getattr(queries, "device", None)
+    dev = torch.device("cuda", getattr(dev, "index", getattr(dev, "id", None)) or 0) if dev is not None else torch.device("cuda")
+    n = int(d.n)
+    P = torch.empty((n, 3), dtype=torch.float64, device=dev)
+    N = torch.empty((n, 3), dtype=torch.float64, device=dev)
+    D = torch.empty(n, dtype=torch.float64, device=dev)
+    search_dev(int(d.data), n, int(d.stride), bool(d.is_f32), P.data_ptr(), N.data_ptr(), D.data_ptr(),
+               torch.cuda.current_stream(dev).cuda_stream)
+    return P, N, D
 
 
 def vcorr(apply_correction=False, vertical_angle_offset=VERTICAL_ANGLE_OFFSET):
@@ -127,10 +209,16 @@ def vcorr(apply_correction=False, vertical_angle_offset=VERTICAL_ANGLE_OFFSET):
     return v
 
 
+def _host(d):
+    if d.on_device:
+        raise TypeError("records: the host restatement needs host records (records.to_host)")
+    return d
+
+
 def range_mask(records, **gate):
     """The gate on the host (madicp_debug_range_mask): uint8 keep flag per record."""
     from . import _capi
-    d = describe(records, **gate)
+    d = _host(describe(records, **gate))
     keep = np.empty(max(int(d.n), 1), np.uint8)
     _capi.check(_capi.lib().madicp_debug_range_mask(C.byref(d), keep.ctypes.data_as(_capi.bp)), "madicp_debug_range_mask")
     return keep[:d.n]
@@ -140,7 +228,7 @@ def correct_vertical_angle(records, vertical_angle_offset=VERTICAL_ANGLE_OFFSET,
     """The kept points of `records` (describe's gate keywords), corrected like KittiReader.apply_rotation_correction,
     on the host with the restatement the device applies (madicp_debug_correct_points): an M x 3 float64 array."""
     from . import _capi
-    d = describe(records, **gate)
+    d = _host(describe(records, **gate))
     v = vcorr(True, vertical_angle_offset)
     out = np.empty((max(int(d.n), 1), 3))
     kept = _capi.check(_capi.lib().madicp_debug_correct_points(C.byref(d), C.byref(v), _capi.as_d(out)),
@@ -148,5 +236,5 @@ def correct_vertical_angle(records, vertical_angle_offset=VERTICAL_ANGLE_OFFSET,
     return out[:kept]
 
 
-__all__ = ["pointcloud2_dtype", "describe", "layout", "range_mask", "vcorr", "correct_vertical_angle",
+__all__ = ["pointcloud2_dtype", "describe", "layout", "to_host", "search_cloud_arrays_dev", "range_mask", "vcorr", "correct_vertical_angle",
            "VERTICAL_ANGLE_OFFSET", "RANGE_NONE", "RANGE_INCLUSIVE", "RANGE_STRICT"]

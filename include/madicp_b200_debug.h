@@ -29,6 +29,14 @@ int madicp_debug_cta_stamps(madicp_ctx_t* ctx, int plane, int64_t* out, int cap)
  * launch from the item count; threads_per_cta = 0 restores that.  Returns the CTAs per SM in effect. */
 int madicp_set_gn_grid(madicp_ctx_t* ctx, int threads_per_cta, int ctas_per_sm);
 
+/* Work partition of the persistent kernel for a grid of G CTAs over L moving leaves: CTA b's four stretches are
+ * [lo[p], lo[p] + n[p]).  Returns the CTA's share (the sum of n).  No context, no device work. */
+int madicp_debug_gn_stretch(int64_t L, int G, int b, uint32_t lo[4], uint32_t n[4]);
+/* Bytes per CTA the persistent kernel's launch reserves for its item map with K active keyframes, L moving leaves and
+ * G CTAs, or 0 when it takes no map (the carve-out condition of the launch, which depends on the kernel shape, is not
+ * applied).  No context, no device work. */
+int64_t madicp_debug_gn_map_bytes(int K, int64_t L, int G);
+
 
 /* Path memo of the persistent kernel (kernels.cuh, descend_t): mode 0 walks every (leaf, keyframe) pair from the root
  * in every round; 1 skips the walks whose leaf is proved unchanged; 2 (the default) also resumes the other walks from

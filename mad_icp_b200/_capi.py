@@ -122,6 +122,8 @@ SYMBOLS = {
     "madicp_debug_timing": (C.c_int, [vp, C.c_int, C.POINTER(C.c_int64), C.c_int]),
     "madicp_debug_cta_cycles": (C.c_int, [vp, C.POINTER(C.c_int64), C.c_int]),
     "madicp_set_gn_grid": (C.c_int, [vp, C.c_int, C.c_int]),
+    "madicp_debug_gn_stretch": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
+    "madicp_debug_gn_map_bytes": (C.c_int64, [C.c_int, C.c_int64, C.c_int]),
     "madicp_debug_set_memo": (C.c_int, [vp, C.c_int]),
     "madicp_debug_cta_stamps": (C.c_int, [vp, C.c_int, C.POINTER(C.c_int64), C.c_int]),
 }

@@ -912,11 +912,11 @@ static int register_enqueue(madicp_ctx* c, int iters, const double X0[12], int c
   A.iters = iters;
   A.clear_from = clear_from;
   A.matched = c->d_comm->matched[mb];
-  // Item map in shared memory: 4 bytes per CTA-local item, taken only if it neither exceeds the reserve
-  // nor pushes the CTA into the next shared-memory carve-out (that would shrink L1, which holds the tree).
+  // Item map in shared memory: 4 bytes per CTA-local item of the largest share (gn_map_bytes), taken only if it neither
+  // exceeds the reserve nor pushes the CTA into the next shared-memory carve-out (that would shrink L1, which holds the tree).
   size_t map_bytes = 0;
   {
-    const size_t per_cta = size_t(madicp_num_keyframes(c)) * (size_t(c->L) / size_t(c->gn_grid) + 8) * 4 + 128;
+    const size_t per_cta = gn_map_bytes(unsigned(madicp_num_keyframes(c)), unsigned(c->L), unsigned(c->gn_grid));
     auto bucket = [](size_t bytes) {
       const size_t kb[] = {8, 16, 32, 64, 100, 132, 164, 196, 228};
       for (size_t b : kb)
@@ -924,14 +924,14 @@ static int register_enqueue(madicp_ctx* c, int iters, const double X0[12], int c
       return size_t(1 << 20);
     };
     const size_t ctas = size_t(c->gn_grid / c->sm_count);
-    if (per_cta <= kGnMapMaxBytes && c->L < (1 << 26) && bucket((c->gn_smem + per_cta) * ctas) == bucket(c->gn_smem * ctas))
-      map_bytes = per_cta;
+    if (per_cta && bucket((c->gn_smem + per_cta) * ctas) == bucket(c->gn_smem * ctas)) map_bytes = per_cta;
   }
   A.map_in_smem = map_bytes ? 1 : 0;
   {  // path memo: one entry per CTA-local item
     // sized from the CAPACITIES (slots, moving-leaf buffer), not from this scan's counts: a streamed sequence changes
-    // both from scan to scan and must not reallocate
-    const size_t stride = ((size_t(c->max_keyframes) * (c->cap_moving / size_t(c->gn_grid) + 8)) + 31) & ~size_t(31);
+    // both from scan to scan and must not reallocate (gn_share_bound is monotone in L: it covers every L <= cap_moving)
+    const size_t stride =
+        ((size_t(c->max_keyframes) * gn_share_bound(c->cap_moving, unsigned(c->gn_grid))) + 31) & ~size_t(31);
     const size_t need = stride * size_t(c->gn_grid);
     if (need > c->cap_memo) {
       CK(cudaStreamSynchronize(c->stream));
@@ -1295,6 +1295,30 @@ int madicp_set_gn_grid(madicp_ctx_t* c, int threads_per_cta, int ctas_per_sm) {
   if (rc) return rc;
   c->gn_auto = false;
   return c->gn_grid / c->sm_count;
+}
+
+int madicp_debug_gn_stretch(int64_t L, int G, int b, uint32_t lo[4], uint32_t n[4]) {
+  if (L < 1 || L >= (int64_t(1) << 31) || G < 1 || b < 0 || b >= G || !lo || !n) {
+    set_error("madicp_debug_gn_stretch: bad arguments (1 <= L < 2^31, 0 <= b < G)");
+    return MADICP_ERR_INVALID;
+  }
+  int share = 0;
+  for (unsigned p = 0; p < kGnPieces; ++p) {
+    unsigned l = 0, m = 0;
+    gn_stretch(unsigned(L), unsigned(G), unsigned(b), p, l, m);
+    lo[p] = l;
+    n[p] = m;
+    share += int(m);
+  }
+  return share;
+}
+
+int64_t madicp_debug_gn_map_bytes(int K, int64_t L, int G) {
+  if (K < 1 || K > kMaxSlots || L < 1 || L >= (int64_t(1) << 31) || G < 1) {
+    set_error("madicp_debug_gn_map_bytes: bad arguments (1 <= K <= 64, 1 <= L < 2^31, G >= 1)");
+    return MADICP_ERR_INVALID;
+  }
+  return int64_t(gn_map_bytes(unsigned(K), unsigned(L), unsigned(G)));
 }
 
 }  // extern "C"

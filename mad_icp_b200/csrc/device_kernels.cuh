@@ -1,5 +1,6 @@
 // device_kernels.cuh -- the __global__ entry points (see kernels.cuh for the design notes).
 #pragma once
+#include "gn_partition.h"
 #include "kernels.cuh"
 
 namespace madicp {
@@ -452,30 +453,15 @@ k_gn_loop(const __grid_constant__ GnArgs A) {
   const unsigned lane = threadIdx.x & 31;
   const unsigned warp = threadIdx.x >> 5;
   double* stage = s_stage_all + warp * kStageTile;
-  // kPieces contiguous stretches per CTA, dealt serpentine-wise (piece p of CTA b is stretch p*G + b for
-  // even p, p*G + G-1-b for odd p): the cost of a stretch varies smoothly along the DFS order of the scan
-  // (tree depth, gate pass rate; measured 18k..32k cycles per CTA with one stretch each), pairing opposite
-  // ends evens it out while every stretch stays one compact spatial region.
-  constexpr unsigned kPieces = 4;
+  // kPieces contiguous stretches per CTA (gn_partition.h: gn_stretch; measured 18k..32k cycles per CTA with one
+  // stretch each, before the serpentine deal).  CTA 0 gets 5/8 of a share, so that it has the other CTAs' tiles in hand
+  // when the last one arrives.
+  constexpr unsigned kPieces = kGnPieces;
   unsigned p_lo[kPieces], p_n[kPieces];
   unsigned n_b = 0;  // moving leaves of this CTA
 #pragma unroll
-  // CTA 0 also folds the tiles of the round and solves: it gets 5/8 of a share, so that it is done with its own items
-  // early and has the other CTAs' tiles in hand when the last one arrives (weights in eighths; grids below 8 CTAs: equal).
-  const unsigned G = gridDim.x;
-  const unsigned light = (G >= 8u) ? 3u : 0u;
-  const uint64_t W8 = 8ull * G - light;
   for (unsigned p = 0; p < kPieces; ++p) {
-    const unsigned s = (p & 1u) ? (G - 1u - blockIdx.x) : blockIdx.x;  // position of this CTA inside piece p
-    auto cum8 = [&](unsigned pos) -> uint64_t {                         // weight of the positions before `pos`
-      if (p & 1u) return (pos >= G) ? W8 : 8ull * pos;                  // odd pieces: CTA 0 sits last
-      return pos ? 8ull * pos - light : 0ull;                           // even pieces: CTA 0 sits first
-    };
-    const uint64_t p0 = (uint64_t(L) * p) / kPieces, p1 = (uint64_t(L) * (p + 1)) / kPieces;
-    const unsigned lo = unsigned(p0 + ((p1 - p0) * cum8(s)) / W8);
-    const unsigned hi = unsigned(p0 + ((p1 - p0) * cum8(s + 1u)) / W8);
-    p_lo[p] = lo;
-    p_n[p] = hi - lo;
+    gn_stretch(L, gridDim.x, blockIdx.x, p, p_lo[p], p_n[p]);
     n_b += p_n[p];
   }
   const unsigned t_total = unsigned(A.model.K) * n_b;  // CTA-local items
@@ -504,7 +490,7 @@ k_gn_loop(const __grid_constant__ GnArgs A) {
     for (unsigned t0 = warp * 32; t0 < t_total; t0 += THREADS) {
       unsigned k, q;
       item_of(t0, k, q);
-      s_map[t0 + lane] = (k << 26) | q;  // entries past t_total are never used
+      s_map[t0 + lane] = (k << 26) | q;  // entries past t_total are never used (gn_map_bytes reserves whole warp groups)
     }
     __syncwarp();  // a warp only ever reads what it wrote itself
   }
@@ -739,6 +725,5 @@ template <int THREADS>
 constexpr size_t gn_dynamic_smem() {
   return sizeof(double) * size_t(THREADS / 32) * kStageTile;
 }
-constexpr size_t kGnMapMaxBytes = 16 * 1024;  // optional item map behind the tiles (GnArgs::map_in_smem)
 
 }  // namespace madicp

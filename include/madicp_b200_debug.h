@@ -38,6 +38,11 @@ int madicp_debug_gn_stretch(int64_t L, int G, int b, uint32_t lo[4], uint32_t n[
 int64_t madicp_debug_gn_map_bytes(int K, int64_t L, int G);
 
 
+/* The keyframe weight det(H^-1) the persistent kernel returns with its last round, for a row-major H: one thread
+ * copies H into a 6x8 array as the kernel's shared H/b sums are laid out and runs the same routine (solve6.h
+ * inv_det6).  Synchronous. */
+int madicp_debug_inv_det6(madicp_ctx_t* ctx, const double H[36], double* weight);
+
 /* Path memo of the persistent kernel (kernels.cuh, descend_t): mode 0 walks every (leaf, keyframe) pair from the root
  * in every round; 1 skips the walks whose leaf is proved unchanged; 2 (the default) also resumes the other walks from
  * the deepest record of their last path that is proved unchanged.  Results are identical in every mode (the memo only

@@ -883,6 +883,20 @@ int madicp_solve_update(madicp_ctx_t* c, const double H[36], const double b[6], 
   return MADICP_OK;
 }
 
+int madicp_debug_inv_det6(madicp_ctx_t* c, const double H[36], double* weight) {
+  if (!c || !H || !weight) return MADICP_ERR_INVALID;
+  CK(cudaSetDevice(c->device));
+  memcpy(c->h_pinned + 12, H, 36 * sizeof(double));
+  CK(cudaMemcpyAsync(c->d_X + 12, c->h_pinned + 12, 36 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  k_inv_det6<<<1, 32, 0, c->stream>>>(c->d_X + 12, c->d_X + 48);
+  c->launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(c->h_pinned + 48, c->d_X + 48, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  *weight = c->h_pinned[48];
+  return MADICP_OK;
+}
+
 // clear_from: first round whose gate passes are recorded in the matched flags.
 static int register_enqueue(madicp_ctx* c, int iters, const double X0[12], int clear_from) {
   int rc = check_ready(c, "madicp_register");

@@ -289,6 +289,17 @@ __global__ void k_solve(const double* __restrict__ H, const double* __restrict__
   }
 }
 
+// madicp_debug_inv_det6: the keyframe weight of a row-major H, read with the persistent kernel's row stride of 8
+// (s_tot: H row r, then b[r], then one unused entry) through the same out-of-line routine.
+__global__ void k_inv_det6(const double* __restrict__ H, double* weight) {
+  if (threadIdx.x == 0 && blockIdx.x == 0) {
+    double T[48];
+    for (int r = 0; r < 6; ++r)
+      for (int c = 0; c < 8; ++c) T[r * 8 + c] = (c < 6) ? H[r * 6 + c] : 0.0;
+    *weight = inv_det6_dev(T, 8);
+  }
+}
+
 // MADtreeWrapper::searchCloud / searchCloudDist: arbitrary query points against one keyframe.  Query i is x, y, z at
 // q + i * q_stride (bytes), float32 (q_is_f32) or float64, read in place; a float32 query is widened to float64 as the
 // host converts it.

@@ -56,7 +56,8 @@ inline double inverseDeterminant(const double H[36]) {
       for (int c = k; c < 6; ++c) A[i * 6 + c] -= f * A[k * 6 + c];
     }
   }
-  return 1.0 / det;
+  // a zero last pivot gives NaN, as the reference's inverse().determinant() does (solve6.h inv_det6)
+  return (A[35] == 0.0) ? std::numeric_limits<double>::quiet_NaN() : 1.0 / det;
 }
 
 // odometry/vel_estimator.cpp:45-97.  J = I*dt makes H diagonal, so the 6x6 LDLT of the reference reduces to

@@ -12,12 +12,36 @@
 // un-pivoted with compile-time indices only.  On the device that keeps the working set in
 // registers; the update sits on the critical path between two GN rounds (one thread, nothing to
 // overlap with), and a pointer-indexed version costs ~25 us per round.
+// tests/test_gpu_update.py checks these claims against an exact rational LDL^T written from Eigen's algorithm: all
+// 720 pivot orders, every rank, ties of the largest diagonal that change the answer, the DBL_MIN cut-off of the
+// pseudo-inverse, and an upper triangle that is NaN or differs from the lower one.
 #pragma once
 #include <float.h>
 
 #include "arith.h"
 
 namespace madicp {
+
+#if defined(__CUDACC__)
+#define MADICP_HD_COLD static __host__ __device__ __noinline__
+#else
+#define MADICP_HD_COLD inline
+#endif
+
+// The solve when the first pivot is 0 (the whole diagonal is zero, NaN entries aside) or NaN (H[0][0] is NaN, which
+// no other entry beats).  Eigen stops factoring there and solves with the untouched lower triangle as L and D, in the
+// original order: 0 for a finite H, and NaN where Eigen's own solve meets one.  Out of line, so that the persistent
+// kernel does not carry its registers for a case that finite sums of J^T J never reach.
+MADICP_HD_COLD void ldlt6_solve_neg_unfactored(const double* H, int ld, const double* b, double* x) {
+  for (int i = 0; i < 6; ++i) {
+    double v = -b[i];
+    for (int j = 0; j < i; ++j) v -= H[i * ld + j] * x[j];
+    x[i] = v;
+  }
+  for (int i = 0; i < 6; ++i) x[i] = (fabs(H[i * ld + i]) > DBL_MIN) ? x[i] / H[i * ld + i] : 0.0;
+  for (int i = 5; i >= 0; --i)
+    for (int j = i + 1; j < 6; ++j) x[i] -= H[j * ld + i] * x[j];
+}
 
 // H: 6x6 with row stride `ld` (H[r*ld+c]); only the lower triangle (r >= c) is read.  x = solve(-b).
 MADICP_HD void ldlt6_solve_neg(const double* H, int ld, const double* b, double* x) {
@@ -50,9 +74,8 @@ MADICP_HD void ldlt6_solve_neg(const double* H, int ld, const double* b, double*
       idx[i] = sw ? a : c;
     }
   }
-  if (!(dg[0] > 0.0)) {  // whole diagonal zero: Eigen stops factoring, D = 0 -> solution 0
-#pragma unroll
-    for (int i = 0; i < 6; ++i) x[i] = 0.0;
+  if (!(dg[0] > 0.0)) {
+    ldlt6_solve_neg_unfactored(H, ld, b, x);
     return;
   }
   // (2) permuted lower triangle (entry (i,j) comes from the original LOWER entry of rows idx[i], idx[j])
@@ -70,6 +93,7 @@ MADICP_HD void ldlt6_solve_neg(const double* H, int ld, const double* b, double*
   }
   // (3) left-looking LDL^T, static indices
   double inv[6];
+  bool keep[6];
 #pragma unroll
   for (int k = 0; k < 6; ++k) {
     if (k > 0) {
@@ -91,11 +115,15 @@ MADICP_HD void ldlt6_solve_neg(const double* H, int ld, const double* b, double*
     const double d = A[k][k];
     // one reciprocal per pivot instead of a division per entry (Eigen divides; the quotients differ by
     // <= 1 ulp, far inside the pose tolerance, and a software DDIV is ~25 instructions on the serial path)
-    inv[k] = (fabs(d) > DBL_MIN) ? 1.0 / d : 0.0;
-    if (fabs(d) > 0.0) {
-      const double r = 1.0 / d;
+    keep[k] = fabs(d) > DBL_MIN;
+    inv[k] = keep[k] ? 1.0 / d : 0.0;
+    if (keep[k]) {
 #pragma unroll
-      for (int i = k + 1; i < 6; ++i) A[i][k] *= r;
+      for (int i = k + 1; i < 6; ++i) A[i][k] *= inv[k];
+    } else if (fabs(d) > 0.0) {
+      // a subnormal pivot: its reciprocal may overflow, and 0 * inf would put NaN where Eigen's 0 / d puts 0
+#pragma unroll
+      for (int i = k + 1; i < 6; ++i) A[i][k] /= d;
     }
   }
 #pragma unroll
@@ -103,7 +131,7 @@ MADICP_HD void ldlt6_solve_neg(const double* H, int ld, const double* b, double*
 #pragma unroll
     for (int j = 0; j < i; ++j) y[i] -= A[i][j] * y[j];
 #pragma unroll
-  for (int i = 0; i < 6; ++i) y[i] *= inv[i];  // pseudo-inverse of D: 0 where |D_i| <= DBL_MIN
+  for (int i = 0; i < 6; ++i) y[i] = keep[i] ? y[i] * inv[i] : 0.0;  // pseudo-inverse of D: Eigen sets these to 0
 #pragma unroll
   for (int i = 5; i >= 0; --i)
 #pragma unroll
@@ -154,7 +182,11 @@ MADICP_HD double inv_det6(const double* H, int ld) {
       for (int c = k; c < 6; ++c) A[i][c] = sub_(A[i][c], mul_(f, A[k][c]));
     }
   }
-  return 1.0 / det;
+  // An exactly zero pivot before the last one makes the rows below it 0/0, so det is already NaN.  A zero last pivot
+  // leaves det = +-0, and 1/det would be +-inf: -inf is below every finite weight, and Pipeline would keep that
+  // singular frame as a keyframe.  The reference's H.inverse() divides by that pivot, and the determinant of the
+  // result is NaN, which never wins the smallest-weight search: return the same.
+  return (A[5][5] == 0.0) ? NAN : 1.0 / det;
 }
 
 // Rodrigues with the reference's small-angle branch (theta^2 < 1e-8 -> I + [w]x). R row-major 3x3.

@@ -401,6 +401,13 @@ class Registrar:
         check(capi.lib().madicp_solve_update(self._h, as_d(H), as_d(b), as_d(X)), "madicp_solve_update")
         return X
 
+    def inv_det6(self, H):
+        """The keyframe weight det(H^-1) that register_fetch() returns, for any 6x6 H (madicp_debug_inv_det6)."""
+        H = np.ascontiguousarray(H, dtype=np.float64)
+        w = C.c_double(0)
+        check(capi.lib().madicp_debug_inv_det6(self._h, as_d(H), C.byref(w)), "madicp_debug_inv_det6")
+        return w.value
+
     def register(self, X0, iters=15, want_matched=True):
         """The whole ICP loop on the device.  Returns dict(X 3x4, H 6x6, b 6, matched L, n_matched)."""
         X = pose12(X0).copy()

@@ -23,7 +23,8 @@ _bp = C.POINTER(C.c_ubyte)
 
 def build(force=False):
     """Compile the restatement with oracle/Makefile (gcc only, no GPU needed)."""
-    src_m = max(os.path.getmtime(os.path.join(_HERE, f)) for f in ("oracle_capi.cpp", "madicp_oracle.hpp", "Makefile"))
+    srcs = ("oracle_capi.cpp", "madicp_oracle.hpp", "pipeline_oracle.hpp", "Makefile")
+    src_m = max(os.path.getmtime(os.path.join(_HERE, f)) for f in srcs)
     if force or not os.path.exists(_SO) or os.path.getmtime(_SO) < src_m:
         subprocess.check_call(["make", "-C", _HERE, "-s"])
     return _SO
@@ -173,6 +174,14 @@ def solve_update(H, b, X):
     dx, Xo = np.empty(6), np.empty((3, 4))
     lib().orc_solve_update(_d(Hc), _d(bb), _d(X), _d(dx), _d(Xo))
     return dx, Xo
+
+
+def inverse_determinant(H):
+    """The keyframe weight det(H^-1) of pipeline.cpp:223 (pipeline_oracle.hpp inverseDeterminant6)."""
+    H = np.ascontiguousarray(H, dtype=np.float64).reshape(36)
+    fn = lib().orc_inverse_determinant6
+    fn.restype, fn.argtypes = C.c_double, [_dp]
+    return fn(_d(H))
 
 
 def eig3(cov):

@@ -243,6 +243,13 @@ void orc_pipeline_state(void* p, double* out) {
   for (int i = 0; i < 6; ++i) out[17 + i] = P->current_velocity_.v[i];
 }
 }
+// the keyframe weight (pipeline.cpp:223) of a row-major H, as the restated Pipeline computes it
+extern "C" double orc_inverse_determinant6(const double* H36) {
+  orc::M6 H;
+  for (int r = 0; r < 6; ++r)
+    for (int c = 0; c < 6; ++c) H(r, c) = H36[r * 6 + c];
+  return orc::inverseDeterminant6(H);
+}
 extern "C" void orc_pipeline_deskew(void* p, double* pts, int n, const double* Tprev12, const double* Tnow12) {
   orc::Cloud c(n);
   for (int i = 0; i < n; ++i) c[i] = V3{{pts[3 * i], pts[3 * i + 1], pts[3 * i + 2]}};

@@ -89,7 +89,8 @@ inline double inverseDeterminant6(const M6& H) {
       for (int c = k; c < 6; ++c) A[i][c] -= f * A[k][c];
     }
   }
-  return 1.0 / det;
+  // a zero last pivot: the reference's inverse() divides by it and the determinant of that is NaN (not 1/+-0)
+  return (A[5][5] == 0.0) ? std::numeric_limits<double>::quiet_NaN() : 1.0 / det;
 }
 
 // odometry/vel_estimator.{h,cpp}

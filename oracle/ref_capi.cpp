@@ -197,4 +197,12 @@ void ref_pipeline_deskew(void* p, double* pts, int n, const double* Tprev12, con
 }
 int ref_max_threads() { return omp_get_max_threads(); }
 
+// The keyframe weight of pipeline.cpp:223, H_adder_.inverse().determinant(), for a row-major H.
+double ref_inverse_determinant(const double* H36) {
+  Eigen::Matrix<double, 6, 6> H;
+  for (int r = 0; r < 6; ++r)
+    for (int c = 0; c < 6; ++c) H(r, c) = H36[r * 6 + c];
+  return H.inverse().determinant();
+}
+
 }  // extern "C"

@@ -169,6 +169,16 @@ def max_threads():
     return lib().ref_max_threads()
 
 
+def inverse_determinant(H):
+    """pipeline.cpp:223's keyframe weight, H.inverse().determinant(), evaluated by the reference's own expression.
+    Resolved here rather than in lib(): only tests/golden/make_weight_reference.py calls it, and a library built
+    before the entry point existed still serves every other caller."""
+    H = np.ascontiguousarray(H, dtype=np.float64).reshape(36)
+    fn = lib().ref_inverse_determinant
+    fn.restype, fn.argtypes = C.c_double, [_dp]
+    return fn(_d(H))
+
+
 def variant(so_name, make_target=None):
     """A second instance of this module over another build of the same C entry points (oracle/ref_capi.cpp), e.g.
     `variant("libmadicp_ref_gpu.so", "ref_gpu")`: the reference's unmodified pipeline.cpp / vel_estimator.cpp linked

@@ -164,6 +164,18 @@ int madtree_gpu_num_leaves(const madtree_gpu_t* t);
 int madtree_gpu_num_levels(const madtree_gpu_t* t);
 /* Device -> host (synchronises): the breadth-first records and/or the getLeafs table.  Either may be NULL. */
 int madtree_gpu_download(const madtree_gpu_t* t, madtree_rec_t* recs_out, int32_t* leaf_records_out);
+/* MADtree::getLeafs (tools/mad_tree.cpp:154-163) -> leaf->mean_, as Pipeline::currentLeaves / modelLeaves hand them out
+ * (odometry/pipeline.cpp:290-308).  Leaf means of `count` device trees of one context, in getLeafs order, tree after
+ * tree, gathered in one launch: means_out receives sum(leaves) x 3 doubles.  X (NULL: no poses) holds a pose per tree:
+ * X[k] (NULL, or 12 doubles row-major [R|t]) is applied as MADtree::applyTransform would (the node transform's operand
+ * order, no FMA); NULL rows are copied untouched (-0.0 stays -0.0).  Host output; synchronises.  count == 0 does
+ * nothing.  Returns the number of leaves written. */
+int madtree_gpu_leaf_means(const madtree_gpu_t* const* trees, const double* const* X, int count, double* means_out);
+/* The same into device memory of the trees' device (8-byte aligned), ordered like madicp_search_cloud_dev: the
+ * context's stream first waits for consumer_stream (where the output is allocated; 0: the legacy default stream), and
+ * the result is ready on consumer_stream through an event wait, with no host sync. */
+int madtree_gpu_leaf_means_dev(const madtree_gpu_t* const* trees, const double* const* X, int count, double* means_out,
+                               void* consumer_stream);
 /* Audit dump of a DEVICE-BUILT tree in breadth-first order: mean n x 3, eigenvectors n x 9 (column-major), bbox
  * n x 3, num_points n (any may be NULL).  Valid for the most recently built tree of the context.  Synchronises. */
 int madtree_gpu_export(const madtree_gpu_t* t, double* mean, double* eigenvectors, double* bbox, int32_t* num_points);

@@ -72,6 +72,8 @@ SYMBOLS = {
     "madtree_gpu_num_leaves": (C.c_int, [vp]),
     "madtree_gpu_num_levels": (C.c_int, [vp]),
     "madtree_gpu_download": (C.c_int, [vp, vp, ip]),
+    "madtree_gpu_leaf_means": (C.c_int, [C.POINTER(vp), C.POINTER(dp), C.c_int, dp]),
+    "madtree_gpu_leaf_means_dev": (C.c_int, [C.POINTER(vp), C.POINTER(dp), C.c_int, vp, vp]),
     "madtree_gpu_export": (C.c_int, [vp, dp, dp, dp, ip]),
     "madicp_set_moving_tree": (C.c_int, [vp, vp]),
     "madicp_get_moving": (C.c_int, [vp, dp, C.c_int]),

@@ -290,6 +290,10 @@ int madicp_create(madicp_ctx_t** out, int device, int max_keyframes) {
   CK(cudaMallocHost(&c->h_xform, size_t(madicp_ctx::kXformRing) * 12 * sizeof(double)));
   CK(cudaMallocHost(&c->h_lvl, size_t(madicp_ctx::kXformRing) * (kMaxLevels + 1) * sizeof(int)));
   for (int i = 0; i < madicp_ctx::kXformRing; ++i) CK(cudaEventCreateWithFlags(&c->xform_done[i], cudaEventDisableTiming));
+  c->cap_gather = kMaxSlots;  // (a whole model in one table: growing it synchronises)
+  CK(cudaMallocHost(&c->h_gather, size_t(madicp_ctx::kGatherRing) * c->cap_gather * sizeof(LeafGather)));
+  CK(cudaMalloc(&c->d_gather, size_t(madicp_ctx::kGatherRing) * c->cap_gather * sizeof(LeafGather)));
+  for (int i = 0; i < madicp_ctx::kGatherRing; ++i) CK(cudaEventCreateWithFlags(&c->gather_done[i], cudaEventDisableTiming));
   CK(cudaMallocHost(&c->h_pinned, sizeof(double) * 64));
   CK(cudaMallocHost(&c->h_state, sizeof(GnState)));
   CK(cudaMallocHost(&c->h_matched, kMatchedCap));
@@ -349,6 +353,12 @@ void madicp_destroy(madicp_ctx_t* c) {
   cudaFreeHost(c->h_state);
   for (int i = 0; i < madicp_ctx::kXformRing; ++i)
     if (c->xform_done[i]) cudaEventDestroy(c->xform_done[i]);
+  cudaFree(c->d_gather);
+  cudaFreeHost(c->h_gather);
+  for (int i = 0; i < madicp_ctx::kGatherRing; ++i)
+    if (c->gather_done[i]) cudaEventDestroy(c->gather_done[i]);
+  cudaFree(c->d_leaves);
+  cudaFreeHost(c->h_leaves);
   cudaFreeHost(c->h_matched);
   if (c->tree_free_ev) cudaEventDestroy(c->tree_free_ev);
   if (c->xstream_ev) cudaEventDestroy(c->xstream_ev);
@@ -639,6 +649,82 @@ int madicp_stream_wait(madicp_ctx* c, void* waiter, void* signaller) {
   return MADICP_OK;
 }
 
+// Arguments of a leaf-mean gather (madtree_gpu_leaf_means*): a table of count >= 0 trees of one context and an output.
+// *ctx: the trees' context (nullptr when count == 0), *total: their leaves.
+static int leaf_gather_check(const madtree_gpu_t* const* trees, int count, const void* out, const char* fn, madicp_ctx** ctx,
+                             int* total) {
+  *ctx = nullptr;
+  *total = 0;
+  if (!trees || count < 0) {
+    set_error(std::string(fn) + ": bad arguments (a table of count >= 0 trees)");
+    return MADICP_ERR_INVALID;
+  }
+  if (count == 0) return MADICP_OK;
+  if (!out) {
+    set_error(std::string(fn) + ": no output");
+    return MADICP_ERR_INVALID;
+  }
+  int64_t n = 0;
+  for (int k = 0; k < count; ++k) {
+    if (!trees[k]) {
+      set_error(std::string(fn) + ": tree " + std::to_string(k) + " is NULL");
+      return MADICP_ERR_INVALID;
+    }
+    if (trees[k]->ctx != trees[0]->ctx) {
+      set_error(std::string(fn) + ": trees 0 and " + std::to_string(k) + " live on different contexts");
+      return MADICP_ERR_INVALID;
+    }
+    n += trees[k]->n_leaves;
+  }
+  if (n >= (int64_t(1) << 31)) {
+    set_error(std::string(fn) + ": more than 2^31 - 1 leaves in one call");
+    return MADICP_ERR_INVALID;
+  }
+  *ctx = trees[0]->ctx;
+  *total = int(n);
+  return MADICP_OK;
+}
+
+// The tree table through the next pinned ring entry to its device copy, then k_leaf_means into `out` (device memory),
+// all on the context's stream.  The host waits only when the ring wraps around a gather that has not run yet, or when
+// the table outgrows every earlier one.
+static int leaf_gather_launch(madicp_ctx* c, const madtree_gpu_t* const* trees, const double* const* X, int count, int total,
+                              double* out) {
+  if (size_t(count) > c->cap_gather) {
+    for (int i = 0; i < madicp_ctx::kGatherRing; ++i) CK(cudaEventSynchronize(c->gather_done[i]));
+    cudaFreeHost(c->h_gather);
+    cudaFree(c->d_gather);
+    c->h_gather = c->d_gather = nullptr;
+    c->cap_gather = 0;
+    CK(cudaMallocHost(&c->h_gather, size_t(madicp_ctx::kGatherRing) * size_t(count) * sizeof(LeafGather)));
+    CK(cudaMalloc(&c->d_gather, size_t(madicp_ctx::kGatherRing) * size_t(count) * sizeof(LeafGather)));
+    c->cap_gather = size_t(count);
+  }
+  const int r = int(c->gather_seq % madicp_ctx::kGatherRing);
+  if (c->gather_seq >= madicp_ctx::kGatherRing) CK(cudaEventSynchronize(c->gather_done[r]));
+  LeafGather* h = c->h_gather + size_t(r) * c->cap_gather;
+  LeafGather* d = c->d_gather + size_t(r) * c->cap_gather;
+  int row = 0;
+  for (int k = 0; k < count; ++k) {
+    LeafGather g{};
+    g.recs = trees[k]->recs;
+    g.leaf_of = trees[k]->leaf_of;
+    g.out = row;
+    g.n_leaves = trees[k]->n_leaves;
+    g.has_pose = (X && X[k]) ? 1 : 0;
+    if (g.has_pose) memcpy(g.X, X[k], 12 * sizeof(double));
+    h[k] = g;
+    row += g.n_leaves;
+  }
+  CK(cudaMemcpyAsync(d, h, size_t(count) * sizeof(LeafGather), cudaMemcpyHostToDevice, c->stream));
+  k_leaf_means<<<blocks_for(total), kStepBlock, 0, c->stream>>>(d, count, total, out);
+  c->launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(c->gather_done[r], c->stream));  // (after the kernel: it reads the device copy of the entry)
+  c->gather_seq++;
+  return MADICP_OK;
+}
+
 extern "C" {
 
 int madtree_gpu_upload(madicp_ctx_t* c, const madtree_t* tree, madtree_gpu_t** out) {
@@ -695,6 +781,46 @@ int madtree_gpu_download(const madtree_gpu_t* t, madtree_rec_t* recs_out, int32_
     CK(cudaMemcpyAsync(leaf_records_out, t->leaf_of, size_t(t->n_leaves) * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return MADICP_OK;
+}
+
+int madtree_gpu_leaf_means(const madtree_gpu_t* const* trees, const double* const* X, int count, double* means_out) {
+  madicp_ctx* c = nullptr;
+  int total = 0;
+  if (int rc = leaf_gather_check(trees, count, means_out, "madtree_gpu_leaf_means", &c, &total)) return rc;
+  if (total == 0) return 0;
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  if (size_t(total) > c->cap_leaves) {  // (only this call uses the buffers, and it returns with the stream idle)
+    cudaFree(c->d_leaves);
+    cudaFreeHost(c->h_leaves);
+    c->d_leaves = c->h_leaves = nullptr;
+    c->cap_leaves = 0;
+    const size_t cap = size_t(total) + size_t(total) / 4 + 1024;
+    CK(cudaMalloc(&c->d_leaves, cap * 3 * sizeof(double)));
+    CK(cudaMallocHost(&c->h_leaves, cap * 3 * sizeof(double)));
+    c->cap_leaves = cap;
+  }
+  if (int rc = leaf_gather_launch(c, trees, X, count, total, c->d_leaves)) return rc;
+  CK(cudaMemcpyAsync(c->h_leaves, c->d_leaves, size_t(total) * 3 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  memcpy(means_out, c->h_leaves, size_t(total) * 3 * sizeof(double));
+  return total;
+  MADICP_CATCH("madtree_gpu_leaf_means")
+}
+
+int madtree_gpu_leaf_means_dev(const madtree_gpu_t* const* trees, const double* const* X, int count, double* means_out,
+                               void* consumer_stream) {
+  madicp_ctx* c = nullptr;
+  int total = 0;
+  if (int rc = leaf_gather_check(trees, count, means_out, "madtree_gpu_leaf_means_dev", &c, &total)) return rc;
+  if (!c) return 0;
+  if (int rc = madicp_check_device_ptr(c, means_out, 8, "madtree_gpu_leaf_means_dev (output)")) return rc;
+  if (total == 0) return 0;
+  CK(cudaSetDevice(c->device));
+  if (int rc = madicp_stream_wait(c, c->stream, consumer_stream)) return rc;  // the output is allocated there
+  if (int rc = leaf_gather_launch(c, trees, X, count, total, means_out)) return rc;
+  if (int rc = madicp_stream_wait(c, consumer_stream, c->stream)) return rc;
+  return total;
 }
 
 int madicp_put_keyframe_tree(madicp_ctx_t* c, int slot, const madtree_gpu_t* t, const double X[12]) {

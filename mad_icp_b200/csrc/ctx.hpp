@@ -72,6 +72,17 @@ struct madicp_ctx {
   int* h_lvl = nullptr;
   cudaEvent_t xform_done[kXformRing] = {};
   uint32_t xform_seq = 0;
+  // leaf-mean gathers (madtree_gpu_leaf_means*): their tree tables go up through a pinned ring (kGatherRing tables of
+  // cap_gather entries) into as many device tables, stream-ordered; the host form's means come back through h_leaves
+  static constexpr int kGatherRing = 8;
+  madicp::LeafGather* h_gather = nullptr;
+  madicp::LeafGather* d_gather = nullptr;
+  size_t cap_gather = 0;
+  cudaEvent_t gather_done[kGatherRing] = {};
+  uint32_t gather_seq = 0;
+  double* d_leaves = nullptr;  // host form: L x 3 on the device, then in pinned memory
+  double* h_leaves = nullptr;
+  size_t cap_leaves = 0;
   std::vector<madtree_gpu*> tree_cache;  // freed device trees keep their memory for the next scan
   std::vector<void*> tree_slabs;         // the allocations the trees are carved from
   cudaEvent_t tree_free_ev = nullptr;    // recorded on the context's stream at every madtree_gpu_free

@@ -207,6 +207,35 @@ k_prepare_moving(double* __restrict__ means, int L, const __grid_constant__ IcpP
   out[q] = m;
 }
 
+// Leaf means of several device trees in one launch (MADtree::getLeafs, tools/mad_tree.cpp:154-163, tree after tree): row
+// table[k].out + o of `out` is the mean of the k-th tree's leaf of ordinal o, posed by the tree's X as
+// MADtree::applyTransform would (iso_apply: the node transform's operand order, no FMA).  A tree without a pose is
+// copied: an identity transform would still turn -0.0 into +0.0.  The table is ordered by `out`.
+__global__ void __launch_bounds__(kStepBlock)
+k_leaf_means(const LeafGather* __restrict__ table, int count, int total, double* __restrict__ out) {
+  const int i = blockIdx.x * kStepBlock + threadIdx.x;
+  if (i >= total) return;
+  int lo = 0, hi = count;  // the last tree whose first row is <= i (trees without leaves share their successor's row)
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (table[mid].out <= i) lo = mid; else hi = mid;
+  }
+  const LeafGather& g = table[lo];
+  const madtree_rec_t* r = g.recs + g.leaf_of[i - g.out];
+  double x = r->mean[0], y = r->mean[1], z = r->mean[2];
+  if (g.has_pose) {
+    double X[12];
+#pragma unroll
+    for (int j = 0; j < 12; ++j) X[j] = g.X[j];
+    double px, py, pz;
+    iso_apply(X, x, y, z, px, py, pz);
+    x = px; y = py; z = pz;
+  }
+  out[3 * size_t(i)] = x;
+  out[3 * size_t(i) + 1] = y;
+  out[3 * size_t(i) + 2] = z;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Step API: K1 / K2 / K3
 // ---------------------------------------------------------------------------------------------

@@ -98,24 +98,49 @@ class MADtree {
   int numLeaves() const { return t_ ? madtree_num_leaves(t_) : madtree_gpu_num_leaves(g_); }
   int numNodes() const { return t_ ? madtree_num_nodes(t_) : madtree_gpu_num_nodes(g_); }
   // reference: getLeafs(back_inserter) (mad_tree.cpp:154-163) -> leaf->mean_ (in the frame applyTransform put it in)
-  ContainerType leafMeans() const {
-    ContainerType out(static_cast<size_t>(numLeaves()));
-    if (out.empty()) return out;
-    if (t_) {
-      check(madtree_leaves(t_, out[0].data(), nullptr, nullptr, nullptr), "madtree_leaves");
-    } else {
-      const size_t nn = size_t(numNodes());
-      std::vector<madtree_rec_t> recs(nn);
-      std::vector<int32_t> leaf(out.size());
-      check(madtree_gpu_download(g_, recs.data(), leaf.data()), "madtree_gpu_download");
-      for (size_t i = 0; i < out.size(); ++i) std::memcpy(out[i].data(), recs[size_t(leaf[i])].mean, 24);
-    }
-    if (has_pose_)
-      for (auto& p : out) {  // R*p + t, rows as (a*x + b*y) + c*z, translation last: the node transform's arithmetic
-        const double x = p[0], y = p[1], z = p[2];
-        for (int r = 0; r < 3; ++r) p[size_t(r)] = ((pose_[r * 4] * x + pose_[r * 4 + 1] * y) + pose_[r * 4 + 2] * z) + pose_[r * 4 + 3];
-      }
+  ContainerType leafMeans() const { return leafMeans({this}); }
+  // the same for several trees, tree after tree: sum(numLeaves) x 3 doubles
+  static size_t numLeaves(const std::vector<const MADtree*>& trees) {
+    size_t n = 0;
+    for (const MADtree* t : trees) n += size_t(t->numLeaves());
+    return n;
+  }
+  static ContainerType leafMeans(const std::vector<const MADtree*>& trees) {
+    ContainerType out(numLeaves(trees));
+    if (!out.empty()) leafMeans(trees, out[0].data());
     return out;
+  }
+  // Host output.  Device trees (one context) are gathered and posed on the device in one call; host-built trees are
+  // read and posed here.
+  static void leafMeans(const std::vector<const MADtree*>& trees, double* out) {
+    if (!trees.empty() && trees[0]->g_) {
+      std::vector<const madtree_gpu_t*> g;
+      std::vector<const double*> X;
+      deviceTable(trees, g, X);
+      check(madtree_gpu_leaf_means(g.data(), X.data(), int(g.size()), out), "madtree_gpu_leaf_means");
+      return;
+    }
+    for (const MADtree* t : trees) {
+      if (!t->t_) throw Error("MADtree.leafMeans: host-built and device trees in one call");
+      const size_t n = size_t(t->numLeaves());
+      if (n == 0) continue;
+      check(madtree_leaves(t->t_, out, nullptr, nullptr, nullptr), "madtree_leaves");
+      if (t->has_pose_)
+        for (size_t i = 0; i < n; ++i) {  // R*p + t, rows as (a*x + b*y) + c*z, translation last: the node transform's arithmetic
+          double* p = out + 3 * i;
+          const double x = p[0], y = p[1], z = p[2], *X = t->pose_;
+          for (int r = 0; r < 3; ++r) p[r] = ((X[r * 4] * x + X[r * 4 + 1] * y) + X[r * 4 + 2] * z) + X[r * 4 + 3];
+        }
+      out += 3 * n;
+    }
+  }
+  // Device output (device memory of the trees' device), ready on consumer_stream with no host sync; device trees only.
+  static void leafMeansDev(const std::vector<const MADtree*>& trees, double* out, void* consumer_stream) {
+    if (trees.empty()) return;
+    std::vector<const madtree_gpu_t*> g;
+    std::vector<const double*> X;
+    deviceTable(trees, g, X);
+    check(madtree_gpu_leaf_means_dev(g.data(), X.data(), int(g.size()), out, consumer_stream), "madtree_gpu_leaf_means_dev");
   }
   const madtree_t* hostHandle() const { return t_; }
   const madtree_gpu_t* deviceHandle() const { return g_; }
@@ -130,6 +155,14 @@ class MADtree {
   static uint64_t next_uid() {
     static uint64_t counter = 0;
     return ++counter;
+  }
+  static void deviceTable(const std::vector<const MADtree*>& trees, std::vector<const madtree_gpu_t*>& g,
+                          std::vector<const double*>& X) {
+    for (const MADtree* t : trees) {
+      if (!t->g_) throw Error("MADtree.leafMeans: a device gather needs device trees");
+      g.push_back(t->g_);
+      X.push_back(t->pose());
+    }
   }
   madtree_t* t_ = nullptr;
   madtree_gpu_t* g_ = nullptr;

@@ -255,6 +255,7 @@ class Pipeline {
         realtime_(realtime), icp_(b_max, rho_ker, b_ratio, num_threads, resolveDevice(device), std::max(num_keyframes, 1)),
         vel_(sensor_hz) {
     frame_to_map_ = keyframe_to_map_ = detail::poseIdentity();
+    device_ = resolveDevice(device);
     if (const char* e = std::getenv("MADICP_GPU_BUILD")) gpu_build_ = std::atoi(e) != 0;
     num_threads_ = std::max(num_threads, 1);
     int lvl = 0;
@@ -289,15 +290,17 @@ class Pipeline {
   size_t keyframeID() const { return seq_keyframe_; }
   double inliersRatio() const { return inliers_ratio_; }
   size_t numKeyframes() const { return keyframes_.size(); }
-  ContainerType currentLeaves() const { return current_ ? current_->tree->leafMeans() : ContainerType(); }
-  ContainerType modelLeaves() const {
-    ContainerType all;
-    for (const auto& f : keyframes_) {
-      ContainerType l = f->tree->leafMeans();
-      all.insert(all.end(), l.begin(), l.end());
-    }
-    return all;
+  ContainerType currentLeaves() const { return MADtree::leafMeans(leafTrees(false)); }
+  // every keyframe's leaves in keyframes_ order, each posed by its own pose: one gather on the device
+  ContainerType modelLeaves() const { return MADtree::leafMeans(leafTrees(true)); }
+  // the same as N x 3 doubles into caller memory: numLeaves(model) rows, host memory, or device memory of device() ready
+  // on consumer_stream with no host sync (device-built trees only)
+  size_t numLeaves(bool model) const { return MADtree::numLeaves(leafTrees(model)); }
+  void leafMeans(bool model, double* out) const { MADtree::leafMeans(leafTrees(model), out); }
+  void leafMeansDev(bool model, double* out, void* consumer_stream) const {
+    MADtree::leafMeansDev(leafTrees(model), out, consumer_stream);
   }
+  int device() const { return device_; }
 
   // test hook: the deskew step alone (poses 4x4 row-major)
   static ContainerType deskewOnly(ContainerType cloud, const Matrix4d& T_prev, const Matrix4d& T_now, double sensor_hz,
@@ -404,6 +407,15 @@ class Pipeline {
   size_t prefetched() { return lookahead_ ? lookahead_->size() : 0; }
 
  private:
+  // the trees of currentLeaves (model == false) or modelLeaves
+  std::vector<const MADtree*> leafTrees(bool model) const {
+    std::vector<const MADtree*> trees;
+    if (model)
+      for (const auto& f : keyframes_) trees.push_back(f->tree.get());
+    else if (current_)
+      trees.push_back(current_->tree.get());
+    return trees;
+  }
   // the scan's MAD-tree: ingest (+ deskew, pipeline.cpp:137-138) and build, on the device or on the host
   std::unique_ptr<MADtree> makeTree(const void* xyz, size_t n, bool is_f32, const madicp_points_t* records,
                                     const madicp_vcorr_t* vc, const DevScan* dev) {
@@ -586,6 +598,7 @@ class Pipeline {
   int num_keyframes_, max_parallel_levels_ = 0;
   bool realtime_;
   bool gpu_build_ = true;   // MADICP_GPU_BUILD=0: host-built trees
+  int device_ = 0;
   int num_threads_ = 1;
   int last_iters_ = 0;
   double round_ms_ = 0.0;   // duration of one GN round on the previous scan (realtime budget)

@@ -40,6 +40,16 @@ static madicp_vcorr_t vcorr_arg(bool apply_correction, double vertical_angle_off
   return v;
 }
 
+// currentLeaves (model == false) / modelLeaves as an (N, 3) float64 numpy array, or with `device` as a float64 CUDA tensor
+// on the pipeline's device, written in place and ready on torch's current stream (records.leaves_array_dev)
+static py::object leaves_array(const py::object& self, bool model, bool device) {
+  if (device) return py::module_::import("mad_icp_b200.records").attr("leaves_array_dev")(self, model);
+  const mb::Pipeline& p = self.cast<const mb::Pipeline&>();
+  py::array_t<double> out({p.numLeaves(model), size_t(3)});
+  if (out.shape(0)) p.leafMeans(model, out.mutable_data());
+  return std::move(out);
+}
+
 PYBIND11_MODULE(pypeline, m) {
   bind_vector_eigen3d(m);
   // KittiReader.vertical_angle_offset, np.radians(0.205), as records.py computes it: the default bit for bit
@@ -62,6 +72,16 @@ PYBIND11_MODULE(pypeline, m) {
       .def("keyframeID", &mb::Pipeline::keyframeID)
       .def("modelLeaves", &mb::Pipeline::modelLeaves)
       .def("currentLeaves", &mb::Pipeline::currentLeaves)
+      // additions (not in the reference): the same points as arrays, gathered on the device, or as CUDA tensors
+      .def("currentLeavesArray", [](const py::object& self, bool device) { return leaves_array(self, false, device); },
+           py::arg("device") = false)
+      .def("modelLeavesArray", [](const py::object& self, bool device) { return leaves_array(self, true, device); },
+           py::arg("device") = false)
+      .def("_numLeaves", &mb::Pipeline::numLeaves)
+      .def("_device", &mb::Pipeline::device)
+      .def("_leafMeansDev", [](const mb::Pipeline& p, bool model, uintptr_t out, uintptr_t stream) {
+        p.leafMeansDev(model, reinterpret_cast<double*>(out), reinterpret_cast<void*>(stream));
+      })
       .def("compute", [](mb::Pipeline& p, double stamp, py::object cloud) {
         // read the points where they are: a bound VectorEigen3d by reference, a numpy array through its buffer, a device
         // array in place (as records without a gate)

@@ -98,6 +98,15 @@ struct __align__(32) Moving4 {
   double px, py, pz, ball;
 };
 
+// One tree of a leaf-mean gather (k_leaf_means): its records and getLeafs table, its first output row, its pose
+// (row-major [R|t], read only when has_pose != 0).  128 bytes.
+struct LeafGather {
+  const madtree_rec_t* recs;
+  const int* leaf_of;
+  int out, n_leaves, has_pose, pad;
+  double X[12];
+};
+
 // Control block + results of one registration, in device global memory.
 // LL-style mailbox cell: a double split into two 32-bit halves, each paired with a 32-bit epoch
 // flag, written with ONE 16-byte store so data and flags arrive together (no fence on the wire).

@@ -105,6 +105,10 @@ class DeviceTree:
         check(capi.lib().madtree_gpu_download(self._h, None, as_i(out)), "madtree_gpu_download")
         return out
 
+    def leaf_means(self, T=None, device=False):
+        """The tree's leaf means in getLeafs order, posed by T (4x4 / 3x4, or None: untouched); see `leaf_means`."""
+        return leaf_means([self], [T], device)
+
     def export(self):
         """Audit dump of a device-BUILT tree, breadth-first: mean, eivecs (column-major), bbox, num_points."""
         n = self.num_nodes
@@ -112,6 +116,33 @@ class DeviceTree:
         check(capi.lib().madtree_gpu_export(self._h, as_d(out["mean"]), as_d(out["eivecs"]), as_d(out["bbox"]),
                                             as_i(out["num_points"])), "madtree_gpu_export")
         return out
+
+
+def leaf_means(trees, poses=None, device=False):
+    """Leaf means of DeviceTrees of one Registrar, in getLeafs order, tree after tree, gathered in one launch
+    (madtree_gpu_leaf_means): poses[k] (4x4 / 3x4, or None) is applied as MADtree::applyTransform would, a tree without a
+    pose is copied untouched.  An (N, 3) float64 numpy array, or with device=True a float64 torch tensor on the
+    registrar's device, written in place and ready on torch's current stream (madtree_gpu_leaf_means_dev)."""
+    trees = list(trees)
+    poses = [None] * len(trees) if poses is None else list(poses)
+    if len(poses) != len(trees):
+        raise ValueError("leaf_means: one pose (or None) per tree")
+    k = len(trees)
+    Xs = [None if T is None else pose12(T) for T in poses]
+    tab = (C.c_void_p * k)(*[t._h for t in trees])
+    xtab = (capi.dp * k)(*[as_d(X) if X is not None else None for X in Xs])
+    n = sum(t.num_leaves for t in trees)
+    if not device:
+        out = np.empty((n, 3))
+        check(capi.lib().madtree_gpu_leaf_means(tab, xtab, k, as_d(out)), "madtree_gpu_leaf_means")
+        return out
+    import torch
+    dev = torch.device("cuda", trees[0]._reg.device if trees else 0)
+    out = torch.empty((n, 3), dtype=torch.float64, device=dev)
+    check(capi.lib().madtree_gpu_leaf_means_dev(tab, xtab, k, C.c_void_p(out.data_ptr()),
+                                                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+          "madtree_gpu_leaf_means_dev")
+    return out
 
 
 class DeskewPlan:
@@ -504,4 +535,4 @@ class Registrar:
         return capi.lib().madicp_comm_world(self._h)
 
 
-__all__ = ["FlatTree", "DeviceTree", "Registrar", "MadIcpError"]
+__all__ = ["FlatTree", "DeviceTree", "Registrar", "MadIcpError", "leaf_means"]

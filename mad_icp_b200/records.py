@@ -199,6 +199,21 @@ def search_cloud_arrays_dev(search_dev, queries):
     return P, N, D
 
 
+def leaves_array_dev(pipeline, model):
+    """Pipeline.currentLeavesArray / modelLeavesArray(device=True): the leaf means as an (N, 3) float64 torch tensor on the
+    pipeline's device, written by the gather kernel in place and ready on torch's current stream (no host sync).  With
+    host-built trees (MADICP_GPU_BUILD=0) the host array is copied up once."""
+    import torch
+    dev = torch.device("cuda", pipeline._device())
+    if not pipeline.gpuBuild():
+        return torch.from_numpy(pipeline.modelLeavesArray() if model else pipeline.currentLeavesArray()).to(dev)
+    n = pipeline._numLeaves(model)
+    out = torch.empty((n, 3), dtype=torch.float64, device=dev)
+    if n:
+        pipeline._leafMeansDev(model, out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+    return out
+
+
 def vcorr(apply_correction=False, vertical_angle_offset=VERTICAL_ANGLE_OFFSET):
     """madicp_vcorr_t of the reader's `apply_correction` / `vertical_angle_offset`, or None without a correction."""
     if not apply_correction:
@@ -236,5 +251,5 @@ def correct_vertical_angle(records, vertical_angle_offset=VERTICAL_ANGLE_OFFSET,
     return out[:kept]
 
 
-__all__ = ["pointcloud2_dtype", "describe", "layout", "to_host", "search_cloud_arrays_dev", "range_mask", "vcorr", "correct_vertical_angle",
+__all__ = ["pointcloud2_dtype", "describe", "layout", "to_host", "search_cloud_arrays_dev", "leaves_array_dev", "range_mask", "vcorr", "correct_vertical_angle",
            "VERTICAL_ANGLE_OFFSET", "RANGE_NONE", "RANGE_INCLUSIVE", "RANGE_STRICT"]

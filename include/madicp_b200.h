@@ -308,6 +308,51 @@ int madtree_gpu_build_batch_points_dev(madicp_ctx_t* ctx, const madicp_points_t*
 int madicp_plan_points_dev(madicp_ctx_t* ctx, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int num_threads,
                            void* producer_stream, madicp_plan_t** out);
 
+/* ---------------- deskew by per-point time stamps (not in the reference) ------------------------------------------
+ * A scan may carry a time field: one little-endian scalar per record at byte `offset`, uint32, float32 or float64.
+ * With it a deskew needs no azimuth order.  Each kept point i (after the gate, the NaN drop and the correction, in
+ * record order) takes its chunk from its own stamp tau_i:
+ *   u_i = (double(tau_i) - double(t_end)) * scale          seconds, <= 0 for points before t_end
+ *   s_i = rint(((-u_i) * sensor_hz) * (CHUNKS - 1))        steps back from the newest chunk; IEEE float64, no FMA,
+ *                                                           round half to even, in exactly this order
+ *   k_i = CHUNKS - 1 - clamp(s_i, 0, CHUNKS - 1)           CHUNKS = 1024 (tools/constants.h)
+ *   p_i' = pose[k_i] * p_i                                  pose[k]: the azimuth deskew's chunk table (t accumulated
+ *                                                           from -1/sensor_hz, odometry/pipeline.cpp:100-119)
+ * scale: seconds per unit (1e-9 for nanoseconds), finite and > 0.  t_end (field units, finite) is used when has_t_end
+ * != 0; otherwise it is the largest time among the kept points.  The kept points stay in record order (no sort), so
+ * the tree is built from them as the sensor gave them.  A kept point whose time is NaN or infinite fails the call with
+ * MADICP_ERR_STATE (read at the next host synchronisation, as a correction outside its table is).  Without a deskew the
+ * time field is read and ignored: the cloud is the one the call without it gives, bit for bit.
+ * Invalid (MADICP_ERR_INVALID, with a message): a field outside the stride or misaligned for its type (offset and
+ * stride multiples of its size), an unknown type, scale <= 0 or not finite, t_end not finite. */
+#define MADICP_TIME_NONE 0
+#define MADICP_TIME_U32 1
+#define MADICP_TIME_F32 2
+#define MADICP_TIME_F64 3
+typedef struct madicp_times {
+  int32_t offset; /* byte offset of the field in the record */
+  int32_t type;   /* MADICP_TIME_*; MADICP_TIME_NONE: no time field */
+  double scale;   /* seconds per unit */
+  double t_end;   /* field units, used when has_t_end != 0 */
+  int32_t has_t_end;
+  int32_t reserved;
+} madicp_times_t;
+/* The record calls with a time field: times (nullable: none) next to the correction.  Deskewing with a time field runs
+ * the whole per-point deskew on the device: no sort, no copy of the points to the host.  A plan with a time field does
+ * the gate, the correction and the compaction on the context's stream at once, without a host thread; consuming it
+ * applies the chunk poses.  Staging and batch builds take no time field: a deskewed scan is never part of a forest. */
+int madicp_ingest_points_t(madicp_ctx_t* ctx, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
+                           const madicp_times_t* times, int deskew, const double T_prev[12], const double T_now[12],
+                           double sensor_hz, int num_threads, int64_t* n_kept, double* points_out);
+int madicp_ingest_points_dev_t(madicp_ctx_t* ctx, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
+                               const madicp_times_t* times, int deskew, const double T_prev[12], const double T_now[12],
+                               double sensor_hz, int num_threads, void* producer_stream, int64_t* n_kept,
+                               double* points_out);
+int madicp_plan_points_t(madicp_ctx_t* ctx, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
+                         const madicp_times_t* times, int num_threads, madicp_plan_t** out);
+int madicp_plan_points_dev_t(madicp_ctx_t* ctx, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
+                             const madicp_times_t* times, int num_threads, void* producer_stream, madicp_plan_t** out);
+
 /* K1 only -- MADtree::bestMatchingLeafFast (tools/mad_tree.cpp:144-152) of X*mean for every moving
  * leaf against every active keyframe.  out_ordinals: K_active x L int32 on the host (row k = k-th
  * active slot in ascending slot order); values are getLeafs ordinals of the matched leaf. */

@@ -73,6 +73,17 @@ int madicp_debug_deskew_plan(const madicp_points_t* desc, const madicp_vcorr_t* 
                              const double T_now[12], double sensor_hz, int split, int num_threads, int32_t* perm,
                              uint16_t* chunk, double* poses, int* n_poses, int64_t* n_kept);
 
+/* The chunk of every kept point of a scan with a time field (madicp_times_t): the gate, the correction's table check and
+ * the chunk rule of include/madicp_b200.h restated on the host, the same arithmetic the device applies.  chunk_out
+ * receives *n_kept entries (room for desc->n).  MADICP_ERR_STATE when a kept point's time is NaN or infinite or its
+ * rotation angle falls outside the correction's table.  No device work. */
+int madicp_debug_time_chunks(const madicp_points_t* desc, const madicp_vcorr_t* vcorr, const madicp_times_t* times,
+                             double sensor_hz, uint16_t* chunk_out, int64_t* n_kept);
+/* The chunk poses of the deskew (both kinds): n_chunks x 12 row-major, the motion from T_prev to T_now.  No device
+ * work. */
+int madicp_debug_chunk_poses(const double T_prev[12], const double T_now[12], double sensor_hz, int n_chunks,
+                             double* poses);
+
 #ifdef __cplusplus
 }
 #endif

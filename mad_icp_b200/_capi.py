@@ -35,6 +35,16 @@ class Vcorr(C.Structure):
 
 vc_p = C.POINTER(Vcorr)
 
+
+class Times(C.Structure):
+    """madicp_times_t: a per-point time field (offset, type MADICP_TIME_*, seconds per unit, optional sweep end)."""
+    _fields_ = [("offset", C.c_int32), ("type", C.c_int32), ("scale", C.c_double), ("t_end", C.c_double),
+                ("has_t_end", C.c_int32), ("reserved", C.c_int32)]
+
+
+assert C.sizeof(Times) == 32
+tm_p = C.POINTER(Times)
+
 # every symbol include/madicp_b200.h and include/madicp_b200_debug.h declare: name -> (restype, argtypes)
 SYMBOLS = {
     "madicp_last_error": (C.c_char_p, []),
@@ -93,6 +103,14 @@ SYMBOLS = {
                                            dp]),
     "madtree_gpu_build_batch_points_dev": (C.c_int, [vp, pts_p, vc_p, C.c_int, C.c_double, C.c_double, vp, C.POINTER(vp)]),
     "madicp_plan_points_dev": (C.c_int, [vp, pts_p, vc_p, C.c_int, vp, C.POINTER(vp)]),
+    "madicp_ingest_points_t": (C.c_int, [vp, pts_p, vc_p, tm_p, C.c_int, dp, dp, C.c_double, C.c_int, C.POINTER(C.c_int64),
+                                         dp]),
+    "madicp_ingest_points_dev_t": (C.c_int, [vp, pts_p, vc_p, tm_p, C.c_int, dp, dp, C.c_double, C.c_int, vp,
+                                             C.POINTER(C.c_int64), dp]),
+    "madicp_plan_points_t": (C.c_int, [vp, pts_p, vc_p, tm_p, C.c_int, C.POINTER(vp)]),
+    "madicp_plan_points_dev_t": (C.c_int, [vp, pts_p, vc_p, tm_p, C.c_int, vp, C.POINTER(vp)]),
+    "madicp_debug_time_chunks": (C.c_int, [pts_p, vc_p, tm_p, C.c_double, C.POINTER(C.c_uint16), C.POINTER(C.c_int64)]),
+    "madicp_debug_chunk_poses": (C.c_int, [dp, dp, C.c_double, C.c_int, dp]),
     "madicp_search_cloud_dev": (C.c_int, [vp, C.c_int, vp, C.c_int64, C.c_int64, C.c_int, vp, vp, vp, vp, vp]),
     "madicp_debug_deskew_plan": (C.c_int, [pts_p, vc_p, dp, dp, C.c_double, C.c_int, C.c_int, ip,
                                            C.POINTER(C.c_uint16), dp, C.POINTER(C.c_int), C.POINTER(C.c_int64)]),

@@ -14,6 +14,7 @@
 #include <deque>
 #include <limits>
 
+#include "../../../include/madicp_b200_debug.h"
 #include "../pose_math.h"
 #include "../records.hpp"
 #include "facade.hpp"
@@ -111,6 +112,7 @@ class Lookahead {
     bool records = false;             // raw sensor records (Pipeline::prefetchRecords): `pts` describes them, `vc` is
     madicp_points_t pts{};            // their vertical correction (disabled: none)
     madicp_vcorr_t vc{};
+    madicp_times_t tm{};              // a deskewed scan's time field (none: the azimuth deskew)
     bool dev = false;                 // records in device memory, ready on `stream` (DevScan): never staged
     void* stream = nullptr;
     std::shared_ptr<void> keepalive;
@@ -137,8 +139,9 @@ class Lookahead {
     fifo_.push_back(std::move(j));
     Job& q = fifo_.back();  // (planned where its private copy, if any, will stay)
     const madicp_points_t d = q.records ? q.pts : madicp::packed_points(q.data(), int64_t(q.n), q.is_f32 ? 1 : 0);
-    const int rc = q.dev ? madicp_plan_points_dev(ctx_, &d, &q.vc, num_threads, q.stream, &q.plan)
-                         : madicp_plan_points(ctx_, &d, q.records ? &q.vc : nullptr, num_threads, &q.plan);
+    const int rc = q.dev ? madicp_plan_points_dev_t(ctx_, &d, &q.vc, &q.tm, num_threads, q.stream, &q.plan)
+                         : madicp_plan_points_t(ctx_, &d, q.records ? &q.vc : nullptr, q.records ? &q.tm : nullptr,
+                                                num_threads, &q.plan);
     if (rc < 0) {
       const std::string msg = "madicp_plan_points failed (" + std::to_string(rc) + "): " + madicp_last_error();
       fifo_.pop_back();
@@ -336,16 +339,26 @@ class Pipeline {
   // same restatement, then the host path runs.
   // dev (nullable): the records are device memory, read in place (host-built trees, MADICP_GPU_BUILD=0, need host records:
   // the caller copies them over first)
-  void computeRecords(double stamp, const madicp_points_t& pts, const madicp_vcorr_t* vc = nullptr, const DevScan* dev = nullptr) {
+  // tm (nullable): the records' time field; a deskewed scan with one takes each point's chunk from its own stamp
+  // (include/madicp_b200.h, madicp_times_t) instead of the azimuth order.  Without a deskew it is ignored.
+  void computeRecords(double stamp, const madicp_points_t& pts, const madicp_vcorr_t* vc = nullptr, const DevScan* dev = nullptr,
+                      const madicp_times_t* tm = nullptr) {
     check(madicp::check_vcorr(vc, "Pipeline.computeRecords"), "Pipeline.computeRecords");
     if (dev && !gpu_build_) throw Error("Pipeline.computeRecords: device records need device-built trees (MADICP_GPU_BUILD)");
+    if (tm && tm->type != madicp::kTimeNone) {
+      check(madicp::check_points(&pts, "Pipeline.computeRecords"), "Pipeline.computeRecords");
+      check(madicp::check_times(tm, &pts, "Pipeline.computeRecords"), "Pipeline.computeRecords");
+    }
+    const madicp_times_t t = madicp::times_of(tm);
     if (!gpu_build_) {
-      compute(stamp, packRecords(pts, vc));
+      const ContainerType cloud = packRecords(pts, vc);
+      const madicp_vcorr_t v = madicp::vcorr_of(vc);
+      computeRaw(stamp, cloud[0].data(), cloud.size(), false, t.type ? &pts : nullptr, &v, nullptr, t.type ? &t : nullptr);
       return;
     }
     if (!pts.data || pts.n <= 0) throw Error("Pipeline.computeRecords: empty scan");
     const madicp_vcorr_t v = madicp::vcorr_of(vc);
-    computeRaw(stamp, pts.data, size_t(pts.n), pts.is_f32 != 0, &pts, &v, dev);
+    computeRaw(stamp, pts.data, size_t(pts.n), pts.is_f32 != 0, &pts, &v, dev, t.type ? &t : nullptr);
   }
   bool gpuBuild() const { return gpu_build_; }
   int lastIcpIterations() const { return last_iters_; }  // rounds the realtime budget allowed for the last scan
@@ -360,7 +373,7 @@ class Pipeline {
   // plan consumed.
   bool prefetch(const void* xyz, size_t n, bool is_f32, std::shared_ptr<void> keepalive = nullptr,
                 const madicp_points_t* records = nullptr, const madicp_vcorr_t* vc = nullptr, bool deskew_ahead = false,
-                const DevScan* dev = nullptr) {
+                const DevScan* dev = nullptr, const madicp_times_t* tm = nullptr) {
     if (!gpu_build_ || (deskew_ && !deskew_ahead) || !xyz || n == 0) return false;
     const auto p0 = clk();
     struct Tick {  // (the hand-over runs on the thread that launches the registrations: its cost is part of the scan's)
@@ -381,7 +394,9 @@ class Pipeline {
       // a descriptor the library would reject must not enter the queue (every later batch would fail on it)
       check(madicp::check_points(records, "Pipeline.prefetchRecords"), "Pipeline.prefetchRecords");
       check(madicp::check_vcorr(vc, "Pipeline.prefetchRecords"), "Pipeline.prefetchRecords");
+      check(madicp::check_times(tm, records, "Pipeline.prefetchRecords"), "Pipeline.prefetchRecords");
       j.records = true;
+      if (deskew_) j.tm = madicp::times_of(tm);  // (a scan that is not deskewed goes into a batch build: no time field)
       j.pts = *records;
       j.vc = madicp::vcorr_of(vc);
       j.dev = dev != nullptr;
@@ -400,9 +415,9 @@ class Pipeline {
     return true;
   }
   bool prefetchRecords(const madicp_points_t& pts, std::shared_ptr<void> keepalive, const madicp_vcorr_t* vc = nullptr,
-                       bool deskew_ahead = false, const DevScan* dev = nullptr) {
+                       bool deskew_ahead = false, const DevScan* dev = nullptr, const madicp_times_t* tm = nullptr) {
     return prefetch(pts.data, pts.n > 0 ? size_t(pts.n) : 0, pts.is_f32 != 0, std::move(keepalive), &pts, vc, deskew_ahead,
-                    dev);
+                    dev, tm);
   }
   size_t prefetched() { return lookahead_ ? lookahead_->size() : 0; }
 
@@ -417,8 +432,10 @@ class Pipeline {
     return trees;
   }
   // the scan's MAD-tree: ingest (+ deskew, pipeline.cpp:137-138) and build, on the device or on the host
+  // tm (nullable): the records' time field.  Host-built trees (MADICP_GPU_BUILD=0): xyz is the packed kept cloud and
+  // `records` the scan it came from, for the stamps.
   std::unique_ptr<MADtree> makeTree(const void* xyz, size_t n, bool is_f32, const madicp_points_t* records,
-                                    const madicp_vcorr_t* vc, const DevScan* dev) {
+                                    const madicp_vcorr_t* vc, const DevScan* dev, const madicp_times_t* tm) {
     const bool dsk = deskew_ && is_initialized_ && trajectory_.size() > 1;
     const double* Ta = dsk ? trajectory_[trajectory_.size() - 2].m : nullptr;
     const double* Tb = dsk ? trajectory_[trajectory_.size() - 1].m : nullptr;
@@ -430,14 +447,14 @@ class Pipeline {
     if (lookahead_ && !lookahead_->empty())  // built ahead of time by a worker lane
       return std::unique_ptr<MADtree>(new MADtree(icp_.context(), lookahead_->pop(), b_max_));
     if (gpu_build_ && records && dev) {
-      check(madicp_ingest_points_dev(icp_.context(), records, vc, dsk ? 1 : 0, Ta, Tb, sensor_hz_,
-                                     std::max(1 << max_parallel_levels_, 1), dev->stream, nullptr, nullptr),
+      check(madicp_ingest_points_dev_t(icp_.context(), records, vc, tm, dsk ? 1 : 0, Ta, Tb, sensor_hz_,
+                                       std::max(1 << max_parallel_levels_, 1), dev->stream, nullptr, nullptr),
             "madicp_ingest_points_dev");
       return std::unique_ptr<MADtree>(new MADtree(icp_.context(), b_max_, b_min_));
     }
     if (gpu_build_ && records) {
-      check(madicp_ingest_points_ex(icp_.context(), records, vc, dsk ? 1 : 0, Ta, Tb, sensor_hz_,
-                                    std::max(1 << max_parallel_levels_, 1), nullptr, nullptr), "madicp_ingest_points");
+      check(madicp_ingest_points_t(icp_.context(), records, vc, tm, dsk ? 1 : 0, Ta, Tb, sensor_hz_,
+                                   std::max(1 << max_parallel_levels_, 1), nullptr, nullptr), "madicp_ingest_points");
       return std::unique_ptr<MADtree>(new MADtree(icp_.context(), b_max_, b_min_));
     }
     if (gpu_build_) {
@@ -446,6 +463,17 @@ class Pipeline {
       return std::unique_ptr<MADtree>(new MADtree(icp_.context(), b_max_, b_min_));
     }
     const double* pts = static_cast<const double*>(xyz);
+    if (dsk && tm && records) {  // the host restatement of the time-stamp deskew (madicp_debug_time_chunks)
+      std::vector<uint16_t> chunk(size_t(records->n));
+      int64_t kept = 0;
+      check(madicp_debug_time_chunks(records, vc, tm, sensor_hz_, chunk.data(), &kept), "madicp_debug_time_chunks");
+      if (size_t(kept) != n) throw Error("Pipeline.computeRecords: internal error (kept count)");
+      std::vector<detail::Pose> poses(kChunks);
+      check(madicp_debug_chunk_poses(Ta, Tb, sensor_hz_, kChunks, poses[0].m), "madicp_debug_chunk_poses");
+      ContainerType cloud(n);
+      for (size_t i = 0; i < n; ++i) madicp_pose::poseApply(poses[chunk[i]], pts + 3 * i, cloud[i].data());
+      return std::unique_ptr<MADtree>(new MADtree(cloud[0].data(), n, b_max_, b_min_, max_parallel_levels_));
+    }
     if (dsk) {
       ContainerType cloud(n);
       std::memcpy(cloud[0].data(), pts, sizeof(double) * 3 * n);
@@ -456,7 +484,7 @@ class Pipeline {
   }
 
   void computeRaw(double stamp, const void* xyz, size_t n, bool is_f32, const madicp_points_t* records = nullptr,
-                  const madicp_vcorr_t* vc = nullptr, const DevScan* dev = nullptr) {
+                  const madicp_vcorr_t* vc = nullptr, const DevScan* dev = nullptr, const madicp_times_t* tm = nullptr) {
     if (!xyz || n == 0) throw Error("Pipeline.compute: empty cloud");
     is_map_updated_ = false;
     if (!is_initialized_) {  // pipeline.cpp:267-284
@@ -464,7 +492,7 @@ class Pipeline {
       f->frame = int(seq_);
       f->to_map = frame_to_map_;
       f->stamp = stamp;
-      f->tree = makeTree(xyz, n, is_f32, records, vc, dev);
+      f->tree = makeTree(xyz, n, is_f32, records, vc, dev, tm);
       keyframes_.push_back(f);
       current_ = f;
       trajectory_.push_back(detail::poseIdentity());
@@ -475,7 +503,7 @@ class Pipeline {
     const auto c0 = clk();
     const auto c1 = c0;
     auto cur = std::make_shared<FrameB>();
-    cur->tree = makeTree(xyz, n, is_f32, records, vc, dev);
+    cur->tree = makeTree(xyz, n, is_f32, records, vc, dev, tm);
     const auto c2 = clk();
     double t[3], w[3];
     for (int a = 0; a < 3; ++a) {

@@ -32,6 +32,19 @@ static madicp_points_t records_arg(const py::object& records, double min_range, 
   return d;
 }
 
+// time_field / time_scale / time_end -> madicp_times_t (records.time_layout; type MADICP_TIME_NONE without a field)
+static madicp_times_t times_arg(const py::object& records, const py::object& field, double scale, const py::object& t_end) {
+  madicp_times_t t{};
+  if (field.is_none()) return t;
+  const py::tuple l = py::module_::import("mad_icp_b200.records").attr("time_layout")(records, field, scale, t_end).cast<py::tuple>();
+  t.offset = l[0].cast<int32_t>();
+  t.type = l[1].cast<int32_t>();
+  t.scale = l[2].cast<double>();
+  t.t_end = l[3].cast<double>();
+  t.has_t_end = l[4].cast<int32_t>();
+  return t;
+}
+
 // apply_correction / vertical_angle_offset (KittiReader's names) -> madicp_vcorr_t
 static madicp_vcorr_t vcorr_arg(bool apply_correction, double vertical_angle_offset) {
   madicp_vcorr_t v{};
@@ -143,33 +156,41 @@ PYBIND11_MODULE(pypeline, m) {
       // additions (not in the reference): raw sensor records, filtered on the way in like the dataset readers do
       // (mad_icp_b200/records.py describes the array; it is read in place); apply_correction: KITTI's vertical-angle
       // correction of the kept points, as KittiReader applies it
+      // time_field (a structured field name, or a column index of a 2-D array): the records' per-point time stamps, in
+      // units of time_scale seconds; a deskewing pipeline takes each point's chunk from its own stamp (time_end: the
+      // sweep's end in field units, default the largest kept stamp) -- no azimuth sort
       .def("computeRecords", [](mb::Pipeline& p, double stamp, const py::object& records, double min_range, double max_range,
-                                bool inclusive, bool drop_nan, bool apply_correction, double vertical_angle_offset) {
+                                bool inclusive, bool drop_nan, bool apply_correction, double vertical_angle_offset,
+                                const py::object& time_field, double time_scale, const py::object& time_end) {
         const madicp_vcorr_t v = vcorr_arg(apply_correction, vertical_angle_offset);
         const py::object recs = (on_device(records) && !p.gpuBuild()) ? to_host(records) : records;
         mb::DevScan dev;
         bool is_dev = false;
         const madicp_points_t d = records_arg(recs, min_range, max_range, inclusive, drop_nan, &dev, &is_dev);
-        p.computeRecords(stamp, d, &v, is_dev ? &dev : nullptr);
+        const madicp_times_t t = times_arg(recs, time_field, time_scale, time_end);
+        p.computeRecords(stamp, d, &v, is_dev ? &dev : nullptr, t.type ? &t : nullptr);
       }, py::arg("stamp"), py::arg("records"), py::arg("min_range") = 0.0,
          py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false,
-         py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle)
+         py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle, py::arg("time_field") = py::none(),
+         py::arg("time_scale") = 1.0, py::arg("time_end") = py::none())
       // deskew_ahead (prefetch, prefetchRecords): on a deskewing pipeline the scan is planned ahead -- uploaded, gated,
       // corrected and sorted by azimuth while earlier scans register -- and compute applies its chunk poses
       .def("prefetchRecords", [](mb::Pipeline& p, const py::object& records, double min_range, double max_range,
                                  bool inclusive, bool drop_nan, bool apply_correction, double vertical_angle_offset,
-                                 bool deskew_ahead) {
+                                 bool deskew_ahead, const py::object& time_field, double time_scale, const py::object& time_end) {
         if (on_device(records) && !p.gpuBuild()) return false;  // (host-built trees: no look-ahead)
         mb::DevScan dev;
         bool is_dev = false;
         const madicp_points_t d = records_arg(records, min_range, max_range, inclusive, drop_nan, &dev, &is_dev);
         const madicp_vcorr_t v = vcorr_arg(apply_correction, vertical_angle_offset);
+        const madicp_times_t t = times_arg(records, time_field, time_scale, time_end);
         py::object* ref = new py::object(records);  // dropped once the scan's tree is built (see prefetch)
         return p.prefetchRecords(d, std::shared_ptr<void>(ref, [](void* q) { delete static_cast<py::object*>(q); }), &v,
-                                 deskew_ahead, is_dev ? &dev : nullptr);
+                                 deskew_ahead, is_dev ? &dev : nullptr, t.type ? &t : nullptr);
       }, py::arg("records"), py::arg("min_range") = 0.0,
          py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false,
-         py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle, py::arg("deskew_ahead") = false)
+         py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle, py::arg("deskew_ahead") = false,
+         py::arg("time_field") = py::none(), py::arg("time_scale") = 1.0, py::arg("time_end") = py::none())
       .def("prefetched", &mb::Pipeline::prefetched)
       .def("lastIcpIterations", &mb::Pipeline::lastIcpIterations)
       .def("gpuBuild", &mb::Pipeline::gpuBuild)

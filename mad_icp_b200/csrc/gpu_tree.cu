@@ -92,6 +92,10 @@ struct BuildState {
   std::vector<double> vtab_angle;      // angle of slot k
   int* h_vc_err = nullptr;             // mapped: a corrected point's rotation angle fell outside its table
   bool vc_check = false;               // the resident cloud was corrected: the next build checks h_vc_err
+  // time-stamp deskew (time_deskew.h): the largest kept stamp's key, and a kept stamp that is NaN or infinite (mapped)
+  unsigned long long* d_tmax = nullptr;
+  int* h_t_err = nullptr;
+  bool time_check = false;             // the resident cloud was deskewed by its stamps: the next build checks h_t_err
   int* d_perm = nullptr;
   unsigned short* d_chunk = nullptr;
   double* d_poses = nullptr;
@@ -237,6 +241,8 @@ int ensure_state(void** slot, cudaStream_t stream, size_t n, size_t raw_bytes, B
   if (!rc) rc = dev_alloc(bs, &bs->d_vtab, size_t(kMaxBatch));
   if (!rc) rc = host_alloc(bs, &bs->h_vtab, size_t(kMaxBatch));
   if (!rc) rc = host_alloc(bs, &bs->h_vc_err, 1);
+  if (!rc) rc = dev_alloc(bs, &bs->d_tmax, 1);
+  if (!rc) rc = host_alloc(bs, &bs->h_t_err, 1);
   if (!rc) rc = dev_alloc(bs, &bs->d_perm, cap);
   if (!rc) rc = dev_alloc(bs, &bs->d_chunk, cap);
   if (!rc) rc = dev_alloc(bs, &bs->d_poses, size_t(65536) * 12);
@@ -513,6 +519,10 @@ int build_forest(madicp_ctx* c, BuildState* bs, cudaStream_t st, int n_trees, co
       set_error("madtree_gpu_build: a point's rotation angle lies outside the table of the vertical correction");
       return MADICP_ERR_STATE;
     }
+    if (depth == 0 && bs->time_check && *bs->h_t_err) {
+      set_error("madtree_gpu_build: a kept point's time stamp is NaN or infinite");
+      return MADICP_ERR_STATE;
+    }
     if (depth == 0)
       for (int b = 0; b < check_kept; ++b)
         if (bs->h_kept[b] != offs[b + 1] - offs[b]) {
@@ -720,6 +730,42 @@ int launch_compaction(madicp_ctx* c, BuildState* bs, cudaStream_t st, const RecB
   CK(cudaGetLastError());
   return MADICP_OK;
 }
+// The device side of a time field (TimeArgs, gpu_tree_kernels.cuh).  base: the scan's first record on the device (a
+// float64 field is read with one 64-bit load where it is 8-byte aligned: offset and stride are multiples of 8); poses /
+// tau_out select what pass 2 writes.
+TimeArgs time_args(const madicp_times_t& tm, const void* base, double sensor_hz, unsigned long long* tmax, int* err,
+                   const double* poses, double* tau_out) {
+  TimeArgs T{};
+  T.off = tm.offset;
+  T.type = tm.type;
+  T.wide = reinterpret_cast<uintptr_t>(base) % 8 == 0 ? 1 : 0;
+  T.has_t_end = tm.has_t_end;
+  T.scale = tm.scale;
+  T.t_end = tm.t_end;
+  T.sensor_hz = sensor_hz;
+  T.tmax = tmax;
+  T.err = err;
+  T.poses = poses;
+  T.tau_out = tau_out;
+  return T;
+}
+// launch_compaction for a one-scan batch with a time field: passes 1 and 2 of the time-stamp deskew (T.tmax and T.err
+// are reset first).  With T.poses the chunk poses must already be queued on `st`.
+int launch_compaction_time(madicp_ctx* c, BuildState* bs, cudaStream_t st, const RecBatch& B, const TimeArgs& T, double* out,
+                           int* kept, int* vc_err, bool vc) {
+  CK(cudaMemsetAsync(T.tmax, 0, sizeof(unsigned long long), st));
+  CK(cudaMemsetAsync(T.err, 0, sizeof(int), st));
+  const int tiles = (B.n_rec + kTile - 1) / kTile;
+  k_gate_flags_time<<<blocks(B.n_rec), kBlock, 0, st>>>(B, bs->flag, T);
+  k_scan_tiles<<<tiles, kTile, 0, st>>>(bs->flag, B.n_rec, bs->G, bs->tile);
+  k_scan_tile_sums<<<1, 1024, 0, st>>>(bs->tile, tiles);
+  auto k = vc ? k_compact_time<true> : k_compact_time<false>;
+  k<<<blocks(std::max(B.n_rec, B.count)), kBlock, 0, st>>>(B, bs->flag, bs->G, bs->tile, out, kept, bs->d_vtab, vc_err, T);
+  c->launches += 4;
+  CK(cudaGetLastError());
+  return MADICP_OK;
+}
+std::string time_not_finite(const char* fn) { return std::string(fn) + ": a kept point's time stamp is NaN or infinite"; }
 
 // The batch build behind madtree_gpu_build_batch and madtree_gpu_build_batch_points[_ex|_dev] (descriptors and
 // corrections validated; vcorrs nullable).  dev: the scans are in device memory (the context's stream already waits for
@@ -777,6 +823,7 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* v
   bs->has_root_S = false;
   bs->kept_check = 0;
   bs->vc_check = corrected;
+  bs->time_check = false;
   if (!direct) {
     RecBatch B;
     B.count = count;
@@ -855,6 +902,7 @@ int stage(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int
     bs->has_root_S = false;
     bs->kept_check = 0;
     bs->vc_check = false;
+    bs->time_check = false;
   }
   const size_t at = align16(bs->staged_bytes);
   if (bs->staged_raw != raw || size_t(bs->staged_points + d.n) > bs->cap || (raw && at + bytes > bs->raw_cap) ||
@@ -896,14 +944,23 @@ struct PlanBuf {
   cudaEvent_t free_ev = nullptr;  // context stream: the last ingest that read the device buffers has run
   // a plan of device records (madicp_plan_points_dev): d_raw holds its kept points, compacted and corrected as packed
   // float64 on the context's stream; the order half reads them back
-  int* h_cnt = nullptr;              // mapped: [0] kept points, [1] a correction fell outside its table
+  int* h_cnt = nullptr;              // mapped: [0] kept points, [1] a correction fell outside its table, [2] a kept time
+                                     // stamp is NaN or infinite
   double* h_pts = nullptr;           // pinned, 3 x cap, at first use: the kept points for the order half
   cudaEvent_t compacted = nullptr;   // context stream: the compaction has run
+  // a plan with a time field (madicp_plan_points_t): its kept points, corrected, and their stamps, compacted on the
+  // context's stream; d_tmax: the largest kept stamp's key.  At first use.
+  double* d_pts = nullptr;
+  double* d_tau = nullptr;
+  unsigned long long* d_tmax = nullptr;
 };
 void free_buf(PlanBuf* b) {
   if (b->ready) cudaEventSynchronize(b->ready);
   if (b->free_ev) cudaEventSynchronize(b->free_ev);
   if (b->compacted) cudaEventSynchronize(b->compacted);
+  cudaFree(b->d_pts);
+  cudaFree(b->d_tau);
+  cudaFree(b->d_tmax);
   cudaFree(b->d_raw);
   cudaFree(b->d_perm);
   cudaFree(b->d_chunk);
@@ -1023,7 +1080,7 @@ int plan_buf(PlanLane* L, size_t n, size_t bytes, PlanBuf** out) {
   if (e == cudaSuccess) e = cudaHostAlloc(&b->h_chunk, b->cap * sizeof(uint16_t), 0);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->ready, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->free_ev, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaHostAlloc(&b->h_cnt, 2 * sizeof(int), cudaHostAllocMapped);
+  if (e == cudaSuccess) e = cudaHostAlloc(&b->h_cnt, 4 * sizeof(int), cudaHostAllocMapped);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->compacted, cudaEventDisableTiming);
   if (e != cudaSuccess) {
     free_buf(b);
@@ -1046,6 +1103,7 @@ struct madicp_plan {
   madicp_points_t d{};
   madicp_vcorr_t vc{};
   bool dev = false;  // device records: buf->d_raw holds the kept points (PlanBuf)
+  madicp_times_t tm{};  // a time field (tm.type != kTimeNone): no order half, buf->d_pts / d_tau hold the kept points
   PlanBuf* buf = nullptr;
   std::promise<void> done_p;
   std::future<void> done;  // the order half has run and its uploads are queued
@@ -1106,6 +1164,7 @@ void plan_order(madicp_plan* p) {
 void plan_release(madicp_plan* p, bool wait_uploads) {
   p->done.wait();
   if (wait_uploads) cudaEventSynchronize(p->buf->ready);
+  if (wait_uploads && p->tm.type != kTimeNone) cudaEventSynchronize(p->buf->compacted);  // (it reads the records too)
   return_buf(p->lane, p->buf);
   delete p;
 }
@@ -1156,9 +1215,11 @@ int ingest_done(BuildState* bs, cudaStream_t st, int64_t kept, int64_t* n_kept, 
 // for uploaded records, and the kept count comes back from the device (one synchronisation).  deskew: the kept points
 // are compacted into P[1], copied back for the host's order half (madicp_deskew_plan over a packed, plain cloud -- the
 // same points, so the same permutation and chunks), and gathered from there into P[0].
+// With a time field and a deskew the whole deskew is the compaction's pass 2 (launch_compaction_time), straight into P[0].
 int ingest_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int deskew, const double T_prev[12],
                const double T_now[12], double sensor_hz, int num_threads, int64_t* n_kept, double* points_out,
-               const char* fn) {
+               const char* fn, const madicp_times_t& tm = madicp_times_t{}) {
+  const bool timed = deskew && tm.type != kTimeNone;
   BuildState* bs = nullptr;
   int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
   if (!rc) rc = ensure_state(c, size_t(d.n), 0, &bs);
@@ -1167,6 +1228,7 @@ int ingest_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc
   bs->n_resident = 0;
   bs->kept_check = 0;
   bs->vc_check = false;  // (an angle outside the table fails this call)
+  bs->time_check = false;
   int64_t kept = d.n;
   if (is_direct(d, vc) && !deskew) {
     CK(cudaMemcpyAsync(bs->P[0], d.data, size_t(d.n) * 24, cudaMemcpyDeviceToDevice, st));
@@ -1179,10 +1241,22 @@ int ingest_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc
     B.count = 1;
     B.n_rec = int(d.n);
     B.s[0] = rec_src(d, d.data, 0, slot);
-    if (int e = launch_compaction(c, bs, st, B, deskew ? bs->P[1] : bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) return e;
+    if (timed) {
+      PlanLane* L = nullptr;
+      if (int e = plan_lane(c, &L)) return e;
+      if (int e = stage_chunk_poses(L, st, T_prev, T_now, sensor_hz, kTimeChunks, bs->d_poses)) return e;
+      const TimeArgs T = time_args(tm, d.data, sensor_hz, bs->d_tmax, bs->h_t_err, bs->d_poses, nullptr);
+      if (int e = launch_compaction_time(c, bs, st, B, T, bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) return e;
+    } else if (int e = launch_compaction(c, bs, st, B, deskew ? bs->P[1] : bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) {
+      return e;
+    }
     CK(cudaStreamSynchronize(st));
     if (vc.enabled && *bs->h_vc_err) {
       set_error(vcorr_out_of_table(fn, vc.angle));
+      return MADICP_ERR_STATE;
+    }
+    if (timed && *bs->h_t_err) {
+      set_error(time_not_finite(fn));
       return MADICP_ERR_STATE;
     }
     kept = bs->h_kept[0];
@@ -1191,7 +1265,7 @@ int ingest_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc
     set_error(std::string(fn) + ": no point inside the range gate");
     return MADICP_ERR_INVALID;
   }
-  if (deskew) {
+  if (deskew && !timed) {
     if (!bs->h_packed)
       if (int e = host_alloc(bs, &bs->h_packed, 3 * bs->cap)) return e;
     CK(cudaMemcpyAsync(bs->h_packed, bs->P[1], size_t(kept) * 24, cudaMemcpyDeviceToHost, st));
@@ -1230,6 +1304,7 @@ int ingest_planned_dev(madicp_ctx* c, madicp_plan* plan, int deskew, const doubl
   bs->n_resident = 0;
   bs->kept_check = 0;
   bs->vc_check = false;
+  bs->time_check = false;
   const int64_t kept = plan->kept;
   const double* pts = reinterpret_cast<const double*>(plan->buf->d_raw);
   CK(cudaStreamWaitEvent(st, plan->buf->ready, 0));
@@ -1245,12 +1320,57 @@ int ingest_planned_dev(madicp_ctx* c, madicp_plan* plan, int deskew, const doubl
   return ingest_done(bs, st, kept, n_kept, points_out);
 }
 
-// The ingest behind madicp_ingest, madicp_ingest_points[_ex] and madicp_ingest_plan (descriptor and correction
-// validated).  plan (nullable): the scan's records are already on their way up, with its deskew order (madicp_plan_points).
+// madicp_ingest_plan of a plan with a time field: its kept points and their stamps were compacted on the context's stream
+// when it was handed over (plan_time); what is left is the chunk poses and one k_deskew_times.
+int ingest_planned_time(madicp_ctx* c, madicp_plan* plan, int deskew, const double T_prev[12], const double T_now[12],
+                        double sensor_hz, int64_t* n_kept, double* points_out, const char* fn) {
+  CK(cudaSetDevice(c->device));
+  PlanBuf* b = plan->buf;
+  CK(cudaEventSynchronize(b->compacted));  // (long done when the plan was handed over ahead of its turn)
+  if (b->h_cnt[1]) {
+    set_error(vcorr_out_of_table(fn, plan->vc.angle));
+    return MADICP_ERR_STATE;
+  }
+  if (deskew && b->h_cnt[2]) {
+    set_error(time_not_finite(fn));
+    return MADICP_ERR_STATE;
+  }
+  const int64_t kept = b->h_cnt[0];
+  if (kept == 0) {
+    set_error(std::string(fn) + ": no point inside the range gate");
+    return MADICP_ERR_INVALID;
+  }
+  BuildState* bs = nullptr;
+  int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
+  if (!rc) rc = ensure_state(c, size_t(plan->d.n), 0, &bs);
+  if (rc) return rc;
+  cudaStream_t st = c->stream;
+  bs->n_resident = 0;
+  bs->kept_check = 0;
+  bs->vc_check = false;
+  bs->time_check = false;
+  if (deskew) {
+    if (int e = stage_chunk_poses(plan->lane, st, T_prev, T_now, sensor_hz, kTimeChunks, bs->d_poses)) return e;
+    const TimeArgs T = time_args(plan->tm, nullptr, sensor_hz, b->d_tmax, nullptr, bs->d_poses, nullptr);
+    k_deskew_times<<<blocks(kept), kBlock, 0, st>>>(b->d_pts, b->d_tau, int(kept), T, bs->P[0]);
+    c->launches++;
+  } else {
+    CK(cudaMemcpyAsync(bs->P[0], b->d_pts, size_t(kept) * 24, cudaMemcpyDeviceToDevice, st));
+  }
+  CK(cudaEventRecord(b->free_ev, st));  // (the plan's buffers may be reused once this has run)
+  return ingest_done(bs, st, kept, n_kept, points_out);
+}
+
+// The ingest behind madicp_ingest, madicp_ingest_points[_ex|_t] and madicp_ingest_plan (descriptor, correction and time
+// field validated).  plan (nullable): the scan's records are already on their way up, with its deskew order
+// (madicp_plan_points).  tm: a time field; with a deskew the whole deskew is the compaction's pass 2 on the device.
 int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int deskew, const double T_prev[12],
            const double T_now[12], double sensor_hz, int num_threads, madicp_plan* plan, int64_t* n_kept, double* points_out,
-           const char* fn) {
+           const char* fn, const madicp_times_t& tm = madicp_times_t{}) {
+  if (plan && plan->tm.type != kTimeNone)
+    return ingest_planned_time(c, plan, deskew, T_prev, T_now, sensor_hz, n_kept, points_out, fn);
   if (plan && plan->dev) return ingest_planned_dev(c, plan, deskew, T_prev, T_now, sensor_hz, n_kept, points_out, fn);
+  const bool timed = deskew && tm.type != kTimeNone && !plan;
   CK(cudaSetDevice(c->device));
   BuildState* bs = nullptr;
   const int64_t n = d.n;
@@ -1262,12 +1382,13 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
   bs->n_resident = 0;
   bs->kept_check = 0;
   bs->vc_check = vc.enabled != 0;
+  bs->time_check = false;
   const char* raw = static_cast<const char*>(bs->d_raw);
   if (plan) {  // the records, the permutation and the chunks went up on the plan lane's stream
     CK(cudaStreamWaitEvent(st, plan->buf->ready, 0));
     raw = plan->buf->d_raw;
   } else {  // the raw scan goes up while the host works out the order (deskew) or the root's sums
-    CK(cudaMemcpyAsync(bs->d_raw, d.data, points_bytes(d), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(bs->d_raw, d.data, timed ? points_bytes(d, tm) : points_bytes(d), cudaMemcpyHostToDevice, st));
   }
   int slot = -1;
   if (vc.enabled) CK(cudaMemsetAsync(bs->h_vc_err, 0, sizeof(int), st));
@@ -1290,6 +1411,15 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
                                          bs->d_vtab, bs->h_vc_err);
       c->launches++;
     }
+  } else if (timed) {  // no order, no host half: the chunk poses through the pinned ring, then passes 1 and 2
+    PlanLane* L = nullptr;
+    if (int e = plan_lane(c, &L)) return e;
+    if (int e = stage_chunk_poses(L, st, T_prev, T_now, sensor_hz, kTimeChunks, bs->d_poses)) return e;
+    const TimeArgs T = time_args(tm, raw, sensor_hz, bs->d_tmax, bs->h_t_err, bs->d_poses, nullptr);
+    if (int e = launch_compaction_time(c, bs, st, B, T, bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) return e;
+    kept = kept_count_host(d);  // (compared with the device's count at the build's first host sync, as the stamps are)
+    bs->kept_check = 1;
+    bs->time_check = true;
   } else if (deskew) {
     CK(cudaStreamSynchronize(st));  // h_perm / h_chunk / h_poses of the previous scan have been consumed
     int n_poses = 0;
@@ -1333,6 +1463,11 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
     CK(cudaStreamSynchronize(st));
     if (bs->vc_check && *bs->h_vc_err) {
       set_error(vcorr_out_of_table(fn, vc.angle));
+      bs->n_resident = 0;
+      return MADICP_ERR_STATE;
+    }
+    if (bs->time_check && *bs->h_t_err) {
+      set_error(time_not_finite(fn));
       bs->n_resident = 0;
       return MADICP_ERR_STATE;
     }
@@ -1475,6 +1610,7 @@ int madtree_gpu_build(madicp_ctx_t* c, const double* points_xyz, int64_t n, doub
   bs->kept_check = 0;
   root_sums_host(packed_points(points_xyz, n, 0), bs->root_S);
   bs->vc_check = false;
+  bs->time_check = false;
   bs->has_root_S = true;
   return build_resident(c, bs, c->stream, n, b_max, b_min, bs->root_S, out);
   MADICP_CATCH("madtree_gpu_build")
@@ -1565,6 +1701,46 @@ int madicp_ingest_points_dev(madicp_ctx_t* c, const madicp_points_t* desc, const
   if (int e = madicp_check_device_ptr(c, desc->data, desc->is_f32 ? 4 : 8, fn)) return e;
   if (int e = madicp_stream_wait(c, c->stream, producer_stream)) return e;
   const int rc = ingest_dev(c, *desc, vcorr_of(vcorr), deskew, T_prev, T_now, sensor_hz, num_threads, n_kept, points_out, fn);
+  CK(cudaStreamSynchronize(c->stream));  // returns once nothing reads the caller's records, whatever the outcome
+  return rc;
+  MADICP_CATCH(fn)
+}
+
+int madicp_ingest_points_t(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
+                           const madicp_times_t* times, int deskew, const double T_prev[12], const double T_now[12],
+                           double sensor_hz, int num_threads, int64_t* n_kept, double* points_out) {
+  const char* fn = "madicp_ingest_points_t";
+  if (!c || (deskew && (!T_prev || !T_now || !(sensor_hz > 0.0)))) {
+    set_error(std::string(fn) + ": bad arguments");
+    return MADICP_ERR_INVALID;
+  }
+  if (int e = check_points(desc, fn)) return e;
+  if (int e = check_vcorr(vcorr, fn)) return e;
+  if (int e = check_times(times, desc, fn)) return e;
+  MADICP_TRY
+  return ingest(c, *desc, vcorr_of(vcorr), deskew, T_prev, T_now, sensor_hz, num_threads, nullptr, n_kept, points_out, fn,
+                times_of(times));
+  MADICP_CATCH(fn)
+}
+
+int madicp_ingest_points_dev_t(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
+                               const madicp_times_t* times, int deskew, const double T_prev[12], const double T_now[12],
+                               double sensor_hz, int num_threads, void* producer_stream, int64_t* n_kept,
+                               double* points_out) {
+  const char* fn = "madicp_ingest_points_dev_t";
+  if (!c || (deskew && (!T_prev || !T_now || !(sensor_hz > 0.0)))) {
+    set_error(std::string(fn) + ": bad arguments");
+    return MADICP_ERR_INVALID;
+  }
+  if (int e = check_points(desc, fn)) return e;
+  if (int e = check_vcorr(vcorr, fn)) return e;
+  if (int e = check_times(times, desc, fn)) return e;
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  if (int e = madicp_check_device_ptr(c, desc->data, desc->is_f32 ? 4 : 8, fn)) return e;
+  if (int e = madicp_stream_wait(c, c->stream, producer_stream)) return e;
+  const int rc = ingest_dev(c, *desc, vcorr_of(vcorr), deskew, T_prev, T_now, sensor_hz, num_threads, n_kept, points_out, fn,
+                            times_of(times));
   CK(cudaStreamSynchronize(c->stream));  // returns once nothing reads the caller's records, whatever the outcome
   return rc;
   MADICP_CATCH(fn)
@@ -1666,6 +1842,111 @@ int madicp_plan_points_dev(madicp_ctx_t* c, const madicp_points_t* desc, const m
   L->submit(std::max(1, std::min(num_threads, 64)), [q]() { plan_order(q); });
   *out = p.release();
   return MADICP_OK;
+  MADICP_CATCH(fn)
+}
+
+namespace {
+// The whole hand-over of a plan with a time field: host records go up on the lane's stream, then on the context's stream
+// (whose build lane holds the compaction's scratch) passes 1 and 2 write the kept points, corrected, and their stamps into
+// the plan's buffer; b->compacted follows.  No host thread: the plan is complete once its kernels have run.
+int plan_time(madicp_ctx* c, madicp_plan* p, void* producer) {
+  PlanBuf* b = p->buf;
+  const madicp_points_t& d = p->d;
+  if (!b->d_pts) {
+    CK(cudaMalloc(&b->d_pts, b->cap * 3 * sizeof(double)));
+    CK(cudaMalloc(&b->d_tau, b->cap * sizeof(double)));
+    CK(cudaMalloc(&b->d_tmax, sizeof(unsigned long long)));
+  }
+  BuildState* bs = static_cast<BuildState*>(c->build_state);
+  if (bs && bs->cap < size_t(d.n))  // the lane is about to be re-allocated: early uploads are lost
+    if (int e = drop_staged(bs, c->stream)) return e;
+  if (int e = ensure_state(c, size_t(d.n), 0, &bs)) return e;
+  cudaStream_t st = c->stream;
+  const void* base = d.data;
+  if (p->dev) {
+    if (int e = madicp_stream_wait(c, st, producer)) return e;
+  } else {  // (once the last ingest that read this buffer has run)
+    CK(cudaStreamWaitEvent(p->lane->stream, b->free_ev, 0));
+    CK(cudaMemcpyAsync(b->d_raw, d.data, points_bytes(d, p->tm), cudaMemcpyHostToDevice, p->lane->stream));
+    CK(cudaEventRecord(b->ready, p->lane->stream));
+    CK(cudaStreamWaitEvent(st, b->ready, 0));
+    base = b->d_raw;
+  }
+  int slot = -1;
+  if (int e = vtab_room(bs, st, &p->vc, 1)) return e;
+  if (int e = vtab_slot(bs, st, p->vc, &slot)) return e;
+  b->h_cnt[0] = b->h_cnt[1] = b->h_cnt[2] = 0;  // (the buffer's last consumer has read them)
+  RecBatch B;
+  B.count = 1;
+  B.n_rec = int(d.n);
+  B.s[0] = rec_src(d, base, 0, slot);
+  const TimeArgs T = time_args(p->tm, base, 0.0, b->d_tmax, b->h_cnt + 2, nullptr, b->d_tau);
+  if (int e = launch_compaction_time(c, bs, st, B, T, b->d_pts, b->h_cnt, b->h_cnt + 1, p->vc.enabled)) return e;
+  CK(cudaEventRecord(b->compacted, st));
+  return MADICP_OK;
+}
+// madicp_plan_points_t / _dev_t with a time field (validated)
+int plan_points_time(madicp_ctx* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, const madicp_times_t* times,
+                     bool dev, void* producer_stream, madicp_plan_t** out, const char* fn) {
+  CK(cudaSetDevice(c->device));
+  if (dev)
+    if (int e = madicp_check_device_ptr(c, desc->data, desc->is_f32 ? 4 : 8, fn)) return e;
+  PlanLane* L = nullptr;
+  if (int e = plan_lane(c, &L)) return e;
+  PlanBuf* b = nullptr;
+  if (int e = plan_buf(L, size_t(desc->n), dev ? 0 : points_bytes(*desc, times_of(times)), &b)) return e;
+  std::unique_ptr<madicp_plan> p(new madicp_plan);
+  p->ctx = c;
+  p->lane = L;
+  p->d = *desc;
+  p->vc = vcorr_of(vcorr);
+  p->tm = times_of(times);
+  p->dev = dev;
+  p->buf = b;
+  p->done = p->done_p.get_future();
+  if (int e = plan_time(c, p.get(), producer_stream)) {
+    cudaStreamSynchronize(c->stream);  // (nothing may still read the records, nor write the buffer)
+    cudaStreamSynchronize(L->stream);
+    return_buf(L, b);
+    return e;
+  }
+  p->done_p.set_value();
+  *out = p.release();
+  return MADICP_OK;
+}
+}  // namespace
+
+int madicp_plan_points_t(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
+                         const madicp_times_t* times, int num_threads, madicp_plan_t** out) {
+  const char* fn = "madicp_plan_points_t";
+  if (!c || !out) {
+    set_error(std::string(fn) + ": bad arguments");
+    return MADICP_ERR_INVALID;
+  }
+  *out = nullptr;
+  if (int e = check_points(desc, fn)) return e;
+  if (int e = check_vcorr(vcorr, fn)) return e;
+  if (int e = check_times(times, desc, fn)) return e;
+  if (!times || times->type == kTimeNone) return madicp_plan_points(c, desc, vcorr, num_threads, out);
+  MADICP_TRY
+  return plan_points_time(c, desc, vcorr, times, false, nullptr, out, fn);
+  MADICP_CATCH(fn)
+}
+
+int madicp_plan_points_dev_t(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
+                             const madicp_times_t* times, int num_threads, void* producer_stream, madicp_plan_t** out) {
+  const char* fn = "madicp_plan_points_dev_t";
+  if (!c || !out) {
+    set_error(std::string(fn) + ": bad arguments");
+    return MADICP_ERR_INVALID;
+  }
+  *out = nullptr;
+  if (int e = check_points(desc, fn)) return e;
+  if (int e = check_vcorr(vcorr, fn)) return e;
+  if (int e = check_times(times, desc, fn)) return e;
+  if (!times || times->type == kTimeNone) return madicp_plan_points_dev(c, desc, vcorr, num_threads, producer_stream, out);
+  MADICP_TRY
+  return plan_points_time(c, desc, vcorr, times, true, producer_stream, out, fn);
   MADICP_CATCH(fn)
 }
 

@@ -23,6 +23,7 @@
 #include "arith.h"
 #include "eig3.h"
 #include "range_gate.h"
+#include "time_deskew.h"
 #include "vertical_correction.h"
 
 namespace madicp {
@@ -933,13 +934,62 @@ k_gate_flags(const __grid_constant__ RecBatch B, unsigned char* __restrict__ fla
   double x, y, z;
   flag[i] = read_record(B.s[rec_scan(B, i)], i, x, y, z) ? 1 : 0;
 }
-// kept (mapped host memory): kept points of every scan, for the build to compare with the host's count; vtab / vc_err:
-// see correct_record.  kVc: some scan of the batch is corrected (without, the kernel is the uncorrected one exactly)
-template <bool kVc>
+// Deskew by per-point time stamps (madicp_times_t, time_deskew.h) of a one-scan batch.  Pass 1 (k_gate_flags_time):
+// the gate flags plus the largest kept stamp (one atomicMax of an integer-ordered key per warp: a max is exact in any
+// order) and the non-finite flag.  Pass 2 (k_compact_time): each kept record at its rank, corrected, and either moved
+// by the pose of its chunk (poses != nullptr) or written as is with its stamp beside it (tau_out, a plan: the rate and
+// the poses come when it is consumed, k_deskew_times).
+struct TimeArgs {
+  int off;          // byte offset of the field from the record start
+  int type;         // kTimeU32 / kTimeF32 / kTimeF64
+  int wide;         // a float64 field is 8-byte aligned in memory: one 64-bit load (else two 32-bit ones)
+  int has_t_end;
+  double scale, t_end, sensor_hz;
+  unsigned long long* tmax;  // device: time_key of the largest finite kept stamp (0 before pass 1)
+  int* err;                  // mapped host memory: a kept stamp is NaN or infinite
+  const double* poses;       // kTimeChunks x 12, or nullptr (pass 2 of a plan)
+  double* tau_out;           // pass 2 of a plan: the stamp of every kept point, at its rank
+};
+__device__ __forceinline__ double read_time(const RecSrc& s, int r, const TimeArgs& T) {
+  const char* p = s.base + (long long)(r - s.first) * s.stride + T.off;
+  if (T.type == kTimeF64) {
+    if (T.wide) return __ldg(reinterpret_cast<const double*>(p));
+    const unsigned lo = __ldg(reinterpret_cast<const unsigned*>(p)), hi = __ldg(reinterpret_cast<const unsigned*>(p + 4));
+    return __hiloint2double(int(hi), int(lo));
+  }
+  if (T.type == kTimeF32) return double(__ldg(reinterpret_cast<const float*>(p)));
+  return double(__ldg(reinterpret_cast<const unsigned*>(p)));
+}
+__device__ __forceinline__ double time_end(const TimeArgs& T) { return T.has_t_end ? T.t_end : time_of_key(*T.tmax); }
+
 __global__ void __launch_bounds__(kBlock)
-k_compact(const __grid_constant__ RecBatch B, const unsigned char* __restrict__ flag,
-          const int* __restrict__ G, const int* __restrict__ tile_off, double* __restrict__ out, int* __restrict__ kept,
-          const VcorrTable* __restrict__ vtab, int* vc_err) {
+k_gate_flags_time(const __grid_constant__ RecBatch B, unsigned char* __restrict__ flag, const __grid_constant__ TimeArgs T) {
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  unsigned long long key = 0;
+  if (i < B.n_rec) {
+    double x, y, z;
+    const RecSrc& s = B.s[rec_scan(B, i)];
+    const bool keep = read_record(s, i, x, y, z);
+    flag[i] = keep ? 1 : 0;
+    if (keep) {
+      const double t = read_time(s, i, T);
+      if (isfinite(t)) key = time_key(t);
+      else *T.err = 1;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) key = max(key, __shfl_xor_sync(0xffffffffu, key, o));
+  if ((threadIdx.x & 31) == 0 && key) atomicMax(T.tmax, key);
+}
+
+// kept (mapped host memory): kept points of every scan, for the build to compare with the host's count; vtab / vc_err:
+// see correct_record.  kVc: some scan of the batch is corrected (without, the kernel is the uncorrected one exactly).
+// kTime: the time-stamp deskew of pass 2 (T, above); k_compact is the kTime = false instance, unchanged.
+template <bool kVc, bool kTime>
+__device__ __forceinline__ void compact_record(const RecBatch& B, const unsigned char* __restrict__ flag,
+                                               const int* __restrict__ G, const int* __restrict__ tile_off,
+                                               double* __restrict__ out, int* __restrict__ kept,
+                                               const VcorrTable* __restrict__ vtab, int* vc_err, const TimeArgs* T) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
   const int n = B.n_rec;
   auto rank = [&](int r) {  // kept records before r
@@ -950,11 +1000,50 @@ k_compact(const __grid_constant__ RecBatch B, const unsigned char* __restrict__ 
   double x, y, z;
   const RecSrc& s = B.s[rec_scan(B, i)];
   read_record(s, i, x, y, z);
+  double t = 0.0;
+  if (kTime) t = read_time(s, i, *T);  // (beside the x/y/z loads)
   if (kVc) correct_record(s, vtab, vc_err, x, y, z);
   const size_t o = size_t(rank(i));
+  if (kTime) {
+    if (T->poses) {
+      const double* X = T->poses + size_t(time_chunk(t, time_end(*T), T->scale, T->sensor_hz)) * 12;
+      double ox, oy, oz;
+      iso_apply(X, x, y, z, ox, oy, oz);
+      x = ox; y = oy; z = oz;
+    } else {
+      T->tau_out[o] = t;
+    }
+  }
   out[3 * o] = x;
   out[3 * o + 1] = y;
   out[3 * o + 2] = z;
+}
+template <bool kVc>
+__global__ void __launch_bounds__(kBlock)
+k_compact(const __grid_constant__ RecBatch B, const unsigned char* __restrict__ flag,
+          const int* __restrict__ G, const int* __restrict__ tile_off, double* __restrict__ out, int* __restrict__ kept,
+          const VcorrTable* __restrict__ vtab, int* vc_err) {
+  compact_record<kVc, false>(B, flag, G, tile_off, out, kept, vtab, vc_err, nullptr);
+}
+template <bool kVc>
+__global__ void __launch_bounds__(kBlock)
+k_compact_time(const __grid_constant__ RecBatch B, const unsigned char* __restrict__ flag,
+               const int* __restrict__ G, const int* __restrict__ tile_off, double* __restrict__ out, int* __restrict__ kept,
+               const VcorrTable* __restrict__ vtab, int* vc_err, const __grid_constant__ TimeArgs T) {
+  compact_record<kVc, true>(B, flag, G, tile_off, out, kept, vtab, vc_err, &T);
+}
+// A consumed time-stamp plan: the n kept points (packed float64, corrected) and their stamps -> out[i] = pose[k_i] * p_i
+__global__ void __launch_bounds__(kBlock)
+k_deskew_times(const double* __restrict__ pts, const double* __restrict__ tau, int n, const __grid_constant__ TimeArgs T,
+               double* __restrict__ out) {
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  if (i >= n) return;
+  const double* X = T.poses + size_t(time_chunk(tau[i], time_end(T), T.scale, T.sensor_hz)) * 12;
+  double ox, oy, oz;
+  iso_apply(X, pts[3 * size_t(i)], pts[3 * size_t(i) + 1], pts[3 * size_t(i) + 2], ox, oy, oz);
+  out[3 * size_t(i)] = ox;
+  out[3 * size_t(i) + 1] = oy;
+  out[3 * size_t(i) + 2] = oz;
 }
 
 // Ingest (odometry/pipeline.cpp:79-123 + the float32 -> float64 conversion of the readers): out[i] = T[chunk[i]] *

@@ -403,3 +403,57 @@ extern "C" int madicp_debug_deskew_plan(const madicp_points_t* desc, const madic
     madicp::set_error("madicp_debug_deskew_plan: a point's rotation angle lies outside the table of the vertical correction");
   return rc;
 }
+
+// The deskew by time stamps on the host (time_deskew.h): the gate, the correction's table check, the default t_end (the
+// largest kept stamp) and the chunk of every kept point, in record order.
+extern "C" int madicp_debug_time_chunks(const madicp_points_t* desc, const madicp_vcorr_t* vcorr, const madicp_times_t* times,
+                                        double sensor_hz, uint16_t* chunk_out, int64_t* n_kept) {
+  const char* fn = "madicp_debug_time_chunks";
+  if (int e = madicp::check_points(desc, fn)) return e;
+  if (int e = madicp::check_vcorr(vcorr, fn)) return e;
+  if (int e = madicp::check_times(times, desc, fn)) return e;
+  if (!times || times->type == madicp::kTimeNone || !(sensor_hz > 0.0) || !std::isfinite(sensor_hz) || !chunk_out || !n_kept) {
+    madicp::set_error(std::string(fn) + ": bad arguments (a time field, a finite rate > 0, outputs)");
+    return MADICP_ERR_INVALID;
+  }
+  const madicp_times_t tm = madicp::times_of(times);
+  madicp::VcorrTable table;
+  const madicp_vcorr_t v = madicp::vcorr_of(vcorr);
+  if (v.enabled) madicp::vcorr_table_fill(v.angle, &table);
+  std::vector<double> tau;
+  tau.reserve(size_t(desc->n));
+  bool bad_angle = false, bad_time = false;
+  unsigned long long tmax = 0;
+  auto run = [&](auto zero) {
+    const madicp::RecReader<decltype(zero)> rd(*desc, v.enabled ? &table : nullptr);
+    for (int64_t i = 0; i < desc->n; ++i) {
+      double x, y, z;
+      if (!rd.kept_point(i, x, y, z, bad_angle)) continue;
+      const double t = madicp::time_at(*desc, tm, i);
+      if (std::isfinite(t)) tmax = std::max(tmax, madicp::time_key(t));
+      else bad_time = true;
+      tau.push_back(t);
+    }
+  };
+  if (desc->is_f32) run(0.0f);
+  else run(0.0);
+  if (bad_angle || bad_time) {
+    madicp::set_error(std::string(fn) + (bad_time ? ": a kept point's time stamp is NaN or infinite"
+                                                   : ": a point's rotation angle lies outside the table of the vertical correction"));
+    return MADICP_ERR_STATE;
+  }
+  const double t_end = tm.has_t_end ? tm.t_end : madicp::time_of_key(tmax);
+  for (size_t i = 0; i < tau.size(); ++i) chunk_out[i] = uint16_t(madicp::time_chunk(tau[i], t_end, tm.scale, sensor_hz));
+  *n_kept = int64_t(tau.size());
+  return MADICP_OK;
+}
+
+extern "C" int madicp_debug_chunk_poses(const double T_prev[12], const double T_now[12], double sensor_hz, int n_chunks,
+                                        double* poses) {
+  if (!T_prev || !T_now || !(sensor_hz > 0.0) || n_chunks < 0 || n_chunks > 65536 || (n_chunks && !poses)) {
+    madicp::set_error("madicp_debug_chunk_poses: bad arguments");
+    return MADICP_ERR_INVALID;
+  }
+  madicp_deskew_poses(T_prev, T_now, sensor_hz, n_chunks, poses);
+  return MADICP_OK;
+}

@@ -10,6 +10,7 @@
 
 #include "../../include/madicp_b200.h"
 #include "range_gate.h"
+#include "time_deskew.h"
 #include "vertical_correction.h"
 
 namespace madicp {
@@ -81,6 +82,57 @@ inline int check_vcorr(const madicp_vcorr_t* v, const char* fn) {
     return MADICP_ERR_INVALID;
   }
   return MADICP_OK;
+}
+
+// The time field of a nullable madicp_times_t (time_deskew.h): none, or its layout and constants (reserved ignored)
+inline madicp_times_t times_of(const madicp_times_t* t) {
+  madicp_times_t o{};
+  if (t && t->type != kTimeNone) {
+    o = *t;
+    o.reserved = 0;
+    if (!o.has_t_end) o.t_end = 0.0;
+    o.has_t_end = o.has_t_end ? 1 : 0;
+  }
+  return o;
+}
+// MADICP_OK, or MADICP_ERR_INVALID with a message naming `fn`: a time field must fit the stride, be aligned for its
+// type, and come with a finite scale > 0 and a finite t_end (when given)
+inline int check_times(const madicp_times_t* t, const madicp_points_t* d, const char* fn) {
+  if (!t || t->type == kTimeNone) return MADICP_OK;
+  auto bad = [fn](const std::string& why) {
+    set_error(std::string(fn) + ": " + why);
+    return MADICP_ERR_INVALID;
+  };
+  if (t->type < kTimeU32 || t->type > kTimeF64) return bad("time field type must be 0 (none), 1 (uint32), 2 (float32) or 3 (float64)");
+  const int64_t e = time_size(t->type);
+  if (t->offset < 0 || t->offset + e > d->stride) return bad("time field does not fit the stride");
+  if (t->offset % e || d->stride % e) return bad("time field is misaligned for its type (offset and stride must be multiples of its size)");
+  if (!(t->scale > 0.0) || !std::isfinite(t->scale)) return bad("time scale must be finite and > 0");
+  if (t->has_t_end && !std::isfinite(t->t_end)) return bad("time t_end must be finite");
+  return MADICP_OK;
+}
+// points_bytes with the time field: what a scan with one is read up to
+inline size_t points_bytes(const madicp_points_t& d, const madicp_times_t& t) {
+  if (t.type == kTimeNone) return points_bytes(d);
+  const size_t end = size_t((d.n - 1) * d.stride + t.offset + time_size(t.type));
+  return std::max(points_bytes(d), end);
+}
+// record i's time as float64 (exact for every type)
+inline double time_at(const madicp_points_t& d, const madicp_times_t& t, int64_t i) {
+  const char* r = static_cast<const char*>(d.data) + i * d.stride + t.offset;
+  if (t.type == kTimeF64) {
+    double v;
+    std::memcpy(&v, r, 8);
+    return v;
+  }
+  if (t.type == kTimeF32) {
+    float v;
+    std::memcpy(&v, r, 4);
+    return double(v);
+  }
+  uint32_t v;
+  std::memcpy(&v, r, 4);
+  return double(v);
 }
 
 // The gate of one descriptor in field type T, and the correction (nullable table) of its kept points

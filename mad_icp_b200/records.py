@@ -23,19 +23,24 @@ import math
 
 import numpy as np
 
-from ._capi import Points, Vcorr
+from ._capi import Points, Times, Vcorr
 
 RANGE_NONE, RANGE_INCLUSIVE, RANGE_STRICT = 0, 1, 2
 # KittiReader.vertical_angle_offset: the reader's own expression, so the default is its value bit for bit
 VERTICAL_ANGLE_OFFSET = float(np.radians(0.205))
 
 _POINTFIELD_TYPES = {7: np.dtype("<f4"), 8: np.dtype("<f8")}  # sensor_msgs/PointField FLOAT32, FLOAT64
+_POINTFIELD_TIME_TYPES = {6: np.dtype("<u4"), 7: np.dtype("<f4"), 8: np.dtype("<f8")}  # UINT32, FLOAT32, FLOAT64
+TIME_NONE, TIME_U32, TIME_F32, TIME_F64 = 0, 1, 2, 3  # madicp_times_t.type
+_TIME_TYPES = {np.dtype("<u4"): TIME_U32, np.dtype("<f4"): TIME_F32, np.dtype("<f8"): TIME_F64}
 
 
-def pointcloud2_dtype(msg):
+def pointcloud2_dtype(msg, time_field=None):
     """numpy dtype of the records of a sensor_msgs/PointCloud2 message with fields x, y, z (duck-typed: any object with
     `fields` (name, offset, datatype[, count]), `point_step`, `width`, `height`, `row_step`, `is_bigendian`).  Use it as
-    `np.frombuffer(msg.data, pointcloud2_dtype(msg), count=msg.width * msg.height)`."""
+    `np.frombuffer(msg.data, pointcloud2_dtype(msg), count=msg.width * msg.height)`.  time_field (e.g. "t" of an Ouster,
+    "time" of a Velodyne, "timestamp" of a Hesai): that field is kept too, for the time-stamp deskew; it must be UINT32
+    (6), FLOAT32 (7) or FLOAT64 (8)."""
     if getattr(msg, "is_bigendian", False):
         raise ValueError("pointcloud2_dtype: big-endian PointCloud2 is not supported")
     step = int(msg.point_step)
@@ -53,8 +58,20 @@ def pointcloud2_dtype(msg):
         raise ValueError("pointcloud2_dtype: the message has no x, y and z fields")
     if len({found[k][0] for k in found}) != 1:
         raise ValueError("pointcloud2_dtype: x, y and z do not share one float type")
-    return np.dtype({"names": ["x", "y", "z"], "formats": [found[k][0] for k in "xyz"],
-                     "offsets": [found[k][1] for k in "xyz"], "itemsize": step})
+    names, formats, offsets = ["x", "y", "z"], [found[k][0] for k in "xyz"], [found[k][1] for k in "xyz"]
+    if time_field is not None:
+        f = next((f for f in msg.fields if f.name == time_field), None)
+        if f is None or time_field in ("x", "y", "z"):
+            raise ValueError(f"pointcloud2_dtype: the message has no time field {time_field!r}")
+        if int(getattr(f, "count", 1)) != 1:
+            raise ValueError(f"pointcloud2_dtype: field {f.name} has count {f.count}")
+        if int(f.datatype) not in _POINTFIELD_TIME_TYPES:
+            raise ValueError(f"pointcloud2_dtype: time field {f.name} has datatype {f.datatype} "
+                             "(UINT32 = 6, FLOAT32 = 7 or FLOAT64 = 8 only)")
+        names.append(time_field)
+        formats.append(_POINTFIELD_TIME_TYPES[int(f.datatype)])
+        offsets.append(int(f.offset))
+    return np.dtype({"names": names, "formats": formats, "offsets": offsets, "itemsize": step})
 
 
 def _float_type(dt):
@@ -170,6 +187,73 @@ def layout(records, min_range=0.0, max_range=math.inf, inclusive=True, drop_nan=
             d.range_mode, d.drop_nan, d.on_device, d.stream or 0)
 
 
+def time_layout(records, field, scale=1.0, t_end=None):
+    """(offset, type, scale, t_end, has_t_end) of the time field of `records` (as describe() reads them): `field` is a
+    field name of a structured array, or a column index of a 2-D array or device array.  uint32, float32 and float64
+    little-endian fields are accepted."""
+    a = records
+    cai = None if isinstance(a, np.ndarray) else getattr(a, "__cuda_array_interface__", None)
+    if isinstance(field, str):
+        if cai is not None or not isinstance(a, np.ndarray) or not a.dtype.names or field not in a.dtype.names:
+            raise ValueError(f"time_field: the records have no field {field!r}")
+        dt, off = a.dtype.fields[field][0], int(a.dtype.fields[field][1])
+    elif isinstance(field, (int, np.integer)) and not isinstance(field, bool):
+        col = int(field)
+        if cai is not None:
+            shape, e = tuple(int(k) for k in cai["shape"]), {"<f4": 4, "<f8": 8}.get(cai["typestr"])
+            strides = cai.get("strides")
+            s1 = e if strides is None else int(strides[1])
+            dt = np.dtype(cai["typestr"])
+        elif isinstance(a, np.ndarray) and a.ndim == 2 and not a.dtype.names:
+            shape, s1, dt = a.shape, int(a.strides[1]), a.dtype
+        else:
+            raise ValueError("time_field: a column index needs a 2-D array")
+        if not 3 <= col < shape[1]:
+            raise ValueError(f"time_field: column {col} is not a column after x, y, z")
+        off = col * s1
+    else:
+        raise TypeError("time_field: a field name or a column index")
+    kind = None if dt.byteorder == ">" else _TIME_TYPES.get(dt)
+    if kind is None:
+        raise ValueError(f"time_field: {dt} is not a little-endian uint32, float32 or float64 field")
+    return off, kind, float(scale), 0.0 if t_end is None else float(t_end), int(t_end is not None)
+
+
+def describe_times(records, field, scale=1.0, t_end=None):
+    """madicp_times_t of the time field of `records` (time_layout), or None when `field` is None."""
+    if field is None:
+        return None
+    t = Times()
+    t.offset, t.type, t.scale, t.t_end, t.has_t_end = time_layout(records, field, scale, t_end)
+    return t
+
+
+def time_chunks(records, field, scale, sensor_hz, t_end=None, apply_correction=False,
+                vertical_angle_offset=VERTICAL_ANGLE_OFFSET, **gate):
+    """The chunk of every kept record of `records` under the time-stamp deskew, on the host (madicp_debug_time_chunks):
+    a uint16 array in record order."""
+    from . import _capi
+    d = _host(describe(records, **gate))
+    v = vcorr(apply_correction, vertical_angle_offset)
+    t = describe_times(records, field, scale, t_end)
+    out = np.empty(max(int(d.n), 1), np.uint16)
+    kept = C.c_int64(0)
+    _capi.check(_capi.lib().madicp_debug_time_chunks(C.byref(d), C.byref(v) if v else None, C.byref(t), float(sensor_hz),
+                                                     out.ctypes.data_as(C.POINTER(C.c_uint16)), C.byref(kept)),
+                "madicp_debug_time_chunks")
+    return out[:kept.value].copy()
+
+
+def chunk_poses(T_prev, T_now, sensor_hz, n_chunks=1024):
+    """The deskew's chunk poses (madicp_debug_chunk_poses): n_chunks x 3 x 4 float64."""
+    from . import _capi
+    out = np.empty((n_chunks, 12))
+    _capi.check(_capi.lib().madicp_debug_chunk_poses(_capi.as_d(_capi.pose12(T_prev)), _capi.as_d(_capi.pose12(T_now)),
+                                                     float(sensor_hz), int(n_chunks), _capi.as_d(out)),
+                "madicp_debug_chunk_poses")
+    return out.reshape(n_chunks, 3, 4)
+
+
 def to_host(records):
     """A device array copied to the host once, as a numpy array (for host-built trees, MADICP_GPU_BUILD=0)."""
     if hasattr(records, "cpu"):  # torch
@@ -251,5 +335,5 @@ def correct_vertical_angle(records, vertical_angle_offset=VERTICAL_ANGLE_OFFSET,
     return out[:kept]
 
 
-__all__ = ["pointcloud2_dtype", "describe", "layout", "to_host", "search_cloud_arrays_dev", "leaves_array_dev", "range_mask", "vcorr", "correct_vertical_angle",
+__all__ = ["pointcloud2_dtype", "describe", "describe_times", "time_layout", "time_chunks", "chunk_poses", "layout", "to_host", "search_cloud_arrays_dev", "leaves_array_dev", "range_mask", "vcorr", "correct_vertical_angle",
            "VERTICAL_ANGLE_OFFSET", "RANGE_NONE", "RANGE_INCLUSIVE", "RANGE_STRICT"]

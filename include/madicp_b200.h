@@ -176,6 +176,24 @@ int madtree_gpu_leaf_means(const madtree_gpu_t* const* trees, const double* cons
  * the result is ready on consumer_stream through an event wait, with no host sync. */
 int madtree_gpu_leaf_means_dev(const madtree_gpu_t* const* trees, const double* const* X, int count, double* means_out,
                                void* consumer_stream);
+/* Kept clouds.  keep != 0: device trees built on the context from now on (every ingest and batch path) keep the cloud
+ * they were built from -- the scan's points after the gate, the correction and the deskew, in the order the build got
+ * them (odometry/pipeline.cpp:140, before MADtree reorders them) -- and, for every point, the index of the record it came
+ * from in the array the scan was handed over as (relative to that scan in a batch).  keep == 0 stops it; trees keep
+ * what they already hold.  Off by default: no extra memory, copy or launch. */
+int madicp_set_keep_cloud(madicp_ctx_t* ctx, int keep);
+/* Points of a tree's kept cloud, or MADICP_ERR_STATE when the tree kept none. */
+int64_t madtree_gpu_num_cloud_points(const madtree_gpu_t* t);
+/* The kept cloud as N x 3 doubles, posed by X (NULL: copied untouched, -0.0 stays -0.0; else 12 doubles row-major [R|t],
+ * applied with the node transform's operand order, no FMA), and the record indices as N int64.  Either output may be
+ * NULL, not both.  Host output; synchronises.  Returns N. */
+int64_t madtree_gpu_cloud(const madtree_gpu_t* t, const double X[12], double* xyz_out, int64_t* idx_out);
+/* The same into device memory of the tree's device (8-byte aligned), ordered like madtree_gpu_leaf_means_dev: the
+ * context's stream waits for consumer_stream, the result is ready on consumer_stream with no host sync. */
+int64_t madtree_gpu_cloud_dev(const madtree_gpu_t* t, const double X[12], double* xyz_out, int64_t* idx_out,
+                              void* consumer_stream);
+/* Gives the tree's kept cloud back to the context's cache (no-op without one).  Freeing the tree does too. */
+int madtree_gpu_release_cloud(madtree_gpu_t* t);
 /* Audit dump of a DEVICE-BUILT tree in breadth-first order: mean n x 3, eigenvectors n x 9 (column-major), bbox
  * n x 3, num_points n (any may be NULL).  Valid for the most recently built tree of the context.  Synchronises. */
 int madtree_gpu_export(const madtree_gpu_t* t, double* mean, double* eigenvectors, double* bbox, int32_t* num_points);

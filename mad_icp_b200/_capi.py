@@ -112,6 +112,11 @@ SYMBOLS = {
     "madicp_debug_time_chunks": (C.c_int, [pts_p, vc_p, tm_p, C.c_double, C.POINTER(C.c_uint16), C.POINTER(C.c_int64)]),
     "madicp_debug_chunk_poses": (C.c_int, [dp, dp, C.c_double, C.c_int, dp]),
     "madicp_search_cloud_dev": (C.c_int, [vp, C.c_int, vp, C.c_int64, C.c_int64, C.c_int, vp, vp, vp, vp, vp]),
+    "madicp_set_keep_cloud": (C.c_int, [vp, C.c_int]),
+    "madtree_gpu_num_cloud_points": (C.c_int64, [vp]),
+    "madtree_gpu_cloud": (C.c_int64, [vp, dp, dp, C.POINTER(C.c_int64)]),
+    "madtree_gpu_cloud_dev": (C.c_int64, [vp, dp, vp, vp, vp]),
+    "madtree_gpu_release_cloud": (C.c_int, [vp]),
     "madicp_debug_deskew_plan": (C.c_int, [pts_p, vc_p, dp, dp, C.c_double, C.c_int, C.c_int, ip,
                                            C.POINTER(C.c_uint16), dp, C.POINTER(C.c_int), C.POINTER(C.c_int64)]),
     "madicp_register_fetch_weight": (C.c_int, [vp, dp, dp, dp, bp, C.POINTER(C.c_int), dp]),

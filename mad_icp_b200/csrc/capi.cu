@@ -321,6 +321,13 @@ void madicp_destroy(madicp_ctx_t* c) {
     if (c->world > 1 && r != c->rank && c->peer_comm[r]) cudaIpcCloseMemHandle(c->peer_comm[r]);
   madicp_gpu_build_release(c);
   for (madtree_gpu* t : c->tree_cache) delete t;  // (trees still held by the caller are the caller's to free first)
+  for (CloudBuf* b : c->cloud_cache) {
+    cudaFree(b->xyz);
+    cudaFree(b->idx);
+    delete b;
+  }
+  cudaFreeHost(c->h_cloud_xyz);
+  cudaFreeHost(c->h_cloud_idx);
   for (void* slab : c->tree_slabs) cudaFree(slab);
   cudaFree(c->d_pool_recs);
   cudaFree(c->d_pool_child0);
@@ -621,6 +628,41 @@ int madicp_tree_alloc(madicp_ctx* c, size_t cap_nodes, madtree_gpu** out) {
   return MADICP_OK;
 }
 
+// Kept clouds are cached like trees: a released buffer waits for the next build that fits it (the smallest that does).
+// Every reader and writer of a kept cloud runs on the context's stream, so stream order alone keeps a reuse after them.
+int madicp_cloud_alloc(madicp_ctx* c, size_t n, std::shared_ptr<CloudBuf>* out) {
+  CloudBuf* b = nullptr;
+  {
+    std::lock_guard<std::mutex> lk(c->cloud_mu);
+    size_t best = c->cloud_cache.size();
+    for (size_t i = 0; i < c->cloud_cache.size(); ++i)
+      if (c->cloud_cache[i]->cap >= n && (best == c->cloud_cache.size() || c->cloud_cache[i]->cap < c->cloud_cache[best]->cap))
+        best = i;
+    if (best < c->cloud_cache.size()) {
+      b = c->cloud_cache[best];
+      c->cloud_cache.erase(c->cloud_cache.begin() + long(best));
+    }
+  }
+  if (!b) {
+    b = new CloudBuf;
+    b->cap = size_t(1) << 17;
+    while (b->cap < n) b->cap <<= 1;
+    cudaError_t e = cudaMalloc(&b->xyz, b->cap * 3 * sizeof(double));
+    if (e == cudaSuccess) e = cudaMalloc(&b->idx, b->cap * sizeof(int32_t));
+    if (e != cudaSuccess) {
+      cudaFree(b->xyz);
+      delete b;
+      set_error(std::string("kept cloud allocation: ") + cudaGetErrorString(e));
+      return MADICP_ERR_NOMEM;
+    }
+  }
+  *out = std::shared_ptr<CloudBuf>(b, [c](CloudBuf* p) {
+    std::lock_guard<std::mutex> lk(c->cloud_mu);
+    c->cloud_cache.push_back(p);
+  });
+  return MADICP_OK;
+}
+
 int madicp_check_device_ptr(madicp_ctx* c, const void* p, int align, const char* fn) {
   cudaPointerAttributes a{};
   const cudaError_t e = cudaPointerGetAttributes(&a, p);
@@ -764,6 +806,7 @@ void madtree_gpu_free(madtree_gpu_t* t) {
   // free; a builder that picks the memory up writes it from ANOTHER stream, so it first waits for that work)
   cudaSetDevice(c->device);
   cudaEventRecord(c->tree_free_ev, c->stream);
+  t->cloud.reset();  // (its kept cloud, if the last slice, goes back to the context's cache)
   std::lock_guard<std::mutex> lk(c->tree_mu);
   c->tree_cache.push_back(t);  // (its memory belongs to a slab: released with the context)
 }
@@ -821,6 +864,121 @@ int madtree_gpu_leaf_means_dev(const madtree_gpu_t* const* trees, const double* 
   if (int rc = leaf_gather_launch(c, trees, X, count, total, means_out)) return rc;
   if (int rc = madicp_stream_wait(c, consumer_stream, c->stream)) return rc;
   return total;
+}
+
+int madicp_set_keep_cloud(madicp_ctx_t* c, int keep) {
+  if (!c) {
+    set_error("madicp_set_keep_cloud: null context");
+    return MADICP_ERR_INVALID;
+  }
+  c->keep_cloud = keep != 0;
+  return MADICP_OK;
+}
+
+}  // extern "C"
+
+// A kept-cloud output: a tree that kept its cloud, and at least one output
+static int cloud_check(const madtree_gpu_t* t, const void* xyz_out, const void* idx_out, const char* fn) {
+  if (!t) {
+    set_error(std::string(fn) + ": null tree");
+    return MADICP_ERR_INVALID;
+  }
+  if (!t->cloud) {
+    set_error(std::string(fn) + ": the tree kept no cloud (madicp_set_keep_cloud was off when it was built, or the cloud "
+              "was released)");
+    return MADICP_ERR_STATE;
+  }
+  if (!xyz_out && !idx_out) {
+    set_error(std::string(fn) + ": no output");
+    return MADICP_ERR_INVALID;
+  }
+  return MADICP_OK;
+}
+// k_cloud_out of tree t's kept cloud into xyz / idx (device pointers; either may be null), posed by X (nullable)
+static int cloud_launch(const madtree_gpu_t* t, const double* X, double* xyz, int64_t* idx) {
+  madicp_ctx* c = t->ctx;
+  CloudOut a{};
+  a.xyz = t->cloud->xyz + 3 * size_t(t->cloud_off);
+  a.idx = t->cloud->idx + size_t(t->cloud_off);
+  a.n = t->n_points;
+  a.has_pose = X ? 1 : 0;
+  if (X) memcpy(a.X, X, 12 * sizeof(double));
+  k_cloud_out<<<blocks_for(t->n_points), kStepBlock, 0, c->stream>>>(a, xyz, reinterpret_cast<long long*>(idx));
+  c->launches++;
+  CK(cudaGetLastError());
+  return MADICP_OK;
+}
+
+extern "C" {
+
+int64_t madtree_gpu_num_cloud_points(const madtree_gpu_t* t) {
+  if (!t) {
+    set_error("madtree_gpu_num_cloud_points: null tree");
+    return MADICP_ERR_INVALID;
+  }
+  if (!t->cloud) {
+    set_error("madtree_gpu_num_cloud_points: the tree kept no cloud");
+    return MADICP_ERR_STATE;
+  }
+  return t->n_points;
+}
+
+int64_t madtree_gpu_cloud(const madtree_gpu_t* t, const double X[12], double* xyz_out, int64_t* idx_out) {
+  const char* fn = "madtree_gpu_cloud";
+  if (int rc = cloud_check(t, xyz_out, idx_out, fn)) return rc;
+  const int64_t n = t->n_points;
+  if (n == 0) return 0;
+  madicp_ctx* c = t->ctx;
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  if (size_t(n) > c->cap_cloud_out) {  // (only this call uses the staging, and it returns with the stream idle)
+    cudaFreeHost(c->h_cloud_xyz);
+    cudaFreeHost(c->h_cloud_idx);
+    c->h_cloud_xyz = nullptr;
+    c->h_cloud_idx = nullptr;
+    c->cap_cloud_out = 0;
+    const size_t cap = size_t(n) + size_t(n) / 4 + 1024;
+    CK(cudaHostAlloc(&c->h_cloud_xyz, cap * 3 * sizeof(double), cudaHostAllocMapped));
+    CK(cudaHostAlloc(&c->h_cloud_idx, cap * sizeof(int64_t), cudaHostAllocMapped));
+    c->cap_cloud_out = cap;
+  }
+  double* dx = nullptr;
+  int64_t* di = nullptr;
+  CK(cudaHostGetDevicePointer(reinterpret_cast<void**>(&dx), c->h_cloud_xyz, 0));
+  CK(cudaHostGetDevicePointer(reinterpret_cast<void**>(&di), c->h_cloud_idx, 0));
+  if (int rc = cloud_launch(t, X, xyz_out ? dx : nullptr, idx_out ? di : nullptr)) return rc;
+  CK(cudaStreamSynchronize(c->stream));
+  if (xyz_out) memcpy(xyz_out, c->h_cloud_xyz, size_t(n) * 3 * sizeof(double));
+  if (idx_out) memcpy(idx_out, c->h_cloud_idx, size_t(n) * sizeof(int64_t));
+  return n;
+  MADICP_CATCH(fn)
+}
+
+int64_t madtree_gpu_cloud_dev(const madtree_gpu_t* t, const double X[12], double* xyz_out, int64_t* idx_out,
+                              void* consumer_stream) {
+  const char* fn = "madtree_gpu_cloud_dev";
+  if (int rc = cloud_check(t, xyz_out, idx_out, fn)) return rc;
+  madicp_ctx* c = t->ctx;
+  CK(cudaSetDevice(c->device));
+  if (xyz_out)
+    if (int rc = madicp_check_device_ptr(c, xyz_out, 8, "madtree_gpu_cloud_dev (points)")) return rc;
+  if (idx_out)
+    if (int rc = madicp_check_device_ptr(c, idx_out, 8, "madtree_gpu_cloud_dev (indices)")) return rc;
+  const int64_t n = t->n_points;
+  if (n == 0) return 0;
+  if (int rc = madicp_stream_wait(c, c->stream, consumer_stream)) return rc;  // the outputs are allocated there
+  if (int rc = cloud_launch(t, X, xyz_out, idx_out)) return rc;
+  if (int rc = madicp_stream_wait(c, consumer_stream, c->stream)) return rc;
+  return n;
+}
+
+int madtree_gpu_release_cloud(madtree_gpu_t* t) {
+  if (!t) {
+    set_error("madtree_gpu_release_cloud: null tree");
+    return MADICP_ERR_INVALID;
+  }
+  t->cloud.reset();
+  return MADICP_OK;
 }
 
 int madicp_put_keyframe_tree(madicp_ctx_t* c, int slot, const madtree_gpu_t* t, const double X[12]) {

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 
 #include <atomic>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <stdexcept>
@@ -29,6 +30,15 @@ struct CommBlock {
   Mailbox box;
   unsigned char matched[2][kMatchedCap];
 };
+
+// A kept scan cloud (madicp_set_keep_cloud): the points a build got, before it reordered them, and the record index of
+// every point.  One buffer per build (a forest's trees share it, each its own slice); back to the context's cache once
+// the last tree holding a slice lets it go.
+struct CloudBuf {
+  size_t cap = 0;           // points
+  double* xyz = nullptr;    // cap x 3
+  int32_t* idx = nullptr;   // cap
+};
 }  // namespace madicp
 
 struct madicp_ctx;
@@ -48,6 +58,10 @@ struct madtree_gpu {
   double* full = nullptr;         // n_nodes x 16: mean 3, eigenvectors 9 (column-major), bbox 3, num_points
   int64_t n_points = 0;
   uint64_t build_seq = 0;
+  // the cloud the tree was built from and its record indices (madicp_set_keep_cloud): points [cloud_off, cloud_off +
+  // n_points) of `cloud`, or none
+  std::shared_ptr<madicp::CloudBuf> cloud;
+  int64_t cloud_off = 0;
 };
 
 struct madicp_ctx {
@@ -88,6 +102,13 @@ struct madicp_ctx {
   cudaEvent_t tree_free_ev = nullptr;    // recorded on the context's stream at every madtree_gpu_free
   cudaEvent_t xstream_ev = nullptr;      // hand-overs with a caller's stream (madicp_stream_wait)
   std::mutex tree_mu;                    // ... builders on other host threads allocate from it too
+  // kept clouds (madicp_set_keep_cloud): trees built from now on keep their input cloud; released buffers are cached
+  bool keep_cloud = false;
+  std::vector<madicp::CloudBuf*> cloud_cache;
+  std::mutex cloud_mu;
+  int64_t* h_cloud_idx = nullptr;  // mapped staging of madtree_gpu_cloud (host form)
+  double* h_cloud_xyz = nullptr;
+  size_t cap_cloud_out = 0;
   void* build_state = nullptr;           // gpu_tree.cu: working memory of the device build (lazily created)
   void* plan_state = nullptr;            // gpu_tree.cu: buffers and threads of look-ahead plans (lazily created)
   long long* d_dbg_cta = nullptr;  // MADICP_MAX_ITERS x grid item-phase cycles when debug timing is on
@@ -166,6 +187,8 @@ struct madicp_ctx {
 
 // capi.cu
 int madicp_tree_alloc(madicp_ctx* c, size_t cap_nodes, madtree_gpu** out);
+// a kept-cloud buffer of at least n points, from the context's cache or new; it returns to the cache when released
+int madicp_cloud_alloc(madicp_ctx* c, size_t n, std::shared_ptr<madicp::CloudBuf>* out);
 // MADICP_OK, or MADICP_ERR_INVALID with a message naming `fn`: p must be device memory (not host, managed or another
 // device's) of the context's device, aligned to `align` bytes
 int madicp_check_device_ptr(madicp_ctx* c, const void* p, int align, const char* fn);

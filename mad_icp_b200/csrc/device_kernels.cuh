@@ -236,6 +236,26 @@ k_leaf_means(const LeafGather* __restrict__ table, int count, int total, double*
   out[3 * size_t(i) + 2] = z;
 }
 
+// A tree's kept cloud out (madtree_gpu_cloud*): point i posed by the pose (iso_apply, as k_leaf_means) or copied
+// untouched without one, and its record index widened to int64 (either output nullable).  The outputs are the caller's
+// device memory or the context's mapped staging.
+__global__ void __launch_bounds__(kStepBlock)
+k_cloud_out(const __grid_constant__ CloudOut a, double* __restrict__ xyz_out, long long* __restrict__ idx_out) {
+  const long long i = (long long) blockIdx.x * kStepBlock + threadIdx.x;
+  if (i >= a.n) return;
+  if (idx_out) idx_out[i] = a.idx[i];
+  if (!xyz_out) return;
+  double x = a.xyz[3 * i], y = a.xyz[3 * i + 1], z = a.xyz[3 * i + 2];
+  if (a.has_pose) {
+    double px, py, pz;
+    iso_apply(a.X, x, y, z, px, py, pz);
+    x = px; y = py; z = pz;
+  }
+  xyz_out[3 * i] = x;
+  xyz_out[3 * i + 1] = y;
+  xyz_out[3 * i + 2] = z;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Step API: K1 / K2 / K3
 // ---------------------------------------------------------------------------------------------

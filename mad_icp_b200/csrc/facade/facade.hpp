@@ -142,6 +142,58 @@ class MADtree {
     deviceTable(trees, g, X);
     check(madtree_gpu_leaf_means_dev(g.data(), X.data(), int(g.size()), out, consumer_stream), "madtree_gpu_leaf_means_dev");
   }
+  // The cloud the tree was built from, in the order the build got it, and the record index of every point
+  // (madicp_set_keep_cloud for device trees; keepHostCloud for host-built ones).  posed: by the tree's pose, if any,
+  // with the node transform's arithmetic; without a pose the points are copied untouched.
+  size_t numCloudPoints() const {
+    if (t_) {
+      if (!host_cloud_) throw Error("MADtree.cloud: the tree kept no cloud");
+      return host_idx_.size();
+    }
+    const int64_t n = madtree_gpu_num_cloud_points(g_);
+    check(int(n < 0 ? n : 0), "madtree_gpu_num_cloud_points");
+    return size_t(n);
+  }
+  // host output (xyz_out / idx_out nullable)
+  void cloud(bool posed, double* xyz_out, int64_t* idx_out) const {
+    const double* X = posed ? pose() : nullptr;
+    if (g_) {
+      check(int(std::min<int64_t>(0, madtree_gpu_cloud(g_, X, xyz_out, idx_out))), "madtree_gpu_cloud");
+      return;
+    }
+    if (!host_cloud_) throw Error("MADtree.cloud: the tree kept no cloud");
+    const size_t n = host_idx_.size();
+    if (idx_out)
+      for (size_t i = 0; i < n; ++i) idx_out[i] = host_idx_[i];
+    if (!xyz_out) return;
+    if (!X) {
+      std::memcpy(xyz_out, host_xyz_.data(), n * 3 * sizeof(double));
+      return;
+    }
+    for (size_t i = 0; i < n; ++i) {  // the node transform's arithmetic, as leafMeans
+      const double* p = host_xyz_.data() + 3 * i;
+      const double x = p[0], y = p[1], z = p[2];
+      for (int r = 0; r < 3; ++r) xyz_out[3 * i + r] = ((X[r * 4] * x + X[r * 4 + 1] * y) + X[r * 4 + 2] * z) + X[r * 4 + 3];
+    }
+  }
+  // device output (device memory of the tree's device), ready on consumer_stream with no host sync; device trees only
+  void cloudDev(bool posed, double* xyz_out, int64_t* idx_out, void* consumer_stream) const {
+    if (!g_) throw Error("MADtree.cloudDev: a device output needs a device tree");
+    check(int(std::min<int64_t>(0, madtree_gpu_cloud_dev(g_, posed ? pose() : nullptr, xyz_out, idx_out, consumer_stream))),
+          "madtree_gpu_cloud_dev");
+  }
+  // a host-built tree keeps `xyz` (n x 3) and its record indices
+  void keepHostCloud(const double* xyz, size_t n, std::vector<int32_t> idx) {
+    host_xyz_.assign(xyz, xyz + 3 * n);
+    host_idx_ = std::move(idx);
+    host_cloud_ = true;
+  }
+  void releaseCloud() {
+    if (g_) madtree_gpu_release_cloud(g_);
+    host_xyz_ = std::vector<double>();
+    host_idx_ = std::vector<int32_t>();
+    host_cloud_ = false;
+  }
   const madtree_t* hostHandle() const { return t_; }
   const madtree_gpu_t* deviceHandle() const { return g_; }
   madicp_ctx_t* deviceContext() const { return ctx_; }
@@ -172,6 +224,9 @@ class MADtree {
   madicp_ctx_t* ctx_ = nullptr;
   bool has_pose_ = false;
   double pose_[12];
+  bool host_cloud_ = false;  // keepHostCloud
+  std::vector<double> host_xyz_;
+  std::vector<int32_t> host_idx_;
 };
 
 // reference: class MADicp (odometry/mad_icp.h:41-79).  `update(tree)` under the reference's OpenMP loop

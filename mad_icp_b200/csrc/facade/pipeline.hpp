@@ -253,12 +253,13 @@ class Pipeline {
   static constexpr int kMaxIcpIts = 15, kSmoothingT = 10, kFrameWindow = 10, kChunks = 1024;  // tools/constants.h
 
   Pipeline(double sensor_hz, bool deskew, double b_max, double rho_ker, double p_th, double b_min, double b_ratio,
-           int num_keyframes, int num_threads, bool realtime, int device = -1)
+           int num_keyframes, int num_threads, bool realtime, int device = -1, bool keep_cloud = false)
       : sensor_hz_(sensor_hz), deskew_(deskew), b_max_(b_max), p_th_(p_th), b_min_(b_min), num_keyframes_(num_keyframes),
-        realtime_(realtime), icp_(b_max, rho_ker, b_ratio, num_threads, resolveDevice(device), std::max(num_keyframes, 1)),
-        vel_(sensor_hz) {
+        realtime_(realtime), keep_cloud_(keep_cloud),
+        icp_(b_max, rho_ker, b_ratio, num_threads, resolveDevice(device), std::max(num_keyframes, 1)), vel_(sensor_hz) {
     frame_to_map_ = keyframe_to_map_ = detail::poseIdentity();
     device_ = resolveDevice(device);
+    if (keep_cloud_) check(madicp_set_keep_cloud(icp_.context(), 1), "madicp_set_keep_cloud");
     if (const char* e = std::getenv("MADICP_GPU_BUILD")) gpu_build_ = std::atoi(e) != 0;
     num_threads_ = std::max(num_threads, 1);
     int lvl = 0;
@@ -304,6 +305,19 @@ class Pipeline {
     MADtree::leafMeansDev(leafTrees(model), out, consumer_stream);
   }
   int device() const { return device_; }
+  // The current scan's deskewed cloud, as its MAD-tree was built from it (odometry/pipeline.cpp:140: curr_cloud after the
+  // deskew, before MADtree reorders it), and the index of the record behind every point in the array the scan was handed
+  // over as.  keep_cloud pipelines only; empty before the first scan.  map: posed by currentPose() (a scan without a pose,
+  // the first, is copied untouched).  The previous scan's cloud is released when a scan becomes current.
+  bool keepCloud() const { return keep_cloud_; }
+  int64_t kernelLaunches() { return madicp_kernel_launches(icp_.context()); }  // (diagnostics: launches so far)
+  size_t numCloudPoints() const { return requireCloud() ? current_->tree->numCloudPoints() : 0; }
+  void cloud(bool map, double* xyz_out, int64_t* idx_out) const {
+    if (requireCloud()) current_->tree->cloud(map, xyz_out, idx_out);
+  }
+  void cloudDev(bool map, double* xyz_out, int64_t* idx_out, void* consumer_stream) const {
+    if (requireCloud()) current_->tree->cloudDev(map, xyz_out, idx_out, consumer_stream);
+  }
 
   // test hook: the deskew step alone (poses 4x4 row-major)
   static ContainerType deskewOnly(ContainerType cloud, const Matrix4d& T_prev, const Matrix4d& T_now, double sensor_hz,
@@ -351,9 +365,11 @@ class Pipeline {
     }
     const madicp_times_t t = madicp::times_of(tm);
     if (!gpu_build_) {
-      const ContainerType cloud = packRecords(pts, vc);
+      std::vector<int32_t> idx;
+      const ContainerType cloud = packRecords(pts, vc, keep_cloud_ ? &idx : nullptr);
       const madicp_vcorr_t v = madicp::vcorr_of(vc);
-      computeRaw(stamp, cloud[0].data(), cloud.size(), false, t.type ? &pts : nullptr, &v, nullptr, t.type ? &t : nullptr);
+      computeRaw(stamp, cloud[0].data(), cloud.size(), false, t.type ? &pts : nullptr, &v, nullptr, t.type ? &t : nullptr,
+                 keep_cloud_ ? idx.data() : nullptr);
       return;
     }
     if (!pts.data || pts.n <= 0) throw Error("Pipeline.computeRecords: empty scan");
@@ -422,6 +438,11 @@ class Pipeline {
   size_t prefetched() { return lookahead_ ? lookahead_->size() : 0; }
 
  private:
+  // whether there is a current scan whose cloud can be read (throws without keep_cloud)
+  bool requireCloud() const {
+    if (!keep_cloud_) throw Error("Pipeline.currentCloud: the pipeline keeps no cloud (construct it with keep_cloud=True)");
+    return current_ != nullptr;
+  }
   // the trees of currentLeaves (model == false) or modelLeaves
   std::vector<const MADtree*> leafTrees(bool model) const {
     std::vector<const MADtree*> trees;
@@ -435,7 +456,8 @@ class Pipeline {
   // tm (nullable): the records' time field.  Host-built trees (MADICP_GPU_BUILD=0): xyz is the packed kept cloud and
   // `records` the scan it came from, for the stamps.
   std::unique_ptr<MADtree> makeTree(const void* xyz, size_t n, bool is_f32, const madicp_points_t* records,
-                                    const madicp_vcorr_t* vc, const DevScan* dev, const madicp_times_t* tm) {
+                                    const madicp_vcorr_t* vc, const DevScan* dev, const madicp_times_t* tm,
+                                    const int32_t* rec_idx) {
     const bool dsk = deskew_ && is_initialized_ && trajectory_.size() > 1;
     const double* Ta = dsk ? trajectory_[trajectory_.size() - 2].m : nullptr;
     const double* Tb = dsk ? trajectory_[trajectory_.size() - 1].m : nullptr;
@@ -463,6 +485,18 @@ class Pipeline {
       return std::unique_ptr<MADtree>(new MADtree(icp_.context(), b_max_, b_min_));
     }
     const double* pts = static_cast<const double*>(xyz);
+    // keep_cloud: the record of every point of the tree's cloud (rec_idx: of every point of xyz; nullptr: xyz is the
+    // array the caller handed over)
+    std::vector<int32_t> idx;
+    auto tree = [&](const double* cloud) {
+      std::unique_ptr<MADtree> t(new MADtree(cloud, n, b_max_, b_min_, max_parallel_levels_));
+      if (keep_cloud_) t->keepHostCloud(cloud, n, std::move(idx));
+      return t;
+    };
+    if (keep_cloud_ && !(dsk && !(tm && records))) {  // (the azimuth deskew reorders: its indices come with its order)
+      idx.resize(n);
+      for (size_t i = 0; i < n; ++i) idx[i] = rec_idx ? rec_idx[i] : int32_t(i);
+    }
     if (dsk && tm && records) {  // the host restatement of the time-stamp deskew (madicp_debug_time_chunks)
       std::vector<uint16_t> chunk(size_t(records->n));
       int64_t kept = 0;
@@ -472,19 +506,39 @@ class Pipeline {
       check(madicp_debug_chunk_poses(Ta, Tb, sensor_hz_, kChunks, poses[0].m), "madicp_debug_chunk_poses");
       ContainerType cloud(n);
       for (size_t i = 0; i < n; ++i) madicp_pose::poseApply(poses[chunk[i]], pts + 3 * i, cloud[i].data());
-      return std::unique_ptr<MADtree>(new MADtree(cloud[0].data(), n, b_max_, b_min_, max_parallel_levels_));
+      return tree(cloud[0].data());
+    }
+    if (dsk && keep_cloud_) {  // the deskew's plan (its order and chunk poses), applied here: madicp_deskew's cloud, with
+                               // the kept point behind every sorted position
+      const madicp_points_t d = madicp::packed_points(pts, int64_t(n), 0);
+      std::vector<int32_t> perm(n);
+      std::vector<uint16_t> chunk(n);
+      std::vector<detail::Pose> poses(2 * kChunks);  // (the sweep may make one chunk more than kChunks)
+      int n_poses = 0;
+      int64_t kept = 0;
+      check(madicp_debug_deskew_plan(&d, nullptr, Ta, Tb, sensor_hz_, 0, 1 << max_parallel_levels_, perm.data(), chunk.data(),
+                                     poses[0].m, &n_poses, &kept), "madicp_debug_deskew_plan");
+      ContainerType cloud(n);
+      idx.resize(n);
+      for (size_t i = 0; i < n; ++i) {
+        madicp_pose::poseApply(poses[chunk[i]], pts + 3 * size_t(perm[i]), cloud[i].data());
+        idx[i] = rec_idx ? rec_idx[perm[i]] : perm[i];
+      }
+      return tree(cloud[0].data());
     }
     if (dsk) {
       ContainerType cloud(n);
       std::memcpy(cloud[0].data(), pts, sizeof(double) * 3 * n);
       check(madicp_deskew(cloud[0].data(), int64_t(n), Ta, Tb, sensor_hz_, 1 << max_parallel_levels_), "madicp_deskew");
-      return std::unique_ptr<MADtree>(new MADtree(cloud[0].data(), n, b_max_, b_min_, max_parallel_levels_));
+      return tree(cloud[0].data());
     }
-    return std::unique_ptr<MADtree>(new MADtree(pts, n, b_max_, b_min_, max_parallel_levels_));
+    return tree(pts);
   }
 
+  // rec_idx (host-built trees, nullable): the record index of every point of xyz
   void computeRaw(double stamp, const void* xyz, size_t n, bool is_f32, const madicp_points_t* records = nullptr,
-                  const madicp_vcorr_t* vc = nullptr, const DevScan* dev = nullptr, const madicp_times_t* tm = nullptr) {
+                  const madicp_vcorr_t* vc = nullptr, const DevScan* dev = nullptr, const madicp_times_t* tm = nullptr,
+                  const int32_t* rec_idx = nullptr) {
     if (!xyz || n == 0) throw Error("Pipeline.compute: empty cloud");
     is_map_updated_ = false;
     if (!is_initialized_) {  // pipeline.cpp:267-284
@@ -492,7 +546,7 @@ class Pipeline {
       f->frame = int(seq_);
       f->to_map = frame_to_map_;
       f->stamp = stamp;
-      f->tree = makeTree(xyz, n, is_f32, records, vc, dev, tm);
+      f->tree = makeTree(xyz, n, is_f32, records, vc, dev, tm, rec_idx);
       keyframes_.push_back(f);
       current_ = f;
       trajectory_.push_back(detail::poseIdentity());
@@ -503,7 +557,7 @@ class Pipeline {
     const auto c0 = clk();
     const auto c1 = c0;
     auto cur = std::make_shared<FrameB>();
-    cur->tree = makeTree(xyz, n, is_f32, records, vc, dev, tm);
+    cur->tree = makeTree(xyz, n, is_f32, records, vc, dev, tm, rec_idx);
     const auto c2 = clk();
     double t[3], w[3];
     for (int a = 0; a < 3; ++a) {
@@ -543,6 +597,7 @@ class Pipeline {
     cur->weight = (iters > 0 && iters <= MADICP_MAX_ITERS) ? icp_.weight()                        // :223, from the device
                                                            : detail::inverseDeterminant(icp_.H_adder_);
     cur->tree->applyTransform(toM(frame_to_map_));             // :224
+    if (current_ && keep_cloud_) current_->tree->releaseCloud();  // (only the current scan's cloud is kept)
     current_ = cur;
     frames_.push_back(cur);
     if (frames_.size() > size_t(kFrameWindow)) frames_.pop_front();
@@ -590,8 +645,8 @@ class Pipeline {
   }
 
   // the kept points of `pts` as a packed float64 cloud, corrected by `vc` (nullable), with the predicate and the
-  // restatement the device applies (records.hpp)
-  static ContainerType packRecords(const madicp_points_t& pts, const madicp_vcorr_t* vc) {
+  // restatement the device applies (records.hpp); idx (nullable) receives the record index of every kept point
+  static ContainerType packRecords(const madicp_points_t& pts, const madicp_vcorr_t* vc, std::vector<int32_t>* idx = nullptr) {
     check(madicp::check_points(&pts, "Pipeline.computeRecords"), "Pipeline.computeRecords");
     madicp::VcorrTable table;
     const bool corrected = madicp::vcorr_of(vc).enabled != 0;
@@ -603,7 +658,9 @@ class Pipeline {
       const madicp::RecReader<decltype(zero)> rd(pts, corrected ? &table : nullptr);
       for (int64_t i = 0; i < pts.n; ++i) {
         Vector3d p;
-        if (rd.kept_point(i, p[0], p[1], p[2], bad)) cloud.push_back(p);
+        if (!rd.kept_point(i, p[0], p[1], p[2], bad)) continue;
+        cloud.push_back(p);
+        if (idx) idx->push_back(int32_t(i));
       }
     };
     if (pts.is_f32) pack(0.0f);
@@ -625,6 +682,7 @@ class Pipeline {
   double b_max_, p_th_, b_min_;
   int num_keyframes_, max_parallel_levels_ = 0;
   bool realtime_;
+  bool keep_cloud_ = false;  // the current scan's tree keeps its cloud and record indices (currentCloud)
   bool gpu_build_ = true;   // MADICP_GPU_BUILD=0: host-built trees
   int device_ = 0;
   int num_threads_ = 1;

@@ -63,14 +63,46 @@ static py::object leaves_array(const py::object& self, bool model, bool device) 
   return std::move(out);
 }
 
+// currentCloudArray's frame: "map" or "sensor"
+static bool map_frame(const std::string& frame) {
+  if (frame != "map" && frame != "sensor") throw py::value_error("currentCloudArray: frame must be \"map\" or \"sensor\"");
+  return frame == "map";
+}
+
+// currentCloudArray / currentCloudIndices as numpy arrays, or with `device` as CUDA tensors on the pipeline's device,
+// ready on torch's current stream (records.cloud_array_dev)
+static py::object cloud_array(const py::object& self, bool device, bool map) {
+  const mb::Pipeline& p = self.cast<const mb::Pipeline&>();
+  const size_t n = p.numCloudPoints();
+  if (device) return py::module_::import("mad_icp_b200.records").attr("cloud_array_dev")(self, false, map);
+  py::array_t<double> out({n, size_t(3)});
+  if (n) p.cloud(map, out.mutable_data(), nullptr);
+  return std::move(out);
+}
+static py::object cloud_indices(const py::object& self, bool device) {
+  const mb::Pipeline& p = self.cast<const mb::Pipeline&>();
+  const size_t n = p.numCloudPoints();
+  if (device) return py::module_::import("mad_icp_b200.records").attr("cloud_array_dev")(self, true, false);
+  py::array_t<int64_t> out(n);
+  if (n) p.cloud(false, nullptr, out.mutable_data());
+  return std::move(out);
+}
+
 PYBIND11_MODULE(pypeline, m) {
   bind_vector_eigen3d(m);
   // KittiReader.vertical_angle_offset, np.radians(0.205), as records.py computes it: the default bit for bit
   const double kVerticalAngle = py::module_::import("mad_icp_b200.records").attr("VERTICAL_ANGLE_OFFSET").cast<double>();
   py::class_<mb::Pipeline>(m, "Pipeline")
-      .def(py::init<double, bool, double, double, double, double, double, int, int, bool>(), py::arg("sensor_hz"),
-           py::arg("deskew"), py::arg("b_max"), py::arg("rho_ker"), py::arg("p_th"), py::arg("b_min"), py::arg("b_ratio"),
-           py::arg("num_keyframes"), py::arg("num_threads"), py::arg("realtime"))
+      // keep_cloud (not in the reference): the current scan's deskewed cloud and its record indices stay available
+      // (currentCloudArray / currentCloudIndices)
+      .def(py::init([](double sensor_hz, bool deskew, double b_max, double rho_ker, double p_th, double b_min, double b_ratio,
+                       int num_keyframes, int num_threads, bool realtime, bool keep_cloud) {
+             return new mb::Pipeline(sensor_hz, deskew, b_max, rho_ker, p_th, b_min, b_ratio, num_keyframes, num_threads,
+                                     realtime, -1, keep_cloud);
+           }),
+           py::arg("sensor_hz"), py::arg("deskew"), py::arg("b_max"), py::arg("rho_ker"), py::arg("p_th"), py::arg("b_min"),
+           py::arg("b_ratio"), py::arg("num_keyframes"), py::arg("num_threads"), py::arg("realtime"),
+           py::arg("keep_cloud") = false)
       .def("currentPose", [](const mb::Pipeline& p) { return pose_to_numpy(p.currentPose()); })
       .def("trajectory",
            [](const mb::Pipeline& p) {
@@ -90,6 +122,18 @@ PYBIND11_MODULE(pypeline, m) {
            py::arg("device") = false)
       .def("modelLeavesArray", [](const py::object& self, bool device) { return leaves_array(self, true, device); },
            py::arg("device") = false)
+      // the current scan's deskewed cloud (keep_cloud): points in the map frame (currentPose) or the sensor frame, and
+      // the index of every point's record in the array the scan was handed over as
+      .def("currentCloudArray", [](const py::object& self, bool device, const std::string& frame) {
+             return cloud_array(self, device, map_frame(frame));
+           }, py::arg("device") = false, py::arg("frame") = "map")
+      .def("currentCloudIndices", [](const py::object& self, bool device) { return cloud_indices(self, device); },
+           py::arg("device") = false)
+      .def("_numCloudPoints", &mb::Pipeline::numCloudPoints)
+      .def("_kernelLaunches", &mb::Pipeline::kernelLaunches)
+      .def("_cloudDev", [](const mb::Pipeline& p, bool map, uintptr_t xyz, uintptr_t idx, uintptr_t stream) {
+        p.cloudDev(map, reinterpret_cast<double*>(xyz), reinterpret_cast<int64_t*>(idx), reinterpret_cast<void*>(stream));
+      })
       .def("_numLeaves", &mb::Pipeline::numLeaves)
       .def("_device", &mb::Pipeline::device)
       .def("_leafMeansDev", [](const mb::Pipeline& p, bool model, uintptr_t out, uintptr_t stream) {

@@ -103,6 +103,11 @@ struct BuildState {
   uint16_t* h_chunk = nullptr;
   double* h_poses = nullptr;
   double* h_packed = nullptr;  // pinned, 3 x cap, at first use: a deskewed device scan's kept points for the host's order
+  // kept clouds (madicp_set_keep_cloud), at first use: the record index of every point of the cloud in P[0] (valid when
+  // idx_ok), and the records of a compaction's kept ranks before a deskew order is composed with them
+  int* d_idx = nullptr;
+  int* d_rec = nullptr;
+  bool idx_ok = false;
   double* h_root = nullptr;  // pinned: the root's sums when the host computes them
   double root_S[9];          // ... of the cloud madicp_ingest left in P[0] (valid when has_root_S)
   bool has_root_S = false;
@@ -418,6 +423,37 @@ Background& background() {
 
 int blocks(int64_t n, int per = kBlock) { return int(std::max<int64_t>(1, (n + per - 1) / per)); }
 
+// ---- record indices of kept clouds (madicp_set_keep_cloud): nothing below runs unless the context keeps clouds
+int ensure_idx(BuildState* bs) {
+  if (!bs->d_idx)
+    if (int e = dev_alloc(bs, &bs->d_idx, bs->cap)) return e;
+  if (!bs->d_rec)
+    if (int e = dev_alloc(bs, &bs->d_rec, bs->cap)) return e;
+  return MADICP_OK;
+}
+// rec_of[rank] for the records of B (k_kept_records): gated, over the flags and scan of the compaction just launched
+int keep_records(madicp_ctx* c, cudaStream_t st, BuildState* bs, const RecBatch& B, bool gated, int* rec_of) {
+  k_kept_records<<<blocks(B.n_rec), kBlock, 0, st>>>(B, gated ? bs->flag : nullptr, bs->G, bs->tile, rec_of);
+  c->launches++;
+  CK(cudaGetLastError());
+  return MADICP_OK;
+}
+// out[j] = rec_of[perm[j]]
+int keep_compose(madicp_ctx* c, cudaStream_t st, const int* perm, const int* rec_of, int64_t n, int* out) {
+  k_compose_records<<<blocks(n), kBlock, 0, st>>>(perm, rec_of, int(n), out);
+  c->launches++;
+  CK(cudaGetLastError());
+  return MADICP_OK;
+}
+// a batch that only says where each scan's records start (count scans, first[count] records in all)
+RecBatch batch_of_firsts(const int* first, int count) {
+  RecBatch B{};
+  B.count = count;
+  B.n_rec = first[count];
+  for (int b = 0; b < count; ++b) B.s[b].first = first[b];
+  return B;
+}
+
 // Builds the trees of the n_trees clouds that lie back to back in bs->P[0] (tree b = points [offs[b], offs[b+1])) on
 // stream `st`, as ONE forest: the level loop is the same for one tree or sixteen, and so is its latency (the in-order
 // sums are dependent-add chains; sixteen roots are sixteen chains side by side).  root_S (nullable):
@@ -436,6 +472,19 @@ int build_forest(madicp_ctx* c, BuildState* bs, cudaStream_t st, int n_trees, co
     return MADICP_ERR_INVALID;
   }
   const int n = offs[n_trees];
+  // the clouds as the ingest left them, before the level loop reorders P[0]: one copy of the whole range, each tree gets
+  // its slice
+  std::shared_ptr<CloudBuf> kept;
+  if (c->keep_cloud) {
+    if (!bs->idx_ok) {
+      set_error("madtree_gpu_build: the cloud was ingested before madicp_set_keep_cloud: its record indices are unknown");
+      return MADICP_ERR_STATE;
+    }
+    if (int e = madicp_cloud_alloc(c, size_t(n), &kept)) return e;
+    if (st != c->stream) CK(cudaStreamWaitEvent(st, c->tree_free_ev, 0));
+    CK(cudaMemcpyAsync(kept->xyz, bs->P[0], size_t(n) * 3 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(kept->idx, bs->d_idx, size_t(n) * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  }
   bs->seq++;
   struct Hot {  // the levels' libm sections follow each other within a few hundred microseconds
     Hot() { madicp_host_hot(1); }
@@ -598,6 +647,8 @@ int build_forest(madicp_ctx* c, BuildState* bs, cudaStream_t st, int n_trees, co
     t->n_points = offs[b + 1] - offs[b];
     t->full = (n_trees == 1) ? bs->N.full : nullptr;  // the audit dump indexes the build's node arrays: single trees only
     t->build_seq = bs->seq;
+    t->cloud = kept;
+    t->cloud_off = offs[b];
     bs->h_out[b] = TreeOut{t->recs, t->leaf_of, offs[b], 0};
   }
   if (rc) return rc;
@@ -824,6 +875,9 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* v
   bs->kept_check = 0;
   bs->vc_check = corrected;
   bs->time_check = false;
+  bs->idx_ok = false;
+  if (c->keep_cloud)
+    if (int e = ensure_idx(bs)) return e;
   if (!direct) {
     RecBatch B;
     B.count = count;
@@ -842,7 +896,12 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* v
       k<<<blocks(n_rec), kBlock, 0, st>>>(B, nullptr, nullptr, bs->d_poses, n_rec, bs->P[0], bs->d_vtab, bs->h_vc_err);
       c->launches++;
     }
+    if (c->keep_cloud)
+      if (int e = keep_records(c, st, bs, B, gated || dev, bs->d_idx)) return e;
+  } else if (c->keep_cloud) {
+    if (int e = keep_records(c, st, bs, batch_of_firsts(first, count), false, bs->d_idx)) return e;
   }
+  bs->idx_ok = c->keep_cloud;
   const auto ta1 = std::chrono::steady_clock::now();
   // the roots' sums and the kept counts on the host, one scan per host thread, while the scans are being copied up; a
   // batch holding a corrected scan has its roots summed on the device (root_host), and so has a batch of device scans,
@@ -953,6 +1012,8 @@ struct PlanBuf {
   double* d_pts = nullptr;
   double* d_tau = nullptr;
   unsigned long long* d_tmax = nullptr;
+  // kept clouds (madicp_set_keep_cloud), at first use: the record of every kept rank of a compaction done at hand-over
+  int* d_rec = nullptr;
 };
 void free_buf(PlanBuf* b) {
   if (b->ready) cudaEventSynchronize(b->ready);
@@ -961,6 +1022,7 @@ void free_buf(PlanBuf* b) {
   cudaFree(b->d_pts);
   cudaFree(b->d_tau);
   cudaFree(b->d_tmax);
+  cudaFree(b->d_rec);
   cudaFree(b->d_raw);
   cudaFree(b->d_perm);
   cudaFree(b->d_chunk);
@@ -1104,6 +1166,7 @@ struct madicp_plan {
   madicp_vcorr_t vc{};
   bool dev = false;  // device records: buf->d_raw holds the kept points (PlanBuf)
   madicp_times_t tm{};  // a time field (tm.type != kTimeNone): no order half, buf->d_pts / d_tau hold the kept points
+  bool keep = false;    // the hand-over's compaction (device records, time field) wrote buf->d_rec
   PlanBuf* buf = nullptr;
   std::promise<void> done_p;
   std::future<void> done;  // the order half has run and its uploads are queued
@@ -1229,9 +1292,16 @@ int ingest_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc
   bs->kept_check = 0;
   bs->vc_check = false;  // (an angle outside the table fails this call)
   bs->time_check = false;
+  bs->idx_ok = false;
+  const bool keep = c->keep_cloud;
+  if (keep)
+    if (int e = ensure_idx(bs)) return e;
   int64_t kept = d.n;
   if (is_direct(d, vc) && !deskew) {
     CK(cudaMemcpyAsync(bs->P[0], d.data, size_t(d.n) * 24, cudaMemcpyDeviceToDevice, st));
+    const int first[2] = {0, int(d.n)};
+    if (keep)
+      if (int e = keep_records(c, st, bs, batch_of_firsts(first, 1), false, bs->d_idx)) return e;
   } else {
     int slot = -1;
     if (vc.enabled) CK(cudaMemsetAsync(bs->h_vc_err, 0, sizeof(int), st));
@@ -1250,6 +1320,9 @@ int ingest_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc
     } else if (int e = launch_compaction(c, bs, st, B, deskew ? bs->P[1] : bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) {
       return e;
     }
+    // (azimuth deskew: the kept ranks' records, composed with the order below)
+    if (keep)
+      if (int e = keep_records(c, st, bs, B, true, (deskew && !timed) ? bs->d_rec : bs->d_idx)) return e;
     CK(cudaStreamSynchronize(st));
     if (vc.enabled && *bs->h_vc_err) {
       set_error(vcorr_out_of_table(fn, vc.angle));
@@ -1281,8 +1354,26 @@ int ingest_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc
     k_ingest<false><<<blocks(kept), kBlock, 0, st>>>(packed_batch(bs->P[1], kept), bs->d_perm, bs->d_chunk, bs->d_poses,
                                                      int(kept), bs->P[0], bs->d_vtab, bs->h_vc_err);
     c->launches++;
+    if (keep)
+      if (int e = keep_compose(c, st, bs->d_perm, bs->d_rec, kept, bs->d_idx)) return e;
   }
+  bs->idx_ok = keep;
   return ingest_done(bs, st, kept, n_kept, points_out);
+}
+
+// The record indices of a consumed plan's cloud (madicp_set_keep_cloud) into bs->d_idx, from the records of its kept ranks
+// (buf->d_rec, written at hand-over), through perm when a deskew order was applied.  Queued before the plan's free_ev.
+int keep_plan(madicp_ctx* c, cudaStream_t st, BuildState* bs, const madicp_plan* plan, const int* perm, int64_t kept) {
+  bs->idx_ok = false;
+  if (!c->keep_cloud || !plan->keep) return MADICP_OK;  // (handed over before the context kept clouds: the build says so)
+  if (int e = ensure_idx(bs)) return e;
+  if (perm) {
+    if (int e = keep_compose(c, st, perm, plan->buf->d_rec, kept, bs->d_idx)) return e;
+  } else {
+    CK(cudaMemcpyAsync(bs->d_idx, plan->buf->d_rec, size_t(kept) * sizeof(int), cudaMemcpyDeviceToDevice, st));
+  }
+  bs->idx_ok = true;
+  return MADICP_OK;
 }
 
 // madicp_ingest_plan of a plan of device records: its kept points (and, deskewing, their order) are on the device.
@@ -1316,6 +1407,7 @@ int ingest_planned_dev(madicp_ctx* c, madicp_plan* plan, int deskew, const doubl
   } else {
     CK(cudaMemcpyAsync(bs->P[0], pts, size_t(kept) * 24, cudaMemcpyDeviceToDevice, st));
   }
+  if (int e = keep_plan(c, st, bs, plan, deskew ? plan->buf->d_perm : nullptr, kept)) return e;
   CK(cudaEventRecord(plan->buf->free_ev, st));  // (the plan's buffers may be reused once this has run)
   return ingest_done(bs, st, kept, n_kept, points_out);
 }
@@ -1357,6 +1449,7 @@ int ingest_planned_time(madicp_ctx* c, madicp_plan* plan, int deskew, const doub
   } else {
     CK(cudaMemcpyAsync(bs->P[0], b->d_pts, size_t(kept) * 24, cudaMemcpyDeviceToDevice, st));
   }
+  if (int e = keep_plan(c, st, bs, plan, nullptr, kept)) return e;
   CK(cudaEventRecord(b->free_ev, st));  // (the plan's buffers may be reused once this has run)
   return ingest_done(bs, st, kept, n_kept, points_out);
 }
@@ -1383,6 +1476,10 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
   bs->kept_check = 0;
   bs->vc_check = vc.enabled != 0;
   bs->time_check = false;
+  bs->idx_ok = false;
+  const bool keep = c->keep_cloud;
+  if (keep)
+    if (int e = ensure_idx(bs)) return e;
   const char* raw = static_cast<const char*>(bs->d_raw);
   if (plan) {  // the records, the permutation and the chunks went up on the plan lane's stream
     CK(cudaStreamWaitEvent(st, plan->buf->ready, 0));
@@ -1410,6 +1507,8 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
       k<<<blocks(kept), kBlock, 0, st>>>(B, plan->buf->d_perm, plan->buf->d_chunk, bs->d_poses, int(kept), bs->P[0],
                                          bs->d_vtab, bs->h_vc_err);
       c->launches++;
+      if (keep)  // (the plan's order holds record indices already)
+        CK(cudaMemcpyAsync(bs->d_idx, plan->buf->d_perm, size_t(kept) * sizeof(int), cudaMemcpyDeviceToDevice, st));
     }
   } else if (timed) {  // no order, no host half: the chunk poses through the pinned ring, then passes 1 and 2
     PlanLane* L = nullptr;
@@ -1417,6 +1516,8 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
     if (int e = stage_chunk_poses(L, st, T_prev, T_now, sensor_hz, kTimeChunks, bs->d_poses)) return e;
     const TimeArgs T = time_args(tm, raw, sensor_hz, bs->d_tmax, bs->h_t_err, bs->d_poses, nullptr);
     if (int e = launch_compaction_time(c, bs, st, B, T, bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) return e;
+    if (keep)
+      if (int e = keep_records(c, st, bs, B, true, bs->d_idx)) return e;
     kept = kept_count_host(d);  // (compared with the device's count at the build's first host sync, as the stamps are)
     bs->kept_check = 1;
     bs->time_check = true;
@@ -1436,17 +1537,24 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, in
       k<<<blocks(kept), kBlock, 0, st>>>(B, bs->d_perm, bs->d_chunk, bs->d_poses, int(kept), bs->P[0], bs->d_vtab,
                                          bs->h_vc_err);
       c->launches++;
+      if (keep)  // (the order holds record indices already)
+        CK(cudaMemcpyAsync(bs->d_idx, bs->d_perm, size_t(kept) * sizeof(int), cudaMemcpyDeviceToDevice, st));
     }
   } else if (points_gated(d)) {
     if (int e = launch_compaction(c, bs, st, B, bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) return e;
+    if (keep)
+      if (int e = keep_records(c, st, bs, B, true, bs->d_idx)) return e;
     kept = root_host(d, vc, bs->root_S);
     bs->kept_check = 1;
   } else {
     auto k = vc.enabled ? k_ingest<true> : k_ingest<false>;
     k<<<blocks(n), kBlock, 0, st>>>(B, nullptr, nullptr, bs->d_poses, int(n), bs->P[0], bs->d_vtab, bs->h_vc_err);
     c->launches++;
+    if (keep)
+      if (int e = keep_records(c, st, bs, B, false, bs->d_idx)) return e;
     kept = root_host(d, vc, bs->root_S);
   }
+  bs->idx_ok = keep;
   CK(cudaGetLastError());
   if (plan) CK(cudaEventRecord(plan->buf->free_ev, st));  // (the plan's buffers may be reused once this has run)
   if (kept == 0) {
@@ -1612,6 +1720,12 @@ int madtree_gpu_build(madicp_ctx_t* c, const double* points_xyz, int64_t n, doub
   bs->vc_check = false;
   bs->time_check = false;
   bs->has_root_S = true;
+  bs->idx_ok = c->keep_cloud;
+  if (c->keep_cloud) {
+    const int first[2] = {0, int(n)};
+    if (int e = ensure_idx(bs)) return e;
+    if (int e = keep_records(c, c->stream, bs, batch_of_firsts(first, 1), false, bs->d_idx)) return e;
+  }
   return build_resident(c, bs, c->stream, n, b_max, b_min, bs->root_S, out);
   MADICP_CATCH("madtree_gpu_build")
 }
@@ -1787,7 +1901,8 @@ namespace {
 // The device half of madicp_plan_points_dev, on the context's stream (whose build lane holds the scan scratch the
 // compaction needs): the scan's kept points, gated and corrected, into the plan buffer b as packed float64; b->compacted
 // follows.
-int plan_compact_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, void* producer, PlanBuf* b) {
+// keep: the records of the kept ranks go to b->d_rec too (madicp_set_keep_cloud).
+int plan_compact_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, void* producer, PlanBuf* b, bool keep) {
   BuildState* bs = static_cast<BuildState*>(c->build_state);
   if (bs && bs->cap < size_t(d.n))  // the lane is about to be re-allocated: early uploads are lost
     if (int e = drop_staged(bs, c->stream)) return e;
@@ -1803,6 +1918,10 @@ int plan_compact_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr
   B.n_rec = int(d.n);
   B.s[0] = rec_src(d, d.data, 0, slot);
   if (int e = launch_compaction(c, bs, st, B, reinterpret_cast<double*>(b->d_raw), b->h_cnt, b->h_cnt + 1, vc.enabled)) return e;
+  if (keep) {
+    if (!b->d_rec) CK(cudaMalloc(&b->d_rec, b->cap * sizeof(int)));
+    if (int e = keep_records(c, st, bs, B, true, b->d_rec)) return e;
+  }
   CK(cudaEventRecord(b->compacted, st));
   return MADICP_OK;
 }
@@ -1831,9 +1950,10 @@ int madicp_plan_points_dev(madicp_ctx_t* c, const madicp_points_t* desc, const m
   p->d = *desc;
   p->vc = vcorr_of(vcorr);
   p->dev = true;
+  p->keep = c->keep_cloud;
   p->buf = b;
   p->done = p->done_p.get_future();
-  if (int e = plan_compact_dev(c, *desc, p->vc, producer_stream, b)) {
+  if (int e = plan_compact_dev(c, *desc, p->vc, producer_stream, b, p->keep)) {
     cudaStreamSynchronize(c->stream);  // (nothing may still read the caller's records, nor write the buffer)
     return_buf(L, b);
     return e;
@@ -1882,6 +2002,10 @@ int plan_time(madicp_ctx* c, madicp_plan* p, void* producer) {
   B.s[0] = rec_src(d, base, 0, slot);
   const TimeArgs T = time_args(p->tm, base, 0.0, b->d_tmax, b->h_cnt + 2, nullptr, b->d_tau);
   if (int e = launch_compaction_time(c, bs, st, B, T, b->d_pts, b->h_cnt, b->h_cnt + 1, p->vc.enabled)) return e;
+  if (p->keep) {  // (madicp_set_keep_cloud: the records of the kept ranks)
+    if (!b->d_rec) CK(cudaMalloc(&b->d_rec, b->cap * sizeof(int)));
+    if (int e = keep_records(c, st, bs, B, true, b->d_rec)) return e;
+  }
   CK(cudaEventRecord(b->compacted, st));
   return MADICP_OK;
 }
@@ -1902,6 +2026,7 @@ int plan_points_time(madicp_ctx* c, const madicp_points_t* desc, const madicp_vc
   p->vc = vcorr_of(vcorr);
   p->tm = times_of(times);
   p->dev = dev;
+  p->keep = c->keep_cloud;
   p->buf = b;
   p->done = p->done_p.get_future();
   if (int e = plan_time(c, p.get(), producer_stream)) {

@@ -1075,5 +1075,25 @@ k_ingest(const __grid_constant__ RecBatch B, const int* __restrict__ perm,
   out[3 * size_t(i) + 2] = z;
 }
 
+// Record indices of a kept cloud (madicp_set_keep_cloud), beside the ingest kernels above and separate from them (they
+// keep their registers).  k_kept_records: rec_of[rank] = the record's index within its own scan, for every record the
+// gate keeps (flag: the gate flags, G / tile_off their tile scan, as k_compact ranks them) or, with flag == nullptr, for
+// every record (no gate: rank = record).
+__global__ void __launch_bounds__(kBlock)
+k_kept_records(const __grid_constant__ RecBatch B, const unsigned char* __restrict__ flag, const int* __restrict__ G,
+               const int* __restrict__ tile_off, int* __restrict__ rec_of) {
+  const int r = blockIdx.x * kBlock + threadIdx.x;
+  if (r >= B.n_rec || (flag && !flag[r])) return;
+  const int o = flag ? G[r] + tile_off[r >> 10] : r;
+  rec_of[o] = r - B.s[rec_scan(B, r)].first;
+}
+// out[j] = rec_of[perm[j]] (a deskew order over kept ranks), or perm[j] when rec_of == nullptr (over records already)
+__global__ void __launch_bounds__(kBlock)
+k_compose_records(const int* __restrict__ perm, const int* __restrict__ rec_of, int n, int* __restrict__ out) {
+  const int j = blockIdx.x * kBlock + threadIdx.x;
+  if (j >= n) return;
+  out[j] = rec_of ? rec_of[perm[j]] : perm[j];
+}
+
 }  // namespace gtb
 }  // namespace madicp

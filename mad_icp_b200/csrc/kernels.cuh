@@ -107,6 +107,16 @@ struct LeafGather {
   double X[12];
 };
 
+// One kept cloud going out (k_cloud_out): its points and record indices on the device, and its pose (row-major [R|t],
+// read only when has_pose != 0)
+struct CloudOut {
+  const double* xyz;
+  const int32_t* idx;
+  long long n;
+  int has_pose, pad;
+  double X[12];
+};
+
 // Control block + results of one registration, in device global memory.
 // LL-style mailbox cell: a double split into two 32-bit halves, each paired with a 32-bit epoch
 // flag, written with ONE 16-byte store so data and flags arrive together (no fence on the wire).

@@ -109,6 +109,30 @@ class DeviceTree:
         """The tree's leaf means in getLeafs order, posed by T (4x4 / 3x4, or None: untouched); see `leaf_means`."""
         return leaf_means([self], [T], device)
 
+    def cloud(self, T=None, device=False):
+        """The cloud the tree was built from (`Registrar.keep_cloud`) and the record index of every point: an (N, 3)
+        float64 array posed by T (4x4 / 3x4, or None: untouched) and an (N,) int64 array, or with device=True torch
+        tensors on the registrar's device, ready on torch's current stream (madtree_gpu_cloud_dev)."""
+        n = check(capi.lib().madtree_gpu_num_cloud_points(self._h), "madtree_gpu_num_cloud_points")
+        X = None if T is None else pose12(T)
+        if not device:
+            xyz, idx = np.empty((n, 3)), np.empty(n, np.int64)
+            check(capi.lib().madtree_gpu_cloud(self._h, as_d(X), as_d(xyz), idx.ctypes.data_as(C.POINTER(C.c_int64))),
+                  "madtree_gpu_cloud")
+            return xyz, idx
+        import torch
+        dev = torch.device("cuda", self._reg.device)
+        xyz = torch.empty((n, 3), dtype=torch.float64, device=dev)
+        idx = torch.empty(n, dtype=torch.int64, device=dev)
+        if n:
+            check(capi.lib().madtree_gpu_cloud_dev(self._h, as_d(X), C.c_void_p(xyz.data_ptr()), C.c_void_p(idx.data_ptr()),
+                                                   C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                  "madtree_gpu_cloud_dev")
+        return xyz, idx
+
+    def release_cloud(self):
+        check(capi.lib().madtree_gpu_release_cloud(self._h), "madtree_gpu_release_cloud")
+
     def export(self):
         """Audit dump of a device-BUILT tree, breadth-first: mean, eivecs (column-major), bbox, num_points."""
         n = self.num_nodes
@@ -198,6 +222,10 @@ class Registrar:
 
     def set_params(self, min_ball, rho_ker, b_ratio):
         check(capi.lib().madicp_set_params(self._h, min_ball, rho_ker, b_ratio), "madicp_set_params")
+
+    def keep_cloud(self, keep=True):
+        """Trees built from now on keep their input cloud and its record indices (`DeviceTree.cloud`)."""
+        check(capi.lib().madicp_set_keep_cloud(self._h, int(bool(keep))), "madicp_set_keep_cloud")
 
     def set_stream(self, cuda_stream_ptr):
         check(capi.lib().madicp_set_stream(self._h, C.c_void_p(cuda_stream_ptr or 0)))

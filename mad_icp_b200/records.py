@@ -298,6 +298,28 @@ def leaves_array_dev(pipeline, model):
     return out
 
 
+def cloud_array_dev(pipeline, indices, map_frame):
+    """Pipeline.currentCloudArray / currentCloudIndices(device=True): the current scan's kept cloud as an (N, 3) float64
+    torch tensor (posed by currentPose() when map_frame), or its record indices (indices=True) as an (N,) int64 tensor, on
+    the pipeline's device, written by the output kernel in place and ready on torch's current stream (no host sync).
+    With host-built trees (MADICP_GPU_BUILD=0) the host array is copied up once."""
+    import torch
+    dev = torch.device("cuda", pipeline._device())
+    if not pipeline.gpuBuild():
+        host = (pipeline.currentCloudIndices() if indices
+                else pipeline.currentCloudArray(frame="map" if map_frame else "sensor"))
+        return torch.from_numpy(host).to(dev)
+    n = pipeline._numCloudPoints()
+    out = torch.empty((n,) if indices else (n, 3), dtype=torch.int64 if indices else torch.float64, device=dev)
+    if n:
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        if indices:
+            pipeline._cloudDev(False, 0, out.data_ptr(), stream)
+        else:
+            pipeline._cloudDev(map_frame, out.data_ptr(), 0, stream)
+    return out
+
+
 def vcorr(apply_correction=False, vertical_angle_offset=VERTICAL_ANGLE_OFFSET):
     """madicp_vcorr_t of the reader's `apply_correction` / `vertical_angle_offset`, or None without a correction."""
     if not apply_correction:
@@ -335,5 +357,5 @@ def correct_vertical_angle(records, vertical_angle_offset=VERTICAL_ANGLE_OFFSET,
     return out[:kept]
 
 
-__all__ = ["pointcloud2_dtype", "describe", "describe_times", "time_layout", "time_chunks", "chunk_poses", "layout", "to_host", "search_cloud_arrays_dev", "leaves_array_dev", "range_mask", "vcorr", "correct_vertical_angle",
+__all__ = ["pointcloud2_dtype", "describe", "describe_times", "time_layout", "time_chunks", "chunk_poses", "layout", "to_host", "search_cloud_arrays_dev", "leaves_array_dev", "cloud_array_dev", "range_mask", "vcorr", "correct_vertical_angle",
            "VERTICAL_ANGLE_OFFSET", "RANGE_NONE", "RANGE_INCLUSIVE", "RANGE_STRICT"]

@@ -50,6 +50,17 @@ struct RootSums {  // Sigma x, Sigma x x^T of a scan's kept points, and their nu
   int64_t kept;
 };
 
+// The cloud an ingest left in P[0] for madtree_gpu_build_resident, and the checks its build still owes it.  Every ingest
+// starts by resetting all of it (begin_ingest): build_forest trusts these flags for its deferred checks.
+struct Resident {
+  int64_t n = 0;            // points of the cloud (the kept ones); 0: none
+  bool has_root_S = false;  // BuildState::root_S holds its root's sums
+  int kept_check = 0;       // scans of the cloud whose h_kept the next build compares with the host's count
+  bool vc_check = false;    // the cloud was corrected: the next build checks h_vc_err
+  bool time_check = false;  // the cloud was deskewed by its stamps: the next build checks h_t_err
+  bool idx_ok = false;      // d_idx holds the record index of every point
+};
+
 struct BuildState {
   size_t cap = 0;  // points
   double* P[2] = {nullptr, nullptr};
@@ -84,18 +95,15 @@ struct BuildState {
   void* d_raw = nullptr;  // the raw scans as uploaded (packed float32 or records), raw_cap bytes
   size_t raw_cap = 0;
   int* h_kept = nullptr;  // mapped: kept points of every scan, counted by the device's compaction (k_compact)
-  int kept_check = 0;     // scans of the resident cloud whose h_kept the next build compares with the host's count
   // vertical correction (vertical_correction.h): one table per distinct angle, kept while the lane lives.  The host
   // copy of slot k is written once, before its upload is queued, and never again until every upload has run.
   VcorrTable* d_vtab = nullptr;
   VcorrTable* h_vtab = nullptr;        // pinned
   std::vector<double> vtab_angle;      // angle of slot k
   int* h_vc_err = nullptr;             // mapped: a corrected point's rotation angle fell outside its table
-  bool vc_check = false;               // the resident cloud was corrected: the next build checks h_vc_err
   // time-stamp deskew (time_deskew.h): the largest kept stamp's key, and a kept stamp that is NaN or infinite (mapped)
   unsigned long long* d_tmax = nullptr;
   int* h_t_err = nullptr;
-  bool time_check = false;             // the resident cloud was deskewed by its stamps: the next build checks h_t_err
   int* d_perm = nullptr;
   unsigned short* d_chunk = nullptr;
   double* d_poses = nullptr;
@@ -104,14 +112,12 @@ struct BuildState {
   double* h_poses = nullptr;
   double* h_packed = nullptr;  // pinned, 3 x cap, at first use: a deskewed device scan's kept points for the host's order
   // kept clouds (madicp_set_keep_cloud), at first use: the record index of every point of the cloud in P[0] (valid when
-  // idx_ok), and the records of a compaction's kept ranks before a deskew order is composed with them
+  // res.idx_ok), and the records of a compaction's kept ranks before a deskew order is composed with them
   int* d_idx = nullptr;
   int* d_rec = nullptr;
-  bool idx_ok = false;
   double* h_root = nullptr;  // pinned: the root's sums when the host computes them
-  double root_S[9];          // ... of the cloud madicp_ingest left in P[0] (valid when has_root_S)
-  bool has_root_S = false;
-  int64_t n_resident = 0;  // points of the cloud madicp_ingest left in P[0] (the kept ones)
+  double root_S[9];          // ... of the resident cloud (valid when res.has_root_S)
+  Resident res;
   uint64_t seq = 0;        // builds so far (madtree_gpu_export is valid for the latest one only)
   int threads = 16;
   // early uploads for the next batch (madicp_stage_cloud / madicp_stage_points): scans already on their way into P[0]
@@ -304,6 +310,14 @@ int mark_idle(BuildState* bs, cudaStream_t st) {
   CK(cudaEventRecord(bs->idle_ev, st));
   return MADICP_OK;
 }
+// The start of an ingest into P[0] (ensure_state's n and raw_bytes): staged scans are given up, and P[0] holds no
+// resident cloud until the ingest has finished.
+int begin_ingest(madicp_ctx* c, size_t n, size_t raw_bytes, BuildState** out) {
+  if (int e = drop_staged(static_cast<BuildState*>(c->build_state), c->stream)) return e;
+  if (int e = ensure_state(c, n, raw_bytes, out)) return e;
+  (*out)->res = Resident{};
+  return MADICP_OK;
+}
 
 // Sigma x, Sigma x x^T of the whole cloud in array order (tools/utils.h:55-73) on the calling host thread: the root's
 // nine chains are the longest dependent-add chains of the build (n adds each; a CPU core retires one per ~1 ns, the
@@ -476,7 +490,7 @@ int build_forest(madicp_ctx* c, BuildState* bs, cudaStream_t st, int n_trees, co
   // its slice
   std::shared_ptr<CloudBuf> kept;
   if (c->keep_cloud) {
-    if (!bs->idx_ok) {
+    if (!bs->res.idx_ok) {
       set_error("madtree_gpu_build: the cloud was ingested before madicp_set_keep_cloud: its record indices are unknown");
       return MADICP_ERR_STATE;
     }
@@ -564,11 +578,11 @@ int build_forest(madicp_ctx* c, BuildState* bs, cudaStream_t st, int n_trees, co
     CK(cudaStreamSynchronize(st));  // the level's one host round trip: libm for the eigen-decomposition
     const auto ts1 = now();
     t_sync += us(ts0, ts1);
-    if (depth == 0 && bs->vc_check && *bs->h_vc_err) {
+    if (depth == 0 && bs->res.vc_check && *bs->h_vc_err) {
       set_error("madtree_gpu_build: a point's rotation angle lies outside the table of the vertical correction");
       return MADICP_ERR_STATE;
     }
-    if (depth == 0 && bs->time_check && *bs->h_t_err) {
+    if (depth == 0 && bs->res.time_check && *bs->h_t_err) {
       set_error("madtree_gpu_build: a kept point's time stamp is NaN or infinite");
       return MADICP_ERR_STATE;
     }
@@ -675,7 +689,7 @@ int build_forest(madicp_ctx* c, BuildState* bs, cudaStream_t st, int n_trees, co
 int build_resident(madicp_ctx* c, BuildState* bs, cudaStream_t st, int64_t n, double b_max, double b_min, const double* root_S,
                    madtree_gpu** out) {
   const int offs[2] = {0, int(n)};
-  return build_forest(c, bs, st, 1, offs, b_max, b_min, root_S, bs->kept_check, out);
+  return build_forest(c, bs, st, 1, offs, b_max, b_min, root_S, bs->res.kept_check, out);
 }
 
 struct PlanLane;  // (look-ahead plans, below)
@@ -765,6 +779,17 @@ RecSrc rec_src(const madicp_points_t& d, const void* base, int first, int vc) {
   s.lo = d.is_f32 ? double(float(d.min_range)) : d.min_range;  // rounded to the field type once
   s.hi = d.is_f32 ? double(float(d.max_range)) : d.max_range;
   return s;
+}
+// The one-scan batch of the records d at `base` (device memory), its correction's table in place (vtab_room, vtab_slot)
+int one_scan(BuildState* bs, cudaStream_t st, const madicp_points_t& d, const madicp_vcorr_t& vc, const void* base,
+             RecBatch* B) {
+  int slot = -1;
+  if (int e = vtab_room(bs, st, &vc, 1)) return e;
+  if (int e = vtab_slot(bs, st, vc, &slot)) return e;
+  B->count = 1;
+  B->n_rec = int(d.n);
+  B->s[0] = rec_src(d, base, 0, slot);
+  return MADICP_OK;
 }
 // Order-preserving compaction of the gated records of B into `out` (packed float64; bs->P[0] unless a deskew or a plan
 // needs the kept points elsewhere); the kept count of every scan goes to kept[] and a correction outside its table raises
@@ -870,12 +895,8 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* v
                          dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
     else if (!dev) CK(cudaMemcpyAsync(raw + raw_off[b], d[b].data, points_bytes(d[b]), cudaMemcpyHostToDevice, st));
   }
-  bs->n_resident = 0;  // the concatenated clouds are not "the resident cloud" of madtree_gpu_build_resident
-  bs->has_root_S = false;
-  bs->kept_check = 0;
-  bs->vc_check = corrected;
-  bs->time_check = false;
-  bs->idx_ok = false;
+  bs->res = Resident{};  // the concatenated clouds are not "the resident cloud" of madtree_gpu_build_resident
+  bs->res.vc_check = corrected;
   if (c->keep_cloud)
     if (int e = ensure_idx(bs)) return e;
   if (!direct) {
@@ -901,7 +922,7 @@ int build_batch(madicp_ctx* c, const madicp_points_t* d, const madicp_vcorr_t* v
   } else if (c->keep_cloud) {
     if (int e = keep_records(c, st, bs, batch_of_firsts(first, count), false, bs->d_idx)) return e;
   }
-  bs->idx_ok = c->keep_cloud;
+  bs->res.idx_ok = c->keep_cloud;
   const auto ta1 = std::chrono::steady_clock::now();
   // the roots' sums and the kept counts on the host, one scan per host thread, while the scans are being copied up; a
   // batch holding a corrected scan has its roots summed on the device (root_host), and so has a batch of device scans,
@@ -950,18 +971,13 @@ int stage(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int
   if (!bs || bs->staged.empty()) {
     const int64_t res = std::max(reserve_points, d.n);
     const size_t res_bytes = raw ? size_t(res) * size_t(d.stride) + 16 * size_t(kMaxBatch) : 0;
-    int rc = ensure_state(c, size_t(res), res_bytes, &bs);
-    if (rc) return rc;
+    // (nothing is staged: begin_ingest gives nothing up; the cloud madicp_ingest left is about to be overwritten)
+    if (int e = begin_ingest(c, size_t(res), res_bytes, &bs)) return e;
     CK(cudaEventRecord(bs->idle_ev, c->stream));  // whatever is queued on the context's stream may still use the buffers
     CK(cudaStreamWaitEvent(bs->copy_stream, bs->idle_ev, 0));
     bs->staged_raw = raw;
     bs->staged_points = 0;
     bs->staged_bytes = 0;
-    bs->n_resident = 0;  // the cloud madicp_ingest left is about to be overwritten
-    bs->has_root_S = false;
-    bs->kept_check = 0;
-    bs->vc_check = false;
-    bs->time_check = false;
   }
   const size_t at = align16(bs->staged_bytes);
   if (bs->staged_raw != raw || size_t(bs->staged_points + d.n) > bs->cap || (raw && at + bytes > bs->raw_cap) ||
@@ -1166,7 +1182,7 @@ struct madicp_plan {
   madicp_vcorr_t vc{};
   bool dev = false;  // device records: buf->d_raw holds the kept points (PlanBuf)
   madicp_times_t tm{};  // a time field (tm.type != kTimeNone): no order half, buf->d_pts / d_tau hold the kept points
-  bool keep = false;    // the hand-over's compaction (device records, time field) wrote buf->d_rec
+  bool keep = false;    // the context kept clouds at hand-over: a compaction there (device records, time field) wrote buf->d_rec
   PlanBuf* buf = nullptr;
   std::promise<void> done_p;
   std::future<void> done;  // the order half has run and its uploads are queued
@@ -1259,334 +1275,362 @@ RecBatch packed_batch(const double* pts, int64_t kept) {
   return B;
 }
 
-// The end of an ingest: the cloud of `kept` points in P[0] is the resident one (its root summed on the device), and
-// n_kept / points_out (host memory, synchronises) receive it.
-int ingest_done(BuildState* bs, cudaStream_t st, int64_t kept, int64_t* n_kept, double* points_out) {
-  CK(cudaGetLastError());
-  bs->n_resident = kept;
-  bs->has_root_S = false;
-  if (n_kept) *n_kept = kept;
-  if (points_out) {
-    CK(cudaMemcpyAsync(points_out, bs->P[0], size_t(kept) * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+// How a scan is deskewed as it is ingested: the deskew flag, poses, rate and host threads of madicp_ingest*
+struct Deskew {
+  int on;
+  const double* T_prev;
+  const double* T_now;
+  double hz;
+  int num_threads;
+  bool ok() const { return !on || (T_prev && T_now && hz > 0.0); }
+};
+
+std::string no_point(const char* fn) { return std::string(fn) + ": no point inside the range gate"; }
+
+// The outcome of a plan that has been handed over: its kept count, or what its order half or its compaction met.
+// timed: the deskew uses the plan's stamps, which must then be finite.
+int plan_outcome(const madicp_plan* p, bool timed, const char* fn, int64_t* kept) {
+  if (p->tm.type != kTimeNone) {  // compacted on the context's stream when handed over: no host half
+    const PlanBuf* b = p->buf;
+    CK(cudaEventSynchronize(b->compacted));  // (long done when the plan was handed over ahead of its turn)
+    if (b->h_cnt[1]) {
+      set_error(vcorr_out_of_table(fn, p->vc.angle));
+      return MADICP_ERR_STATE;
+    }
+    if (timed && b->h_cnt[2]) {
+      set_error(time_not_finite(fn));
+      return MADICP_ERR_STATE;
+    }
+    *kept = b->h_cnt[0];
+    return MADICP_OK;
   }
+  if (p->rc == MADICP_ERR_STATE) set_error(vcorr_out_of_table(fn, p->vc.angle));
+  else if (p->rc) set_error(p->err);
+  *kept = p->kept;
+  return p->rc;
+}
+
+// The host's deskew order of the records d (madicp_deskew_plan, after the previous scan's h_perm / h_chunk / h_poses
+// have been consumed), uploaded to d_perm / d_chunk / d_poses on `st`.  *kept: the records the gate keeps.
+int host_order(BuildState* bs, cudaStream_t st, const madicp_points_t& d, const madicp_vcorr_t& vc, const Deskew& k,
+               const char* fn, int64_t* kept) {
+  CK(cudaStreamSynchronize(st));
+  int n_poses = 0;
+  VcorrTable table;  // (the azimuths are those of the corrected points)
+  const int rc = madicp_deskew_plan(d, vcorr_table(vc, &table), k.T_prev, k.T_now, k.hz, k.num_threads, bs->h_perm,
+                                    bs->h_chunk, bs->h_poses, &n_poses, kept);
+  if (rc == MADICP_ERR_STATE) set_error(vcorr_out_of_table(fn, vc.angle));
+  if (rc || *kept == 0) return rc;
+  CK(cudaMemcpyAsync(bs->d_perm, bs->h_perm, size_t(*kept) * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(bs->d_chunk, bs->h_chunk, size_t(*kept) * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(bs->d_poses, bs->h_poses, size_t(n_poses) * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
   return MADICP_OK;
 }
 
-// The ingest behind madicp_ingest_points_dev (descriptor, correction and device pointer validated; the context's stream
-// already waits for the producer).  The records are read in place: the gate, the correction and the compaction run as
-// for uploaded records, and the kept count comes back from the device (one synchronisation).  deskew: the kept points
-// are compacted into P[1], copied back for the host's order half (madicp_deskew_plan over a packed, plain cloud -- the
-// same points, so the same permutation and chunks), and gathered from there into P[0].
-// With a time field and a deskew the whole deskew is the compaction's pass 2 (launch_compaction_time), straight into P[0].
-int ingest_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int deskew, const double T_prev[12],
-               const double T_now[12], double sensor_hz, int num_threads, int64_t* n_kept, double* points_out,
-               const char* fn, const madicp_times_t& tm = madicp_times_t{}) {
-  const bool timed = deskew && tm.type != kTimeNone;
-  BuildState* bs = nullptr;
-  int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
-  if (!rc) rc = ensure_state(c, size_t(d.n), 0, &bs);
-  if (rc) return rc;
-  cudaStream_t st = c->stream;
-  bs->n_resident = 0;
-  bs->kept_check = 0;
-  bs->vc_check = false;  // (an angle outside the table fails this call)
-  bs->time_check = false;
-  bs->idx_ok = false;
-  const bool keep = c->keep_cloud;
-  if (keep)
-    if (int e = ensure_idx(bs)) return e;
+// Applies a deskew order: k_ingest gathers the kept points of B through perm into P[0], each moved by the pose of its
+// chunk (d_poses, queued on `st`).  idx: the record indices follow into d_idx -- perm itself when B holds the scan's
+// records, rec[perm] when B holds kept points whose records are rec.
+int apply_order(madicp_ctx* c, BuildState* bs, cudaStream_t st, const RecBatch& B, bool vc, const int* perm,
+                const uint16_t* chunk, int64_t kept, bool idx, const int* rec) {
+  auto k = vc ? k_ingest<true> : k_ingest<false>;
+  k<<<blocks(kept), kBlock, 0, st>>>(B, perm, chunk, bs->d_poses, int(kept), bs->P[0], bs->d_vtab, bs->h_vc_err);
+  c->launches++;
+  if (!idx) return MADICP_OK;
+  if (rec) return keep_compose(c, st, perm, rec, kept, bs->d_idx);
+  CK(cudaMemcpyAsync(bs->d_idx, perm, size_t(kept) * sizeof(int), cudaMemcpyDeviceToDevice, st));
+  return MADICP_OK;
+}
+
+// The end of every ingest: the cloud of `kept` points in P[0] becomes the resident one, and n_kept / points_out (host
+// memory: synchronises, and runs the checks the build would otherwise defer) receive it.
+int finish_ingest(BuildState* bs, cudaStream_t st, int64_t kept, bool has_root_S, int64_t* n_kept, double* points_out,
+                  const char* fn, double angle) {
+  CK(cudaGetLastError());
+  if (kept == 0) {
+    bs->res = Resident{};
+    set_error(no_point(fn));
+    return MADICP_ERR_INVALID;
+  }
+  bs->res.n = kept;
+  bs->res.has_root_S = has_root_S;
+  if (n_kept) *n_kept = kept;
+  if (!points_out) return MADICP_OK;
+  CK(cudaMemcpyAsync(points_out, bs->P[0], size_t(kept) * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  std::string err;
+  if (bs->res.vc_check && *bs->h_vc_err) err = vcorr_out_of_table(fn, angle);
+  else if (bs->res.time_check && *bs->h_t_err) err = time_not_finite(fn);
+  else if (bs->res.kept_check && bs->h_kept[0] != kept)
+    err = std::string(fn) + ": the device kept " + std::to_string(bs->h_kept[0]) + " points, the host " + std::to_string(kept);
+  if (err.empty()) return MADICP_OK;
+  set_error(err);
+  bs->res.n = 0;
+  return MADICP_ERR_STATE;
+}
+
+// The one ingest behind madicp_ingest, madicp_ingest_points[_ex|_t|_dev|_dev_t] and madicp_ingest_plan (arguments
+// validated; dev: the records are in device memory and the context's stream already waits for their producer).  A route
+// is three choices:
+//  - where the records are read from: uploaded into d_raw (host records), in place (dev), or a plan's buffer: the records
+//    as the plan lane uploaded them, or the kept points of a plan compacted when it was handed over (device records, or a
+//    time field);
+//  - how the kept points are made: a copy (a compacted plan; a packed float64 device cloud without gate or correction),
+//    k_ingest (ungated host records), launch_compaction (gated or device records) or launch_compaction_time;
+//  - which deskew: none, the azimuth order (the host's over the host records or over the kept points copied back, or the
+//    plan's), or the time stamps (the compaction's pass 2, or k_deskew_times over a compacted plan).
+// Host records leave the kept-count, correction and time-stamp checks to the build's first host synchronisation (or to
+// points_out); device records and compacted plans are checked here.
+int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, const madicp_times_t& tm, bool dev,
+           madicp_plan* plan, const Deskew& k, int64_t* n_kept, double* points_out, const char* fn) {
+  PlanBuf* pb = plan ? plan->buf : nullptr;
+  const bool compacted = plan && (plan->dev || plan->tm.type != kTimeNone);
+  const bool timed = k.on && tm.type != kTimeNone;
+  const bool deferred = !dev && !compacted;
   int64_t kept = d.n;
-  if (is_direct(d, vc) && !deskew) {
+  CK(cudaSetDevice(c->device));
+  if (compacted) {
+    if (int e = plan_outcome(plan, timed, fn, &kept)) return e;
+    if (kept == 0) {
+      set_error(no_point(fn));
+      return MADICP_ERR_INVALID;
+    }
+  }
+  BuildState* bs = nullptr;
+  if (int e = begin_ingest(c, size_t(d.n), (dev || plan) ? 0 : size_t(d.n) * size_t(d.stride), &bs)) return e;
+  cudaStream_t st = c->stream;
+  bs->res.vc_check = deferred && vc.enabled;
+  const bool idx = c->keep_cloud && (!compacted || plan->keep);  // (a plan handed over before the context kept clouds:
+                                                                 // the build says so)
+  if (c->keep_cloud)
+    if (int e = ensure_idx(bs)) return e;
+  const char* base = static_cast<const char*>(d.data);
+  if (plan) {
+    if (plan->tm.type == kTimeNone) CK(cudaStreamWaitEvent(st, pb->ready, 0));  // (the order half's uploads)
+    base = pb->d_raw;
+  } else if (!dev) {  // the raw scan goes up while the host works out the order (deskew) or the root's sums
+    CK(cudaMemcpyAsync(bs->d_raw, d.data, points_bytes(d, timed ? tm : madicp_times_t{}), cudaMemcpyHostToDevice, st));
+    base = static_cast<const char*>(bs->d_raw);
+  }
+  if (compacted) {  // the plan's kept points, packed float64 (and their stamps)
+    const double* pts = plan->tm.type != kTimeNone ? pb->d_pts : reinterpret_cast<const double*>(pb->d_raw);
+    if (k.on)
+      if (int e = stage_chunk_poses(plan->lane, st, k.T_prev, k.T_now, k.hz, timed ? kTimeChunks : plan->n_chunks,
+                                    bs->d_poses))
+        return e;
+    if (k.on && !timed) {
+      if (int e = apply_order(c, bs, st, packed_batch(pts, kept), false, pb->d_perm, pb->d_chunk, kept, idx, pb->d_rec))
+        return e;
+    } else {
+      if (timed) {
+        const TimeArgs T = time_args(tm, nullptr, k.hz, pb->d_tmax, nullptr, bs->d_poses, nullptr);
+        k_deskew_times<<<blocks(kept), kBlock, 0, st>>>(pts, pb->d_tau, int(kept), T, bs->P[0]);
+        c->launches++;
+      } else {
+        CK(cudaMemcpyAsync(bs->P[0], pts, size_t(kept) * 24, cudaMemcpyDeviceToDevice, st));
+      }
+      if (idx) CK(cudaMemcpyAsync(bs->d_idx, pb->d_rec, size_t(kept) * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    }
+  } else if (dev && !k.on && is_direct(d, vc)) {
     CK(cudaMemcpyAsync(bs->P[0], d.data, size_t(d.n) * 24, cudaMemcpyDeviceToDevice, st));
     const int first[2] = {0, int(d.n)};
-    if (keep)
+    if (idx)
       if (int e = keep_records(c, st, bs, batch_of_firsts(first, 1), false, bs->d_idx)) return e;
   } else {
-    int slot = -1;
     if (vc.enabled) CK(cudaMemsetAsync(bs->h_vc_err, 0, sizeof(int), st));
-    if (int e = vtab_room(bs, st, &vc, 1)) return e;
-    if (int e = vtab_slot(bs, st, vc, &slot)) return e;
     RecBatch B;
-    B.count = 1;
-    B.n_rec = int(d.n);
-    B.s[0] = rec_src(d, d.data, 0, slot);
-    if (timed) {
+    if (int e = one_scan(bs, st, d, vc, base, &B)) return e;
+    if (plan && k.on) {  // a plan of host records: only the chunk poses are left
+      if (int e = plan_outcome(plan, false, fn, &kept)) return e;
+      if (kept > 0) {
+        if (int e = stage_chunk_poses(plan->lane, st, k.T_prev, k.T_now, k.hz, plan->n_chunks, bs->d_poses)) return e;
+        if (int e = apply_order(c, bs, st, B, vc.enabled, pb->d_perm, pb->d_chunk, kept, idx, nullptr)) return e;
+      }
+    } else if (timed) {  // no order, no host half: the chunk poses through the pinned ring, then passes 1 and 2
       PlanLane* L = nullptr;
       if (int e = plan_lane(c, &L)) return e;
-      if (int e = stage_chunk_poses(L, st, T_prev, T_now, sensor_hz, kTimeChunks, bs->d_poses)) return e;
-      const TimeArgs T = time_args(tm, d.data, sensor_hz, bs->d_tmax, bs->h_t_err, bs->d_poses, nullptr);
+      if (int e = stage_chunk_poses(L, st, k.T_prev, k.T_now, k.hz, kTimeChunks, bs->d_poses)) return e;
+      const TimeArgs T = time_args(tm, base, k.hz, bs->d_tmax, bs->h_t_err, bs->d_poses, nullptr);
       if (int e = launch_compaction_time(c, bs, st, B, T, bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) return e;
-    } else if (int e = launch_compaction(c, bs, st, B, deskew ? bs->P[1] : bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) {
-      return e;
+      if (idx)
+        if (int e = keep_records(c, st, bs, B, true, bs->d_idx)) return e;
+    } else if (k.on && !dev) {
+      if (int e = host_order(bs, st, d, vc, k, fn, &kept)) return e;
+      if (kept > 0)
+        if (int e = apply_order(c, bs, st, B, vc.enabled, bs->d_perm, bs->d_chunk, kept, idx, nullptr)) return e;
+    } else if (dev || points_gated(d)) {  // (device records, deskewing: into P[1] for the order below)
+      if (int e = launch_compaction(c, bs, st, B, k.on ? bs->P[1] : bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) return e;
+      if (idx)
+        if (int e = keep_records(c, st, bs, B, true, k.on ? bs->d_rec : bs->d_idx)) return e;
+    } else {
+      auto kern = vc.enabled ? k_ingest<true> : k_ingest<false>;
+      kern<<<blocks(d.n), kBlock, 0, st>>>(B, nullptr, nullptr, bs->d_poses, int(d.n), bs->P[0], bs->d_vtab, bs->h_vc_err);
+      c->launches++;
+      if (idx)
+        if (int e = keep_records(c, st, bs, B, false, bs->d_idx)) return e;
     }
-    // (azimuth deskew: the kept ranks' records, composed with the order below)
-    if (keep)
-      if (int e = keep_records(c, st, bs, B, true, (deskew && !timed) ? bs->d_rec : bs->d_idx)) return e;
-    CK(cudaStreamSynchronize(st));
-    if (vc.enabled && *bs->h_vc_err) {
-      set_error(vcorr_out_of_table(fn, vc.angle));
-      return MADICP_ERR_STATE;
+    if (dev) {  // the device's count, and its checks, now
+      CK(cudaStreamSynchronize(st));
+      if (vc.enabled && *bs->h_vc_err) {
+        set_error(vcorr_out_of_table(fn, vc.angle));
+        return MADICP_ERR_STATE;
+      }
+      if (timed && *bs->h_t_err) {
+        set_error(time_not_finite(fn));
+        return MADICP_ERR_STATE;
+      }
+      kept = bs->h_kept[0];
+      if (k.on && !timed && kept > 0) {  // the kept points come back for the host's order: a packed, plain cloud
+        if (!bs->h_packed)
+          if (int e = host_alloc(bs, &bs->h_packed, 3 * bs->cap)) return e;
+        CK(cudaMemcpyAsync(bs->h_packed, bs->P[1], size_t(kept) * 24, cudaMemcpyDeviceToHost, st));
+        int64_t n_sorted = 0;
+        if (int e = host_order(bs, st, packed_points(bs->h_packed, kept, 0), madicp_vcorr_t{}, k, fn, &n_sorted)) return e;
+        if (int e = apply_order(c, bs, st, packed_batch(bs->P[1], kept), false, bs->d_perm, bs->d_chunk, kept, idx, bs->d_rec))
+          return e;
+      }
+    } else if (!k.on || timed) {  // host records: the host counts (and sums) while the device works; checked later
+      kept = timed ? kept_count_host(d) : root_host(d, vc, bs->root_S);
+      bs->res.kept_check = (timed || points_gated(d)) ? 1 : 0;
+      bs->res.time_check = timed;
     }
-    if (timed && *bs->h_t_err) {
-      set_error(time_not_finite(fn));
-      return MADICP_ERR_STATE;
-    }
-    kept = bs->h_kept[0];
   }
-  if (kept == 0) {
-    set_error(std::string(fn) + ": no point inside the range gate");
-    return MADICP_ERR_INVALID;
-  }
-  if (deskew && !timed) {
-    if (!bs->h_packed)
-      if (int e = host_alloc(bs, &bs->h_packed, 3 * bs->cap)) return e;
-    CK(cudaMemcpyAsync(bs->h_packed, bs->P[1], size_t(kept) * 24, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    int n_poses = 0;
-    int64_t n_sorted = 0;
-    rc = madicp_deskew_plan(packed_points(bs->h_packed, kept, 0), nullptr, T_prev, T_now, sensor_hz, num_threads, bs->h_perm,
-                            bs->h_chunk, bs->h_poses, &n_poses, &n_sorted);
-    if (rc) return rc;
-    CK(cudaMemcpyAsync(bs->d_perm, bs->h_perm, size_t(kept) * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(bs->d_chunk, bs->h_chunk, size_t(kept) * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(bs->d_poses, bs->h_poses, size_t(n_poses) * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
-    k_ingest<false><<<blocks(kept), kBlock, 0, st>>>(packed_batch(bs->P[1], kept), bs->d_perm, bs->d_chunk, bs->d_poses,
-                                                     int(kept), bs->P[0], bs->d_vtab, bs->h_vc_err);
-    c->launches++;
-    if (keep)
-      if (int e = keep_compose(c, st, bs->d_perm, bs->d_rec, kept, bs->d_idx)) return e;
-  }
-  bs->idx_ok = keep;
-  return ingest_done(bs, st, kept, n_kept, points_out);
+  if (plan) CK(cudaEventRecord(pb->free_ev, st));  // (the plan's buffers may be reused once this has run)
+  bs->res.idx_ok = idx;
+  // (a deskewed or corrected cloud exists on the device only: its root sums run there)
+  return finish_ingest(bs, st, kept, deferred && !k.on && !vc.enabled, n_kept, points_out, fn, vc.angle);
 }
 
-// The record indices of a consumed plan's cloud (madicp_set_keep_cloud) into bs->d_idx, from the records of its kept ranks
-// (buf->d_rec, written at hand-over), through perm when a deskew order was applied.  Queued before the plan's free_ev.
-int keep_plan(madicp_ctx* c, cudaStream_t st, BuildState* bs, const madicp_plan* plan, const int* perm, int64_t kept) {
-  bs->idx_ok = false;
-  if (!c->keep_cloud || !plan->keep) return MADICP_OK;  // (handed over before the context kept clouds: the build says so)
-  if (int e = ensure_idx(bs)) return e;
-  if (perm) {
-    if (int e = keep_compose(c, st, perm, plan->buf->d_rec, kept, bs->d_idx)) return e;
-  } else {
-    CK(cudaMemcpyAsync(bs->d_idx, plan->buf->d_rec, size_t(kept) * sizeof(int), cudaMemcpyDeviceToDevice, st));
+// What a plan does when it is handed over.  Host records start going up on the lane's stream once the last ingest that
+// read the buffer has run; a plan of host records without a time field is then the order half's (plan_order).  A plan of
+// device records or with a time field is compacted on the context's stream (whose build lane holds the compaction's
+// scratch) into the plan's buffer: device records as packed float64 into d_raw, for the order half to read back; a time
+// field's kept points and stamps into d_pts / d_tau (passes 1 and 2), which leaves no host half.  b->compacted follows.
+int hand_over(madicp_ctx* c, madicp_plan* p) {
+  PlanBuf* b = p->buf;
+  const madicp_points_t& d = p->d;
+  const bool timed = p->tm.type != kTimeNone;
+  cudaStream_t ls = p->lane->stream;
+  if (!p->dev) {
+    CK(cudaStreamWaitEvent(ls, b->free_ev, 0));
+    CK(cudaMemcpyAsync(b->d_raw, d.data, points_bytes(d, p->tm), cudaMemcpyHostToDevice, ls));
+    if (!timed) return MADICP_OK;
   }
-  bs->idx_ok = true;
-  return MADICP_OK;
-}
-
-// madicp_ingest_plan of a plan of device records: its kept points (and, deskewing, their order) are on the device.
-int ingest_planned_dev(madicp_ctx* c, madicp_plan* plan, int deskew, const double T_prev[12], const double T_now[12],
-                       double sensor_hz, int64_t* n_kept, double* points_out, const char* fn) {
-  CK(cudaSetDevice(c->device));
-  if (plan->rc == MADICP_ERR_STATE) set_error(vcorr_out_of_table(fn, plan->vc.angle));
-  else if (plan->rc) set_error(plan->err);
-  if (plan->rc) return plan->rc;
-  if (plan->kept == 0) {
-    set_error(std::string(fn) + ": no point inside the range gate");
-    return MADICP_ERR_INVALID;
+  if (timed && !b->d_pts) {
+    CK(cudaMalloc(&b->d_pts, b->cap * 3 * sizeof(double)));
+    CK(cudaMalloc(&b->d_tau, b->cap * sizeof(double)));
+    CK(cudaMalloc(&b->d_tmax, sizeof(unsigned long long)));
   }
-  BuildState* bs = nullptr;
-  int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
-  if (!rc) rc = ensure_state(c, size_t(plan->d.n), 0, &bs);
-  if (rc) return rc;
+  BuildState* bs = static_cast<BuildState*>(c->build_state);
+  if (bs && bs->cap < size_t(d.n))  // the lane is about to be re-allocated: early uploads are lost
+    if (int e = drop_staged(bs, c->stream)) return e;
+  if (int e = ensure_state(c, size_t(d.n), 0, &bs)) return e;
   cudaStream_t st = c->stream;
-  bs->n_resident = 0;
-  bs->kept_check = 0;
-  bs->vc_check = false;
-  bs->time_check = false;
-  const int64_t kept = plan->kept;
-  const double* pts = reinterpret_cast<const double*>(plan->buf->d_raw);
-  CK(cudaStreamWaitEvent(st, plan->buf->ready, 0));
-  if (deskew) {
-    if (int e = stage_chunk_poses(plan->lane, st, T_prev, T_now, sensor_hz, plan->n_chunks, bs->d_poses)) return e;
-    k_ingest<false><<<blocks(kept), kBlock, 0, st>>>(packed_batch(pts, kept), plan->buf->d_perm, plan->buf->d_chunk,
-                                                     bs->d_poses, int(kept), bs->P[0], bs->d_vtab, bs->h_vc_err);
-    c->launches++;
-  } else {
-    CK(cudaMemcpyAsync(bs->P[0], pts, size_t(kept) * 24, cudaMemcpyDeviceToDevice, st));
+  const void* base = d.data;
+  if (!p->dev) {
+    CK(cudaEventRecord(b->ready, ls));
+    CK(cudaStreamWaitEvent(st, b->ready, 0));
+    base = b->d_raw;
   }
-  if (int e = keep_plan(c, st, bs, plan, deskew ? plan->buf->d_perm : nullptr, kept)) return e;
-  CK(cudaEventRecord(plan->buf->free_ev, st));  // (the plan's buffers may be reused once this has run)
-  return ingest_done(bs, st, kept, n_kept, points_out);
-}
-
-// madicp_ingest_plan of a plan with a time field: its kept points and their stamps were compacted on the context's stream
-// when it was handed over (plan_time); what is left is the chunk poses and one k_deskew_times.
-int ingest_planned_time(madicp_ctx* c, madicp_plan* plan, int deskew, const double T_prev[12], const double T_now[12],
-                        double sensor_hz, int64_t* n_kept, double* points_out, const char* fn) {
-  CK(cudaSetDevice(c->device));
-  PlanBuf* b = plan->buf;
-  CK(cudaEventSynchronize(b->compacted));  // (long done when the plan was handed over ahead of its turn)
-  if (b->h_cnt[1]) {
-    set_error(vcorr_out_of_table(fn, plan->vc.angle));
-    return MADICP_ERR_STATE;
-  }
-  if (deskew && b->h_cnt[2]) {
-    set_error(time_not_finite(fn));
-    return MADICP_ERR_STATE;
-  }
-  const int64_t kept = b->h_cnt[0];
-  if (kept == 0) {
-    set_error(std::string(fn) + ": no point inside the range gate");
-    return MADICP_ERR_INVALID;
-  }
-  BuildState* bs = nullptr;
-  int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
-  if (!rc) rc = ensure_state(c, size_t(plan->d.n), 0, &bs);
-  if (rc) return rc;
-  cudaStream_t st = c->stream;
-  bs->n_resident = 0;
-  bs->kept_check = 0;
-  bs->vc_check = false;
-  bs->time_check = false;
-  if (deskew) {
-    if (int e = stage_chunk_poses(plan->lane, st, T_prev, T_now, sensor_hz, kTimeChunks, bs->d_poses)) return e;
-    const TimeArgs T = time_args(plan->tm, nullptr, sensor_hz, b->d_tmax, nullptr, bs->d_poses, nullptr);
-    k_deskew_times<<<blocks(kept), kBlock, 0, st>>>(b->d_pts, b->d_tau, int(kept), T, bs->P[0]);
-    c->launches++;
-  } else {
-    CK(cudaMemcpyAsync(bs->P[0], b->d_pts, size_t(kept) * 24, cudaMemcpyDeviceToDevice, st));
-  }
-  if (int e = keep_plan(c, st, bs, plan, nullptr, kept)) return e;
-  CK(cudaEventRecord(b->free_ev, st));  // (the plan's buffers may be reused once this has run)
-  return ingest_done(bs, st, kept, n_kept, points_out);
-}
-
-// The ingest behind madicp_ingest, madicp_ingest_points[_ex|_t] and madicp_ingest_plan (descriptor, correction and time
-// field validated).  plan (nullable): the scan's records are already on their way up, with its deskew order
-// (madicp_plan_points).  tm: a time field; with a deskew the whole deskew is the compaction's pass 2 on the device.
-int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int deskew, const double T_prev[12],
-           const double T_now[12], double sensor_hz, int num_threads, madicp_plan* plan, int64_t* n_kept, double* points_out,
-           const char* fn, const madicp_times_t& tm = madicp_times_t{}) {
-  if (plan && plan->tm.type != kTimeNone)
-    return ingest_planned_time(c, plan, deskew, T_prev, T_now, sensor_hz, n_kept, points_out, fn);
-  if (plan && plan->dev) return ingest_planned_dev(c, plan, deskew, T_prev, T_now, sensor_hz, n_kept, points_out, fn);
-  const bool timed = deskew && tm.type != kTimeNone && !plan;
-  CK(cudaSetDevice(c->device));
-  BuildState* bs = nullptr;
-  const int64_t n = d.n;
-  const size_t bytes = plan ? 0 : size_t(n) * size_t(d.stride);
-  int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
-  if (!rc) rc = ensure_state(c, size_t(n), bytes, &bs);
-  if (rc) return rc;
-  cudaStream_t st = c->stream;
-  bs->n_resident = 0;
-  bs->kept_check = 0;
-  bs->vc_check = vc.enabled != 0;
-  bs->time_check = false;
-  bs->idx_ok = false;
-  const bool keep = c->keep_cloud;
-  if (keep)
-    if (int e = ensure_idx(bs)) return e;
-  const char* raw = static_cast<const char*>(bs->d_raw);
-  if (plan) {  // the records, the permutation and the chunks went up on the plan lane's stream
-    CK(cudaStreamWaitEvent(st, plan->buf->ready, 0));
-    raw = plan->buf->d_raw;
-  } else {  // the raw scan goes up while the host works out the order (deskew) or the root's sums
-    CK(cudaMemcpyAsync(bs->d_raw, d.data, timed ? points_bytes(d, tm) : points_bytes(d), cudaMemcpyHostToDevice, st));
-  }
-  int slot = -1;
-  if (vc.enabled) CK(cudaMemsetAsync(bs->h_vc_err, 0, sizeof(int), st));
-  if (int e = vtab_room(bs, st, &vc, 1)) return e;
-  if (int e = vtab_slot(bs, st, vc, &slot)) return e;
   RecBatch B;
-  B.count = 1;
-  B.n_rec = int(n);
-  B.s[0] = rec_src(d, raw, 0, slot);
-  int64_t kept = n;
-  if (deskew && plan) {  // only the chunk poses are left
-    if (plan->rc == MADICP_ERR_STATE) set_error(vcorr_out_of_table(fn, vc.angle));
-    else if (plan->rc) set_error(plan->err);
-    if (plan->rc) return plan->rc;
-    kept = plan->kept;
-    if (kept > 0) {
-      if (int e = stage_chunk_poses(plan->lane, st, T_prev, T_now, sensor_hz, plan->n_chunks, bs->d_poses)) return e;
-      auto k = vc.enabled ? k_ingest<true> : k_ingest<false>;
-      k<<<blocks(kept), kBlock, 0, st>>>(B, plan->buf->d_perm, plan->buf->d_chunk, bs->d_poses, int(kept), bs->P[0],
-                                         bs->d_vtab, bs->h_vc_err);
-      c->launches++;
-      if (keep)  // (the plan's order holds record indices already)
-        CK(cudaMemcpyAsync(bs->d_idx, plan->buf->d_perm, size_t(kept) * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    }
-  } else if (timed) {  // no order, no host half: the chunk poses through the pinned ring, then passes 1 and 2
-    PlanLane* L = nullptr;
-    if (int e = plan_lane(c, &L)) return e;
-    if (int e = stage_chunk_poses(L, st, T_prev, T_now, sensor_hz, kTimeChunks, bs->d_poses)) return e;
-    const TimeArgs T = time_args(tm, raw, sensor_hz, bs->d_tmax, bs->h_t_err, bs->d_poses, nullptr);
-    if (int e = launch_compaction_time(c, bs, st, B, T, bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) return e;
-    if (keep)
-      if (int e = keep_records(c, st, bs, B, true, bs->d_idx)) return e;
-    kept = kept_count_host(d);  // (compared with the device's count at the build's first host sync, as the stamps are)
-    bs->kept_check = 1;
-    bs->time_check = true;
-  } else if (deskew) {
-    CK(cudaStreamSynchronize(st));  // h_perm / h_chunk / h_poses of the previous scan have been consumed
-    int n_poses = 0;
-    VcorrTable table;  // (the azimuths are those of the corrected points)
-    rc = madicp_deskew_plan(d, vcorr_table(vc, &table), T_prev, T_now, sensor_hz, num_threads, bs->h_perm, bs->h_chunk, bs->h_poses, &n_poses,
-                            &kept);
-    if (rc == MADICP_ERR_STATE) set_error(vcorr_out_of_table(fn, vc.angle));
-    if (rc) return rc;
-    if (kept > 0) {
-      CK(cudaMemcpyAsync(bs->d_perm, bs->h_perm, size_t(kept) * sizeof(int), cudaMemcpyHostToDevice, st));
-      CK(cudaMemcpyAsync(bs->d_chunk, bs->h_chunk, size_t(kept) * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
-      CK(cudaMemcpyAsync(bs->d_poses, bs->h_poses, size_t(n_poses) * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
-      auto k = vc.enabled ? k_ingest<true> : k_ingest<false>;
-      k<<<blocks(kept), kBlock, 0, st>>>(B, bs->d_perm, bs->d_chunk, bs->d_poses, int(kept), bs->P[0], bs->d_vtab,
-                                         bs->h_vc_err);
-      c->launches++;
-      if (keep)  // (the order holds record indices already)
-        CK(cudaMemcpyAsync(bs->d_idx, bs->d_perm, size_t(kept) * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    }
-  } else if (points_gated(d)) {
-    if (int e = launch_compaction(c, bs, st, B, bs->P[0], bs->h_kept, bs->h_vc_err, vc.enabled)) return e;
-    if (keep)
-      if (int e = keep_records(c, st, bs, B, true, bs->d_idx)) return e;
-    kept = root_host(d, vc, bs->root_S);
-    bs->kept_check = 1;
-  } else {
-    auto k = vc.enabled ? k_ingest<true> : k_ingest<false>;
-    k<<<blocks(n), kBlock, 0, st>>>(B, nullptr, nullptr, bs->d_poses, int(n), bs->P[0], bs->d_vtab, bs->h_vc_err);
-    c->launches++;
-    if (keep)
-      if (int e = keep_records(c, st, bs, B, false, bs->d_idx)) return e;
-    kept = root_host(d, vc, bs->root_S);
+  if (int e = one_scan(bs, st, d, p->vc, base, &B)) return e;
+  b->h_cnt[0] = b->h_cnt[1] = b->h_cnt[2] = 0;  // (the buffer's last consumer has read them)
+  if (timed) {
+    const TimeArgs T = time_args(p->tm, base, 0.0, b->d_tmax, b->h_cnt + 2, nullptr, b->d_tau);
+    if (int e = launch_compaction_time(c, bs, st, B, T, b->d_pts, b->h_cnt, b->h_cnt + 1, p->vc.enabled)) return e;
+  } else if (int e = launch_compaction(c, bs, st, B, reinterpret_cast<double*>(b->d_raw), b->h_cnt, b->h_cnt + 1,
+                                       p->vc.enabled)) {
+    return e;
   }
-  bs->idx_ok = keep;
-  CK(cudaGetLastError());
-  if (plan) CK(cudaEventRecord(plan->buf->free_ev, st));  // (the plan's buffers may be reused once this has run)
-  if (kept == 0) {
-    bs->kept_check = 0;
-    set_error(std::string(fn) + ": no point inside the range gate");
+  if (p->keep) {  // (madicp_set_keep_cloud: the records of the kept ranks)
+    if (!b->d_rec) CK(cudaMalloc(&b->d_rec, b->cap * sizeof(int)));
+    if (int e = keep_records(c, st, bs, B, true, b->d_rec)) return e;
+  }
+  CK(cudaEventRecord(b->compacted, st));
+  return MADICP_OK;
+}
+
+// The one plan builder behind madicp_plan_points[_t|_dev|_dev_t] (arguments validated; dev: the context's stream already
+// waits for the records' producer): the lane, the buffer and the plan, its hand-over, then its order half on a lane
+// thread (at most num_threads at a time) unless a time field leaves none.  A failed hand-over returns once nothing
+// reads the records or writes the buffer any more.
+int make_plan(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, const madicp_times_t& tm, bool dev,
+              int num_threads, madicp_plan_t** out) {
+  CK(cudaSetDevice(c->device));
+  const bool timed = tm.type != kTimeNone;
+  PlanLane* L = nullptr;
+  if (int e = plan_lane(c, &L)) return e;
+  PlanBuf* b = nullptr;
+  if (int e = plan_buf(L, size_t(d.n), dev ? (timed ? 0 : size_t(d.n) * 24) : points_bytes(d, tm), &b)) return e;
+  std::unique_ptr<madicp_plan> p(new madicp_plan);
+  p->ctx = c;
+  p->lane = L;
+  p->d = d;
+  p->vc = vc;
+  p->tm = tm;
+  p->dev = dev;
+  p->keep = c->keep_cloud;
+  p->buf = b;
+  p->done = p->done_p.get_future();
+  if (int e = hand_over(c, p.get())) {
+    cudaStreamSynchronize(c->stream);
+    cudaStreamSynchronize(L->stream);
+    return_buf(L, b);
+    return e;
+  }
+  if (timed) {
+    p->done_p.set_value();
+  } else {
+    madicp_plan* q = p.get();
+    L->submit(std::max(1, std::min(num_threads, 64)), [q]() { plan_order(q); });
+  }
+  *out = p.release();
+  return MADICP_OK;
+}
+
+// The checks every ingest and plan entry point makes first, in this order: the context and args_ok (the deskew's poses
+// and rate, or the plan's output), the descriptor, the correction and the time field.  MADICP_OK or MADICP_ERR_INVALID,
+// with a message naming fn.
+int check_scan(madicp_ctx* c, bool args_ok, const madicp_points_t* d, const madicp_vcorr_t* vc, const madicp_times_t* tm,
+               const char* fn) {
+  if (!c || !args_ok) {
+    set_error(std::string(fn) + ": bad arguments");
     return MADICP_ERR_INVALID;
   }
-  bs->n_resident = kept;
-  bs->has_root_S = !deskew && !vc.enabled;  // (a deskewed or corrected cloud exists on the device only: its root sums run
-                                            // there)
-  if (n_kept) *n_kept = kept;
-  if (points_out) {
-    CK(cudaMemcpyAsync(points_out, bs->P[0], size_t(kept) * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (bs->vc_check && *bs->h_vc_err) {
-      set_error(vcorr_out_of_table(fn, vc.angle));
-      bs->n_resident = 0;
-      return MADICP_ERR_STATE;
-    }
-    if (bs->time_check && *bs->h_t_err) {
-      set_error(time_not_finite(fn));
-      bs->n_resident = 0;
-      return MADICP_ERR_STATE;
-    }
-    if (bs->kept_check && bs->h_kept[0] != kept) {
-      set_error(std::string(fn) + ": the device kept " + std::to_string(bs->h_kept[0]) + " points, the host " +
-                std::to_string(kept));
-      bs->n_resident = 0;
-      return MADICP_ERR_STATE;
-    }
-  }
-  return MADICP_OK;
+  if (int e = check_points(d, fn)) return e;
+  if (int e = check_vcorr(vc, fn)) return e;
+  return check_times(tm, d, fn);
+}
+// Device records: device memory of the context's device, and the context's stream waits for their producer
+int enter_device(madicp_ctx* c, const madicp_points_t& d, void* producer, const char* fn) {
+  CK(cudaSetDevice(c->device));
+  if (int e = madicp_check_device_ptr(c, d.data, d.is_f32 ? 4 : 8, fn)) return e;
+  return madicp_stream_wait(c, c->stream, producer);
+}
+
+// madicp_ingest_points[_ex|_t|_dev|_dev_t]: device records are read once the context's stream waits for `producer`,
+// and the call returns once nothing reads them, whatever the outcome
+int ingest_points(madicp_ctx* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, const madicp_times_t* times,
+                  bool dev, void* producer, const Deskew& k, int64_t* n_kept, double* points_out, const char* fn) {
+  if (int e = check_scan(c, k.ok(), desc, vcorr, times, fn)) return e;
+  MADICP_TRY
+  if (dev)
+    if (int e = enter_device(c, *desc, producer, fn)) return e;
+  const int rc = ingest(c, *desc, vcorr_of(vcorr), times_of(times), dev, nullptr, k, n_kept, points_out, fn);
+  if (dev) CK(cudaStreamSynchronize(c->stream));
+  return rc;
+  MADICP_CATCH(fn)
+}
+
+// madicp_plan_points[_t|_dev|_dev_t]
+int plan_points(madicp_ctx* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, const madicp_times_t* times,
+                bool dev, void* producer, int num_threads, madicp_plan_t** out, const char* fn) {
+  if (out) *out = nullptr;
+  if (int e = check_scan(c, out != nullptr, desc, vcorr, times, fn)) return e;
+  MADICP_TRY
+  if (dev)
+    if (int e = enter_device(c, *desc, producer, fn)) return e;
+  return make_plan(c, *desc, vcorr_of(vcorr), times_of(times), dev, num_threads, out);
+  MADICP_CATCH(fn)
 }
 
 }  // namespace
@@ -1710,17 +1754,12 @@ int madtree_gpu_build(madicp_ctx_t* c, const double* points_xyz, int64_t n, doub
   MADICP_TRY
   CK(cudaSetDevice(c->device));
   BuildState* bs = nullptr;
-  int rc = drop_staged(static_cast<BuildState*>(c->build_state), c->stream);
-  if (!rc) rc = ensure_state(c, size_t(n), 0, &bs);
-  if (rc) return rc;
+  if (int e = begin_ingest(c, size_t(n), 0, &bs)) return e;
   CK(cudaMemcpyAsync(bs->P[0], points_xyz, size_t(n) * 3 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  bs->n_resident = n;
-  bs->kept_check = 0;
   root_sums_host(packed_points(points_xyz, n, 0), bs->root_S);
-  bs->vc_check = false;
-  bs->time_check = false;
-  bs->has_root_S = true;
-  bs->idx_ok = c->keep_cloud;
+  bs->res.n = n;
+  bs->res.has_root_S = true;
+  bs->res.idx_ok = c->keep_cloud;
   if (c->keep_cloud) {
     const int first[2] = {0, int(n)};
     if (int e = ensure_idx(bs)) return e;
@@ -1734,13 +1773,13 @@ int madtree_gpu_build_resident(madicp_ctx_t* c, double b_max, double b_min, madt
   if (!c || !out) return MADICP_ERR_INVALID;
   MADICP_TRY
   BuildState* bs = static_cast<BuildState*>(c->build_state);
-  if (!bs || bs->n_resident <= 0) {
+  if (!bs || bs->res.n <= 0) {
     set_error("madtree_gpu_build_resident: no cloud on the device (call madicp_ingest first)");
     return MADICP_ERR_STATE;
   }
   CK(cudaSetDevice(c->device));
   if (int e = drop_staged(bs, c->stream)) return e;
-  return build_resident(c, bs, c->stream, bs->n_resident, b_max, b_min, bs->has_root_S ? bs->root_S : nullptr, out);
+  return build_resident(c, bs, c->stream, bs->res.n, b_max, b_min, bs->res.has_root_S ? bs->root_S : nullptr, out);
   MADICP_CATCH("madtree_gpu_build_resident")
 }
 
@@ -1770,29 +1809,22 @@ int madtree_gpu_export(const madtree_gpu_t* t, double* mean, double* eigenvector
 
 int madicp_ingest(madicp_ctx_t* c, const void* xyz, int64_t n, int is_f32, int deskew, const double T_prev[12],
                   const double T_now[12], double sensor_hz, int num_threads, double* points_out) {
-  if (!c || !xyz || n <= 0 || n > (int64_t(1) << 24) || (deskew && (!T_prev || !T_now || !(sensor_hz > 0.0)))) {
+  const Deskew k{deskew, T_prev, T_now, sensor_hz, num_threads};
+  if (!c || !xyz || n <= 0 || n > (int64_t(1) << 24) || !k.ok()) {
     set_error("madicp_ingest: bad arguments (1 <= n <= 2^24 points)");
     return MADICP_ERR_INVALID;
   }
   MADICP_TRY
-  return ingest(c, packed_points(xyz, n, is_f32), madicp_vcorr_t{}, deskew, T_prev, T_now, sensor_hz, num_threads, nullptr,
-                nullptr, points_out, "madicp_ingest");
+  return ingest(c, packed_points(xyz, n, is_f32), madicp_vcorr_t{}, madicp_times_t{}, false, nullptr, k, nullptr, points_out,
+                "madicp_ingest");
   MADICP_CATCH("madicp_ingest")
 }
 
 int madicp_ingest_points_ex(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int deskew,
                             const double T_prev[12], const double T_now[12], double sensor_hz, int num_threads,
                             int64_t* n_kept, double* points_out) {
-  if (!c || (deskew && (!T_prev || !T_now || !(sensor_hz > 0.0)))) {
-    set_error("madicp_ingest_points: bad arguments");
-    return MADICP_ERR_INVALID;
-  }
-  if (int e = check_points(desc, "madicp_ingest_points")) return e;
-  if (int e = check_vcorr(vcorr, "madicp_ingest_points")) return e;
-  MADICP_TRY
-  return ingest(c, *desc, vcorr_of(vcorr), deskew, T_prev, T_now, sensor_hz, num_threads, nullptr, n_kept, points_out,
-                "madicp_ingest_points");
-  MADICP_CATCH("madicp_ingest_points")
+  return ingest_points(c, desc, vcorr, nullptr, false, nullptr, Deskew{deskew, T_prev, T_now, sensor_hz, num_threads},
+                       n_kept, points_out, "madicp_ingest_points");
 }
 
 int madicp_ingest_points(madicp_ctx_t* c, const madicp_points_t* desc, int deskew, const double T_prev[12],
@@ -1803,276 +1835,43 @@ int madicp_ingest_points(madicp_ctx_t* c, const madicp_points_t* desc, int deske
 int madicp_ingest_points_dev(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int deskew,
                              const double T_prev[12], const double T_now[12], double sensor_hz, int num_threads,
                              void* producer_stream, int64_t* n_kept, double* points_out) {
-  const char* fn = "madicp_ingest_points_dev";
-  if (!c || (deskew && (!T_prev || !T_now || !(sensor_hz > 0.0)))) {
-    set_error(std::string(fn) + ": bad arguments");
-    return MADICP_ERR_INVALID;
-  }
-  if (int e = check_points(desc, fn)) return e;
-  if (int e = check_vcorr(vcorr, fn)) return e;
-  MADICP_TRY
-  CK(cudaSetDevice(c->device));
-  if (int e = madicp_check_device_ptr(c, desc->data, desc->is_f32 ? 4 : 8, fn)) return e;
-  if (int e = madicp_stream_wait(c, c->stream, producer_stream)) return e;
-  const int rc = ingest_dev(c, *desc, vcorr_of(vcorr), deskew, T_prev, T_now, sensor_hz, num_threads, n_kept, points_out, fn);
-  CK(cudaStreamSynchronize(c->stream));  // returns once nothing reads the caller's records, whatever the outcome
-  return rc;
-  MADICP_CATCH(fn)
+  return ingest_points(c, desc, vcorr, nullptr, true, producer_stream, Deskew{deskew, T_prev, T_now, sensor_hz, num_threads},
+                       n_kept, points_out, "madicp_ingest_points_dev");
 }
 
 int madicp_ingest_points_t(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
                            const madicp_times_t* times, int deskew, const double T_prev[12], const double T_now[12],
                            double sensor_hz, int num_threads, int64_t* n_kept, double* points_out) {
-  const char* fn = "madicp_ingest_points_t";
-  if (!c || (deskew && (!T_prev || !T_now || !(sensor_hz > 0.0)))) {
-    set_error(std::string(fn) + ": bad arguments");
-    return MADICP_ERR_INVALID;
-  }
-  if (int e = check_points(desc, fn)) return e;
-  if (int e = check_vcorr(vcorr, fn)) return e;
-  if (int e = check_times(times, desc, fn)) return e;
-  MADICP_TRY
-  return ingest(c, *desc, vcorr_of(vcorr), deskew, T_prev, T_now, sensor_hz, num_threads, nullptr, n_kept, points_out, fn,
-                times_of(times));
-  MADICP_CATCH(fn)
+  return ingest_points(c, desc, vcorr, times, false, nullptr, Deskew{deskew, T_prev, T_now, sensor_hz, num_threads}, n_kept,
+                       points_out, "madicp_ingest_points_t");
 }
 
 int madicp_ingest_points_dev_t(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
                                const madicp_times_t* times, int deskew, const double T_prev[12], const double T_now[12],
                                double sensor_hz, int num_threads, void* producer_stream, int64_t* n_kept,
                                double* points_out) {
-  const char* fn = "madicp_ingest_points_dev_t";
-  if (!c || (deskew && (!T_prev || !T_now || !(sensor_hz > 0.0)))) {
-    set_error(std::string(fn) + ": bad arguments");
-    return MADICP_ERR_INVALID;
-  }
-  if (int e = check_points(desc, fn)) return e;
-  if (int e = check_vcorr(vcorr, fn)) return e;
-  if (int e = check_times(times, desc, fn)) return e;
-  MADICP_TRY
-  CK(cudaSetDevice(c->device));
-  if (int e = madicp_check_device_ptr(c, desc->data, desc->is_f32 ? 4 : 8, fn)) return e;
-  if (int e = madicp_stream_wait(c, c->stream, producer_stream)) return e;
-  const int rc = ingest_dev(c, *desc, vcorr_of(vcorr), deskew, T_prev, T_now, sensor_hz, num_threads, n_kept, points_out, fn,
-                            times_of(times));
-  CK(cudaStreamSynchronize(c->stream));  // returns once nothing reads the caller's records, whatever the outcome
-  return rc;
-  MADICP_CATCH(fn)
+  return ingest_points(c, desc, vcorr, times, true, producer_stream, Deskew{deskew, T_prev, T_now, sensor_hz, num_threads},
+                       n_kept, points_out, "madicp_ingest_points_dev_t");
 }
 
 int madicp_plan_points(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int num_threads,
                        madicp_plan_t** out) {
-  if (!c || !out) {
-    set_error("madicp_plan_points: bad arguments");
-    return MADICP_ERR_INVALID;
-  }
-  *out = nullptr;
-  if (int e = check_points(desc, "madicp_plan_points")) return e;
-  if (int e = check_vcorr(vcorr, "madicp_plan_points")) return e;
-  MADICP_TRY
-  CK(cudaSetDevice(c->device));
-  PlanLane* L = nullptr;
-  if (int e = plan_lane(c, &L)) return e;
-  PlanBuf* b = nullptr;
-  if (int e = plan_buf(L, size_t(desc->n), points_bytes(*desc), &b)) return e;
-  std::unique_ptr<madicp_plan> p(new madicp_plan);
-  p->ctx = c;
-  p->lane = L;
-  p->d = *desc;
-  p->vc = vcorr_of(vcorr);
-  p->buf = b;
-  p->done = p->done_p.get_future();
-  // the records go up now, once the last ingest that read this buffer has run
-  cudaError_t e = cudaStreamWaitEvent(L->stream, b->free_ev, 0);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(b->d_raw, desc->data, points_bytes(*desc), cudaMemcpyHostToDevice, L->stream);
-  if (e != cudaSuccess) {
-    return_buf(L, b);
-    set_error(std::string("madicp_plan_points: ") + cudaGetErrorString(e));
-    return MADICP_ERR_CUDA;
-  }
-  madicp_plan* q = p.get();
-  L->submit(std::max(1, std::min(num_threads, 64)), [q]() { plan_order(q); });
-  *out = p.release();
-  return MADICP_OK;
-  MADICP_CATCH("madicp_plan_points")
+  return plan_points(c, desc, vcorr, nullptr, false, nullptr, num_threads, out, "madicp_plan_points");
 }
-
-namespace {
-// The device half of madicp_plan_points_dev, on the context's stream (whose build lane holds the scan scratch the
-// compaction needs): the scan's kept points, gated and corrected, into the plan buffer b as packed float64; b->compacted
-// follows.
-// keep: the records of the kept ranks go to b->d_rec too (madicp_set_keep_cloud).
-int plan_compact_dev(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, void* producer, PlanBuf* b, bool keep) {
-  BuildState* bs = static_cast<BuildState*>(c->build_state);
-  if (bs && bs->cap < size_t(d.n))  // the lane is about to be re-allocated: early uploads are lost
-    if (int e = drop_staged(bs, c->stream)) return e;
-  if (int e = ensure_state(c, size_t(d.n), 0, &bs)) return e;
-  cudaStream_t st = c->stream;
-  if (int e = madicp_stream_wait(c, st, producer)) return e;
-  int slot = -1;
-  if (int e = vtab_room(bs, st, &vc, 1)) return e;
-  if (int e = vtab_slot(bs, st, vc, &slot)) return e;
-  b->h_cnt[0] = b->h_cnt[1] = 0;  // (the buffer's last order half has read them)
-  RecBatch B;
-  B.count = 1;
-  B.n_rec = int(d.n);
-  B.s[0] = rec_src(d, d.data, 0, slot);
-  if (int e = launch_compaction(c, bs, st, B, reinterpret_cast<double*>(b->d_raw), b->h_cnt, b->h_cnt + 1, vc.enabled)) return e;
-  if (keep) {
-    if (!b->d_rec) CK(cudaMalloc(&b->d_rec, b->cap * sizeof(int)));
-    if (int e = keep_records(c, st, bs, B, true, b->d_rec)) return e;
-  }
-  CK(cudaEventRecord(b->compacted, st));
-  return MADICP_OK;
-}
-}  // namespace
 
 int madicp_plan_points_dev(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, int num_threads,
                            void* producer_stream, madicp_plan_t** out) {
-  const char* fn = "madicp_plan_points_dev";
-  if (!c || !out) {
-    set_error(std::string(fn) + ": bad arguments");
-    return MADICP_ERR_INVALID;
-  }
-  *out = nullptr;
-  if (int e = check_points(desc, fn)) return e;
-  if (int e = check_vcorr(vcorr, fn)) return e;
-  MADICP_TRY
-  CK(cudaSetDevice(c->device));
-  if (int e = madicp_check_device_ptr(c, desc->data, desc->is_f32 ? 4 : 8, fn)) return e;
-  PlanLane* L = nullptr;
-  if (int e = plan_lane(c, &L)) return e;
-  PlanBuf* b = nullptr;
-  if (int e = plan_buf(L, size_t(desc->n), size_t(desc->n) * 24, &b)) return e;
-  std::unique_ptr<madicp_plan> p(new madicp_plan);
-  p->ctx = c;
-  p->lane = L;
-  p->d = *desc;
-  p->vc = vcorr_of(vcorr);
-  p->dev = true;
-  p->keep = c->keep_cloud;
-  p->buf = b;
-  p->done = p->done_p.get_future();
-  if (int e = plan_compact_dev(c, *desc, p->vc, producer_stream, b, p->keep)) {
-    cudaStreamSynchronize(c->stream);  // (nothing may still read the caller's records, nor write the buffer)
-    return_buf(L, b);
-    return e;
-  }
-  madicp_plan* q = p.get();
-  L->submit(std::max(1, std::min(num_threads, 64)), [q]() { plan_order(q); });
-  *out = p.release();
-  return MADICP_OK;
-  MADICP_CATCH(fn)
+  return plan_points(c, desc, vcorr, nullptr, true, producer_stream, num_threads, out, "madicp_plan_points_dev");
 }
-
-namespace {
-// The whole hand-over of a plan with a time field: host records go up on the lane's stream, then on the context's stream
-// (whose build lane holds the compaction's scratch) passes 1 and 2 write the kept points, corrected, and their stamps into
-// the plan's buffer; b->compacted follows.  No host thread: the plan is complete once its kernels have run.
-int plan_time(madicp_ctx* c, madicp_plan* p, void* producer) {
-  PlanBuf* b = p->buf;
-  const madicp_points_t& d = p->d;
-  if (!b->d_pts) {
-    CK(cudaMalloc(&b->d_pts, b->cap * 3 * sizeof(double)));
-    CK(cudaMalloc(&b->d_tau, b->cap * sizeof(double)));
-    CK(cudaMalloc(&b->d_tmax, sizeof(unsigned long long)));
-  }
-  BuildState* bs = static_cast<BuildState*>(c->build_state);
-  if (bs && bs->cap < size_t(d.n))  // the lane is about to be re-allocated: early uploads are lost
-    if (int e = drop_staged(bs, c->stream)) return e;
-  if (int e = ensure_state(c, size_t(d.n), 0, &bs)) return e;
-  cudaStream_t st = c->stream;
-  const void* base = d.data;
-  if (p->dev) {
-    if (int e = madicp_stream_wait(c, st, producer)) return e;
-  } else {  // (once the last ingest that read this buffer has run)
-    CK(cudaStreamWaitEvent(p->lane->stream, b->free_ev, 0));
-    CK(cudaMemcpyAsync(b->d_raw, d.data, points_bytes(d, p->tm), cudaMemcpyHostToDevice, p->lane->stream));
-    CK(cudaEventRecord(b->ready, p->lane->stream));
-    CK(cudaStreamWaitEvent(st, b->ready, 0));
-    base = b->d_raw;
-  }
-  int slot = -1;
-  if (int e = vtab_room(bs, st, &p->vc, 1)) return e;
-  if (int e = vtab_slot(bs, st, p->vc, &slot)) return e;
-  b->h_cnt[0] = b->h_cnt[1] = b->h_cnt[2] = 0;  // (the buffer's last consumer has read them)
-  RecBatch B;
-  B.count = 1;
-  B.n_rec = int(d.n);
-  B.s[0] = rec_src(d, base, 0, slot);
-  const TimeArgs T = time_args(p->tm, base, 0.0, b->d_tmax, b->h_cnt + 2, nullptr, b->d_tau);
-  if (int e = launch_compaction_time(c, bs, st, B, T, b->d_pts, b->h_cnt, b->h_cnt + 1, p->vc.enabled)) return e;
-  if (p->keep) {  // (madicp_set_keep_cloud: the records of the kept ranks)
-    if (!b->d_rec) CK(cudaMalloc(&b->d_rec, b->cap * sizeof(int)));
-    if (int e = keep_records(c, st, bs, B, true, b->d_rec)) return e;
-  }
-  CK(cudaEventRecord(b->compacted, st));
-  return MADICP_OK;
-}
-// madicp_plan_points_t / _dev_t with a time field (validated)
-int plan_points_time(madicp_ctx* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr, const madicp_times_t* times,
-                     bool dev, void* producer_stream, madicp_plan_t** out, const char* fn) {
-  CK(cudaSetDevice(c->device));
-  if (dev)
-    if (int e = madicp_check_device_ptr(c, desc->data, desc->is_f32 ? 4 : 8, fn)) return e;
-  PlanLane* L = nullptr;
-  if (int e = plan_lane(c, &L)) return e;
-  PlanBuf* b = nullptr;
-  if (int e = plan_buf(L, size_t(desc->n), dev ? 0 : points_bytes(*desc, times_of(times)), &b)) return e;
-  std::unique_ptr<madicp_plan> p(new madicp_plan);
-  p->ctx = c;
-  p->lane = L;
-  p->d = *desc;
-  p->vc = vcorr_of(vcorr);
-  p->tm = times_of(times);
-  p->dev = dev;
-  p->keep = c->keep_cloud;
-  p->buf = b;
-  p->done = p->done_p.get_future();
-  if (int e = plan_time(c, p.get(), producer_stream)) {
-    cudaStreamSynchronize(c->stream);  // (nothing may still read the records, nor write the buffer)
-    cudaStreamSynchronize(L->stream);
-    return_buf(L, b);
-    return e;
-  }
-  p->done_p.set_value();
-  *out = p.release();
-  return MADICP_OK;
-}
-}  // namespace
 
 int madicp_plan_points_t(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
                          const madicp_times_t* times, int num_threads, madicp_plan_t** out) {
-  const char* fn = "madicp_plan_points_t";
-  if (!c || !out) {
-    set_error(std::string(fn) + ": bad arguments");
-    return MADICP_ERR_INVALID;
-  }
-  *out = nullptr;
-  if (int e = check_points(desc, fn)) return e;
-  if (int e = check_vcorr(vcorr, fn)) return e;
-  if (int e = check_times(times, desc, fn)) return e;
-  if (!times || times->type == kTimeNone) return madicp_plan_points(c, desc, vcorr, num_threads, out);
-  MADICP_TRY
-  return plan_points_time(c, desc, vcorr, times, false, nullptr, out, fn);
-  MADICP_CATCH(fn)
+  return plan_points(c, desc, vcorr, times, false, nullptr, num_threads, out, "madicp_plan_points_t");
 }
 
 int madicp_plan_points_dev_t(madicp_ctx_t* c, const madicp_points_t* desc, const madicp_vcorr_t* vcorr,
                              const madicp_times_t* times, int num_threads, void* producer_stream, madicp_plan_t** out) {
-  const char* fn = "madicp_plan_points_dev_t";
-  if (!c || !out) {
-    set_error(std::string(fn) + ": bad arguments");
-    return MADICP_ERR_INVALID;
-  }
-  *out = nullptr;
-  if (int e = check_points(desc, fn)) return e;
-  if (int e = check_vcorr(vcorr, fn)) return e;
-  if (int e = check_times(times, desc, fn)) return e;
-  if (!times || times->type == kTimeNone) return madicp_plan_points_dev(c, desc, vcorr, num_threads, producer_stream, out);
-  MADICP_TRY
-  return plan_points_time(c, desc, vcorr, times, true, producer_stream, out, fn);
-  MADICP_CATCH(fn)
+  return plan_points(c, desc, vcorr, times, true, producer_stream, num_threads, out, "madicp_plan_points_dev_t");
 }
 
 int madicp_ingest_plan(madicp_ctx_t* c, madicp_plan_t* plan, int deskew, const double T_prev[12], const double T_now[12],
@@ -2081,8 +1880,9 @@ int madicp_ingest_plan(madicp_ctx_t* c, madicp_plan_t* plan, int deskew, const d
     set_error("madicp_ingest_plan: null plan");
     return MADICP_ERR_INVALID;
   }
+  const Deskew k{deskew, T_prev, T_now, sensor_hz, 0};
   int rc = MADICP_OK;
-  if (!c || c != plan->ctx || (deskew && (!T_prev || !T_now || !(sensor_hz > 0.0)))) {
+  if (!c || c != plan->ctx || !k.ok()) {
     set_error("madicp_ingest_plan: bad arguments (the plan's context, and the poses and rate when deskewing)");
     rc = MADICP_ERR_INVALID;
   }
@@ -2092,8 +1892,7 @@ int madicp_ingest_plan(madicp_ctx_t* c, madicp_plan_t* plan, int deskew, const d
       set_error(plan->err);
       rc = plan->rc;
     }
-    if (!rc)
-      rc = ingest(c, plan->d, plan->vc, deskew, T_prev, T_now, sensor_hz, 0, plan, n_kept, points_out, "madicp_ingest_plan");
+    if (!rc) rc = ingest(c, plan->d, plan->vc, plan->tm, plan->dev, plan, k, n_kept, points_out, "madicp_ingest_plan");
   } catch (const std::bad_alloc&) {
     set_error("madicp_ingest_plan: out of host memory");
     rc = MADICP_ERR_NOMEM;

@@ -304,9 +304,9 @@ class Registrar:
     def ingest_records(self, records, min_range=0.0, max_range=math.inf, inclusive=True, drop_nan=False, deskew=False,
                        T_prev=None, T_now=None, sensor_hz=10.0, num_threads=1, want_points=False, apply_correction=False,
                        vertical_angle_offset=VERTICAL_ANGLE_OFFSET, time_field=None, time_scale=1.0, time_end=None):
-        """Records -> device-resident float64 cloud of the kept points (madicp_ingest_points_ex; a device array is read
-        in place, madicp_ingest_points_dev).  time_field (records.time_layout): a deskew takes each point's chunk from
-        its own stamp (madicp_ingest_points_t), time_scale seconds per unit, time_end the sweep's end (default: the
+        """Records -> device-resident float64 cloud of the kept points (madicp_ingest_points_t; a device array is read
+        in place, madicp_ingest_points_dev_t).  time_field (records.time_layout): a deskew takes each point's chunk from
+        its own stamp, time_scale seconds per unit, time_end the sweep's end (default: the
         largest kept stamp).  Returns the kept points (want_points) or their number."""
         d = describe(records, min_range, max_range, inclusive, drop_nan)
         v = vcorr(apply_correction, vertical_angle_offset)
@@ -315,23 +315,15 @@ class Registrar:
         kept = C.c_int64(0)
         Tp = as_d(pose12(T_prev)) if T_prev is not None else None
         Tn = as_d(pose12(T_now)) if T_now is not None else None
-        if t is not None:
-            if d.on_device:
-                check(capi.lib().madicp_ingest_points_dev_t(self._h, C.byref(d), C.byref(v) if v else None, C.byref(t),
-                                                            int(deskew), Tp, Tn, sensor_hz, num_threads, d.stream,
-                                                            C.byref(kept), as_d(out)), "madicp_ingest_points_dev_t")
-            else:
-                check(capi.lib().madicp_ingest_points_t(self._h, C.byref(d), C.byref(v) if v else None, C.byref(t),
-                                                        int(deskew), Tp, Tn, sensor_hz, num_threads, C.byref(kept),
-                                                        as_d(out)), "madicp_ingest_points_t")
-        elif d.on_device:  # read in place on the device, after the producer's stream (records.describe)
-            check(capi.lib().madicp_ingest_points_dev(self._h, C.byref(d), C.byref(v) if v else None, int(deskew), Tp, Tn,
-                                                      sensor_hz, num_threads, d.stream, C.byref(kept), as_d(out)),
-                  "madicp_ingest_points_dev")
+        t = C.byref(t) if t is not None else None
+        if d.on_device:  # read in place on the device, after the producer's stream (records.describe)
+            check(capi.lib().madicp_ingest_points_dev_t(self._h, C.byref(d), C.byref(v) if v else None, t, int(deskew), Tp,
+                                                        Tn, sensor_hz, num_threads, d.stream, C.byref(kept), as_d(out)),
+                  "madicp_ingest_points_dev_t")
         else:
-            check(capi.lib().madicp_ingest_points_ex(self._h, C.byref(d), C.byref(v) if v else None, int(deskew), Tp, Tn,
-                                                     sensor_hz, num_threads, C.byref(kept), as_d(out)),
-                  "madicp_ingest_points")
+            check(capi.lib().madicp_ingest_points_t(self._h, C.byref(d), C.byref(v) if v else None, t, int(deskew), Tp, Tn,
+                                                    sensor_hz, num_threads, C.byref(kept), as_d(out)),
+                  "madicp_ingest_points_t")
         return out[:kept.value].copy() if want_points else kept.value
 
     def stage_records(self, records, reserve_points=0, apply_correction=False, vertical_angle_offset=VERTICAL_ANGLE_OFFSET,
@@ -370,28 +362,22 @@ class Registrar:
     def plan_records(self, records, min_range=0.0, max_range=math.inf, inclusive=True, drop_nan=False, num_threads=1,
                      apply_correction=False, vertical_angle_offset=VERTICAL_ANGLE_OFFSET, time_field=None, time_scale=1.0,
                      time_end=None):
-        """Hands a future scan over for a deskewed look-ahead (madicp_plan_points): the records start going up at once
+        """Hands a future scan over for a deskewed look-ahead (madicp_plan_points_t): the records start going up at once
         and the pose-free half of the deskew runs on a host thread (at most num_threads at a time).  With a time_field
-        (as in ingest_records, madicp_plan_points_t) there is no host half: the gate, the correction and the compaction
+        (as in ingest_records) there is no host half: the gate, the correction and the compaction
         run on the device at once.  Returns a DeskewPlan for ingest_plan; the array is read in place and must stay
         unchanged until then."""
         d = describe(records, min_range, max_range, inclusive, drop_nan)
         v = vcorr(apply_correction, vertical_angle_offset)
         t = describe_times(records, time_field, time_scale, time_end)
         h = C.c_void_p()
-        if t is not None:
-            if d.on_device:
-                check(capi.lib().madicp_plan_points_dev_t(self._h, C.byref(d), C.byref(v) if v else None, C.byref(t),
-                                                          int(num_threads), d.stream, C.byref(h)), "madicp_plan_points_dev_t")
-            else:
-                check(capi.lib().madicp_plan_points_t(self._h, C.byref(d), C.byref(v) if v else None, C.byref(t),
-                                                      int(num_threads), C.byref(h)), "madicp_plan_points_t")
-        elif d.on_device:
-            check(capi.lib().madicp_plan_points_dev(self._h, C.byref(d), C.byref(v) if v else None, int(num_threads),
-                                                    d.stream, C.byref(h)), "madicp_plan_points_dev")
+        t = C.byref(t) if t is not None else None
+        if d.on_device:
+            check(capi.lib().madicp_plan_points_dev_t(self._h, C.byref(d), C.byref(v) if v else None, t, int(num_threads),
+                                                      d.stream, C.byref(h)), "madicp_plan_points_dev_t")
         else:
-            check(capi.lib().madicp_plan_points(self._h, C.byref(d), C.byref(v) if v else None, int(num_threads),
-                                                C.byref(h)), "madicp_plan_points")
+            check(capi.lib().madicp_plan_points_t(self._h, C.byref(d), C.byref(v) if v else None, t, int(num_threads),
+                                                  C.byref(h)), "madicp_plan_points_t")
         return DeskewPlan(h, self, records)
 
     def ingest_plan(self, plan, deskew=False, T_prev=None, T_now=None, sensor_hz=10.0, want_points=False):

@@ -94,31 +94,27 @@ static int ensure_pool(madicp_ctx* c, size_t need) {
     set_error("keyframe pool would exceed 2^30 nodes");
     return MADICP_ERR_NOMEM;
   }
-  madtree_rec_t* recs = nullptr;
-  int *child0 = nullptr, *rec_of = nullptr;
-  QuadRec* quad = nullptr;
-  double* ww = nullptr;
+  // the new pool is built aside: a failure leaves the old one in place
+  DevPtr<madtree_rec_t> recs;
+  DevPtr<int> child0, rec_of;
+  DevPtr<QuadRec> quad;
+  DevPtr<double> ww;
   const size_t total = cap * size_t(c->max_keyframes);
-  CK(cudaMalloc(&recs, total * sizeof(madtree_rec_t)));
-  CK(cudaMalloc(&child0, total * sizeof(int)));
-  CK(cudaMalloc(&rec_of, total * sizeof(int)));
-  CK(cudaMalloc(&quad, 2 * total * sizeof(QuadRec)));
-  CK(cudaMalloc(&ww, total * sizeof(double)));
+  CK(cudaMalloc(recs.put(), total * sizeof(madtree_rec_t)));
+  CK(cudaMalloc(child0.put(), total * sizeof(int)));
+  CK(cudaMalloc(rec_of.put(), total * sizeof(int)));
+  CK(cudaMalloc(quad.put(), 2 * total * sizeof(QuadRec)));
+  CK(cudaMalloc(ww.put(), total * sizeof(double)));
   for (int s = 0; s < c->max_keyframes; ++s)
     if (c->slots[s].n_nodes > 0)
       CK(cudaMemcpyAsync(recs + size_t(s) * cap, c->d_pool_recs + size_t(s) * c->pool_cap,
                          size_t(c->slots[s].n_nodes) * sizeof(madtree_rec_t), cudaMemcpyDeviceToDevice, c->stream));
   CK(cudaStreamSynchronize(c->stream));
-  cudaFree(c->d_pool_recs);
-  cudaFree(c->d_pool_child0);
-  cudaFree(c->d_pool_rec_of);
-  cudaFree(c->d_quad);
-  cudaFree(c->d_pool_ww);
-  c->d_pool_ww = ww;
-  c->d_pool_recs = recs;
-  c->d_pool_child0 = child0;
-  c->d_pool_rec_of = rec_of;
-  c->d_quad = quad;
+  c->d_pool_ww = std::move(ww);
+  c->d_pool_recs = std::move(recs);
+  c->d_pool_child0 = std::move(child0);
+  c->d_pool_rec_of = std::move(rec_of);
+  c->d_quad = std::move(quad);
   c->quad_cap = 2 * cap;
   c->pool_cap = cap;
   for (int s = 0; s < c->max_keyframes; ++s)
@@ -153,12 +149,9 @@ static int slot_rank(const madicp_ctx* c, int slot) {
 static int ensure_items(madicp_ctx* c, size_t items) {
   if (items <= c->cap_items) return MADICP_OK;
   CK(cudaStreamSynchronize(c->stream));
-  if (c->d_hit) cudaFree(c->d_hit);
-  if (c->d_ord) cudaFree(c->d_ord);
-  c->d_hit = c->d_ord = nullptr;
   c->cap_items = 0;
-  CK(cudaMalloc(&c->d_hit, items * sizeof(int)));
-  CK(cudaMalloc(&c->d_ord, items * sizeof(int)));
+  CK(cudaMalloc(c->d_hit.put(), items * sizeof(int)));
+  CK(cudaMalloc(c->d_ord.put(), items * sizeof(int)));
   c->cap_items = items;
   return MADICP_OK;
 }
@@ -241,6 +234,16 @@ static int grid_for(const madicp_ctx* c, int64_t items) {
   return int(g);
 }
 
+madicp_ctx::~madicp_ctx() {
+  cudaSetDevice(device);
+  if (stream) cudaStreamSynchronize(stream);  // (none before madicp_create made the context's own)
+  for (int r = 0; r < world; ++r)
+    if (world > 1 && r != rank && peer_comm[r]) cudaIpcCloseMemHandle(peer_comm[r]);
+  madicp_gpu_build_release(this);
+  for (madtree_gpu* t : tree_cache) delete t;  // (trees still held by the caller are the caller's to free first)
+  for (CloudBuf* b : cloud_cache) delete b;
+}
+
 extern "C" {
 
 const char* madicp_last_error(void) { return g_error.c_str(); }
@@ -267,7 +270,7 @@ int madicp_create(madicp_ctx_t** out, int device, int max_keyframes) {
     set_error("madicp_create: device is not sm_90 (H100); kernels are built for sm_90a only");
     return MADICP_ERR_CUDA;
   }
-  madicp_ctx* c = new madicp_ctx;
+  std::unique_ptr<madicp_ctx> c(new madicp_ctx);
   c->device = device;
   c->max_keyframes = max_keyframes;
   c->sm_count = prop.multiProcessorCount;
@@ -275,103 +278,45 @@ int madicp_create(madicp_ctx_t** out, int device, int max_keyframes) {
   {  // registration runs at the highest priority: the build lanes (lowest) fill the gaps
     int lo_pri = 0, hi_pri = 0;
     CK(cudaDeviceGetStreamPriorityRange(&lo_pri, &hi_pri));
-    CK(cudaStreamCreateWithPriority(&c->own_stream, cudaStreamNonBlocking, hi_pri));
+    CK(cudaStreamCreateWithPriority(c->own_stream.put(), cudaStreamNonBlocking, hi_pri));
   }
   c->stream = c->own_stream;
-  CK(cudaMalloc(&c->d_state, sizeof(GnState)));
+  CK(cudaMalloc(c->d_state.put(), sizeof(GnState)));
   CK(cudaMemset(c->d_state, 0, sizeof(GnState)));
-  CK(cudaMalloc(&c->d_X, sizeof(double) * 64));
-  CK(cudaMalloc(&c->d_comm, sizeof(CommBlock)));
+  CK(cudaMalloc(c->d_X.put(), sizeof(double) * 64));
+  CK(cudaMalloc(c->d_comm.put(), sizeof(CommBlock)));
   CK(cudaMemset(c->d_comm, 0, sizeof(CommBlock)));
-  CK(cudaEventCreateWithFlags(&c->tree_free_ev, cudaEventDisableTiming));
-  CK(cudaEventCreateWithFlags(&c->xstream_ev, cudaEventDisableTiming));
-  CK(cudaMalloc(&c->d_pool_lvl, size_t(max_keyframes) * (kMaxLevels + 1) * sizeof(int)));
-  CK(cudaMalloc(&c->d_xform, size_t(madicp_ctx::kXformRing) * 12 * sizeof(double)));
-  CK(cudaMallocHost(&c->h_xform, size_t(madicp_ctx::kXformRing) * 12 * sizeof(double)));
-  CK(cudaMallocHost(&c->h_lvl, size_t(madicp_ctx::kXformRing) * (kMaxLevels + 1) * sizeof(int)));
-  for (int i = 0; i < madicp_ctx::kXformRing; ++i) CK(cudaEventCreateWithFlags(&c->xform_done[i], cudaEventDisableTiming));
+  CK(cudaEventCreateWithFlags(c->tree_free_ev.put(), cudaEventDisableTiming));
+  CK(cudaEventCreateWithFlags(c->xstream_ev.put(), cudaEventDisableTiming));
+  CK(cudaMalloc(c->d_pool_lvl.put(), size_t(max_keyframes) * (kMaxLevels + 1) * sizeof(int)));
+  CK(cudaMalloc(c->d_xform.put(), size_t(madicp_ctx::kXformRing) * 12 * sizeof(double)));
+  CK(cudaMallocHost(c->h_xform.put(), size_t(madicp_ctx::kXformRing) * 12 * sizeof(double)));
+  CK(cudaMallocHost(c->h_lvl.put(), size_t(madicp_ctx::kXformRing) * (kMaxLevels + 1) * sizeof(int)));
+  for (Event& ev : c->xform_done) CK(cudaEventCreateWithFlags(ev.put(), cudaEventDisableTiming));
   c->cap_gather = kMaxSlots;  // (a whole model in one table: growing it synchronises)
-  CK(cudaMallocHost(&c->h_gather, size_t(madicp_ctx::kGatherRing) * c->cap_gather * sizeof(LeafGather)));
-  CK(cudaMalloc(&c->d_gather, size_t(madicp_ctx::kGatherRing) * c->cap_gather * sizeof(LeafGather)));
-  for (int i = 0; i < madicp_ctx::kGatherRing; ++i) CK(cudaEventCreateWithFlags(&c->gather_done[i], cudaEventDisableTiming));
-  CK(cudaMallocHost(&c->h_pinned, sizeof(double) * 64));
-  CK(cudaMallocHost(&c->h_state, sizeof(GnState)));
-  CK(cudaMallocHost(&c->h_matched, kMatchedCap));
+  CK(cudaMallocHost(c->h_gather.put(), size_t(madicp_ctx::kGatherRing) * c->cap_gather * sizeof(LeafGather)));
+  CK(cudaMalloc(c->d_gather.put(), size_t(madicp_ctx::kGatherRing) * c->cap_gather * sizeof(LeafGather)));
+  for (Event& ev : c->gather_done) CK(cudaEventCreateWithFlags(ev.put(), cudaEventDisableTiming));
+  CK(cudaMallocHost(c->h_pinned.put(), sizeof(double) * 64));
+  CK(cudaMallocHost(c->h_state.put(), sizeof(GnState)));
+  CK(cudaMallocHost(c->h_matched.put(), kMatchedCap));
   if (const char* e = getenv("MADICP_NO_MEMO")) c->memo_mode = (atoi(e) == 0) ? 2 : 0;
   int threads = 1024, ctas = 1;
   if (const char* e = getenv("MADICP_GN_SHAPE"))
     if (sscanf(e, "%d,%d", &threads, &ctas) == 2) c->gn_auto = false;
-  int rc = configure_gn(c, threads, ctas);
+  int rc = configure_gn(c.get(), threads, ctas);
   if (rc) return rc;
   c->cap_partial = size_t(c->sm_count) * 8 * kAcc;
-  CK(cudaMalloc(&c->d_partial, c->cap_partial * sizeof(double)));
-  CK(cudaMalloc(&c->d_tiles, c->cap_partial * sizeof(LLCell)));
+  CK(cudaMalloc(c->d_partial.put(), c->cap_partial * sizeof(double)));
+  CK(cudaMalloc(c->d_tiles.put(), c->cap_partial * sizeof(LLCell)));
   CK(cudaMemset(c->d_tiles, 0, c->cap_partial * sizeof(LLCell)));  // epoch 0 is never used
   c->peer_comm[0] = c->d_comm;
-  *out = c;
+  *out = c.release();
   return MADICP_OK;
   MADICP_CATCH("madicp_create")
 }
 
-void madicp_destroy(madicp_ctx_t* c) {
-  if (!c) return;
-  cudaSetDevice(c->device);
-  cudaStreamSynchronize(c->stream);
-  for (int r = 0; r < c->world; ++r)
-    if (c->world > 1 && r != c->rank && c->peer_comm[r]) cudaIpcCloseMemHandle(c->peer_comm[r]);
-  madicp_gpu_build_release(c);
-  for (madtree_gpu* t : c->tree_cache) delete t;  // (trees still held by the caller are the caller's to free first)
-  for (CloudBuf* b : c->cloud_cache) {
-    cudaFree(b->xyz);
-    cudaFree(b->idx);
-    delete b;
-  }
-  cudaFreeHost(c->h_cloud_xyz);
-  cudaFreeHost(c->h_cloud_idx);
-  for (void* slab : c->tree_slabs) cudaFree(slab);
-  cudaFree(c->d_pool_recs);
-  cudaFree(c->d_pool_child0);
-  cudaFree(c->d_pool_rec_of);
-  cudaFree(c->d_pool_lvl);
-  cudaFree(c->d_quad);
-  cudaFree(c->d_pool_ww);
-  cudaFree(c->d_xform);
-  cudaFree(c->d_dbg_cta);
-  cudaFree(c->d_moving);
-  cudaFree(c->d_mov4);
-  cudaFree(c->d_step_matched);
-  cudaFree(c->d_hit);
-  cudaFree(c->d_ord);
-  cudaFree(c->d_cloud_q);
-  cudaFree(c->d_cloud_o);
-  cudaFree(c->d_partial);
-  cudaFree(c->d_tiles);
-  cudaFree(c->d_memo_leaf);
-  cudaFree(c->d_memo_margin);
-  cudaFree(c->d_memo_ckpt);
-  cudaFree(c->d_memo_ckpt_up);
-  cudaFree(c->d_state);
-  cudaFree(c->d_X);
-  cudaFree(c->d_comm);
-  cudaFree(c->d_dbg);
-  cudaFreeHost(c->h_xform);
-  cudaFreeHost(c->h_lvl);
-  cudaFreeHost(c->h_pinned);
-  cudaFreeHost(c->h_state);
-  for (int i = 0; i < madicp_ctx::kXformRing; ++i)
-    if (c->xform_done[i]) cudaEventDestroy(c->xform_done[i]);
-  cudaFree(c->d_gather);
-  cudaFreeHost(c->h_gather);
-  for (int i = 0; i < madicp_ctx::kGatherRing; ++i)
-    if (c->gather_done[i]) cudaEventDestroy(c->gather_done[i]);
-  cudaFree(c->d_leaves);
-  cudaFreeHost(c->h_leaves);
-  cudaFreeHost(c->h_matched);
-  if (c->tree_free_ev) cudaEventDestroy(c->tree_free_ev);
-  if (c->xstream_ev) cudaEventDestroy(c->xstream_ev);
-  cudaStreamDestroy(c->own_stream);
-  delete c;
-}
+void madicp_destroy(madicp_ctx_t* c) { delete c; }
 
 int madicp_set_params(madicp_ctx_t* c, double min_ball, double rho_ker, double b_ratio) {
   if (!c || !(min_ball > 0) || rho_ker < 0) {
@@ -603,17 +548,18 @@ int madicp_tree_alloc(madicp_ctx* c, size_t cap_nodes, madtree_gpu** out) {
     while (cap < cap_nodes) cap <<= 1;
     const size_t one = ((cap * sizeof(madtree_rec_t) + size_t(kMaxLevels + 1) * sizeof(int) + cap * sizeof(int)) + 255) & ~size_t(255);
     const int per_slab = cap <= (size_t(1) << 17) ? 16 : 1;
-    void* slab = nullptr;
-    cudaError_t e = cudaMalloc(&slab, one * size_t(per_slab));
+    DevPtr<void> slab;
+    cudaError_t e = cudaMalloc(slab.put(), one * size_t(per_slab));
     if (e != cudaSuccess) {
       set_error(std::string("device tree allocation: ") + cudaGetErrorString(e));
       return MADICP_ERR_NOMEM;
     }
-    c->tree_slabs.push_back(slab);
+    char* base = static_cast<char*>(slab.get());
+    c->tree_slabs.push_back(std::move(slab));
     for (int k = 0; k < per_slab; ++k) {
       madtree_gpu* n = new madtree_gpu;
       n->ctx = c;
-      n->block = static_cast<char*>(slab) + size_t(k) * one;
+      n->block = base + size_t(k) * one;
       n->cap_nodes = cap;
       n->recs = static_cast<madtree_rec_t*>(n->block);
       n->lvl = reinterpret_cast<int*>(n->recs + cap);
@@ -644,17 +590,16 @@ int madicp_cloud_alloc(madicp_ctx* c, size_t n, std::shared_ptr<CloudBuf>* out) 
     }
   }
   if (!b) {
-    b = new CloudBuf;
-    b->cap = size_t(1) << 17;
-    while (b->cap < n) b->cap <<= 1;
-    cudaError_t e = cudaMalloc(&b->xyz, b->cap * 3 * sizeof(double));
-    if (e == cudaSuccess) e = cudaMalloc(&b->idx, b->cap * sizeof(int32_t));
+    std::unique_ptr<CloudBuf> nb(new CloudBuf);
+    nb->cap = size_t(1) << 17;
+    while (nb->cap < n) nb->cap <<= 1;
+    cudaError_t e = cudaMalloc(nb->xyz.put(), nb->cap * 3 * sizeof(double));
+    if (e == cudaSuccess) e = cudaMalloc(nb->idx.put(), nb->cap * sizeof(int32_t));
     if (e != cudaSuccess) {
-      cudaFree(b->xyz);
-      delete b;
       set_error(std::string("kept cloud allocation: ") + cudaGetErrorString(e));
       return MADICP_ERR_NOMEM;
     }
+    b = nb.release();
   }
   *out = std::shared_ptr<CloudBuf>(b, [c](CloudBuf* p) {
     std::lock_guard<std::mutex> lk(c->cloud_mu);
@@ -734,12 +679,9 @@ static int leaf_gather_launch(madicp_ctx* c, const madtree_gpu_t* const* trees, 
                               double* out) {
   if (size_t(count) > c->cap_gather) {
     for (int i = 0; i < madicp_ctx::kGatherRing; ++i) CK(cudaEventSynchronize(c->gather_done[i]));
-    cudaFreeHost(c->h_gather);
-    cudaFree(c->d_gather);
-    c->h_gather = c->d_gather = nullptr;
     c->cap_gather = 0;
-    CK(cudaMallocHost(&c->h_gather, size_t(madicp_ctx::kGatherRing) * size_t(count) * sizeof(LeafGather)));
-    CK(cudaMalloc(&c->d_gather, size_t(madicp_ctx::kGatherRing) * size_t(count) * sizeof(LeafGather)));
+    CK(cudaMallocHost(c->h_gather.put(), size_t(madicp_ctx::kGatherRing) * size_t(count) * sizeof(LeafGather)));
+    CK(cudaMalloc(c->d_gather.put(), size_t(madicp_ctx::kGatherRing) * size_t(count) * sizeof(LeafGather)));
     c->cap_gather = size_t(count);
   }
   const int r = int(c->gather_seq % madicp_ctx::kGatherRing);
@@ -834,13 +776,10 @@ int madtree_gpu_leaf_means(const madtree_gpu_t* const* trees, const double* cons
   MADICP_TRY
   CK(cudaSetDevice(c->device));
   if (size_t(total) > c->cap_leaves) {  // (only this call uses the buffers, and it returns with the stream idle)
-    cudaFree(c->d_leaves);
-    cudaFreeHost(c->h_leaves);
-    c->d_leaves = c->h_leaves = nullptr;
     c->cap_leaves = 0;
     const size_t cap = size_t(total) + size_t(total) / 4 + 1024;
-    CK(cudaMalloc(&c->d_leaves, cap * 3 * sizeof(double)));
-    CK(cudaMallocHost(&c->h_leaves, cap * 3 * sizeof(double)));
+    CK(cudaMalloc(c->d_leaves.put(), cap * 3 * sizeof(double)));
+    CK(cudaMallocHost(c->h_leaves.put(), cap * 3 * sizeof(double)));
     c->cap_leaves = cap;
   }
   if (int rc = leaf_gather_launch(c, trees, X, count, total, c->d_leaves)) return rc;
@@ -932,14 +871,10 @@ int64_t madtree_gpu_cloud(const madtree_gpu_t* t, const double X[12], double* xy
   MADICP_TRY
   CK(cudaSetDevice(c->device));
   if (size_t(n) > c->cap_cloud_out) {  // (only this call uses the staging, and it returns with the stream idle)
-    cudaFreeHost(c->h_cloud_xyz);
-    cudaFreeHost(c->h_cloud_idx);
-    c->h_cloud_xyz = nullptr;
-    c->h_cloud_idx = nullptr;
     c->cap_cloud_out = 0;
     const size_t cap = size_t(n) + size_t(n) / 4 + 1024;
-    CK(cudaHostAlloc(&c->h_cloud_xyz, cap * 3 * sizeof(double), cudaHostAllocMapped));
-    CK(cudaHostAlloc(&c->h_cloud_idx, cap * sizeof(int64_t), cudaHostAllocMapped));
+    CK(cudaHostAlloc(c->h_cloud_xyz.put(), cap * 3 * sizeof(double), cudaHostAllocMapped));
+    CK(cudaHostAlloc(c->h_cloud_idx.put(), cap * sizeof(int64_t), cudaHostAllocMapped));
     c->cap_cloud_out = cap;
   }
   double* dx = nullptr;
@@ -1009,17 +944,11 @@ int madicp_put_keyframe_tree(madicp_ctx_t* c, int slot, const madtree_gpu_t* t, 
 static int ensure_moving(madicp_ctx* c, int L) {
   if (size_t(L) <= c->cap_moving) return MADICP_OK;
   CK(cudaStreamSynchronize(c->stream));
-  if (c->d_moving) cudaFree(c->d_moving);
-  if (c->d_mov4) cudaFree(c->d_mov4);
-  if (c->d_step_matched) cudaFree(c->d_step_matched);
-  c->d_moving = nullptr;
-  c->d_mov4 = nullptr;
-  c->d_step_matched = nullptr;
   c->cap_moving = 0;
   const size_t cap = size_t(L) + size_t(L) / 4 + 1024;
-  CK(cudaMalloc(&c->d_moving, cap * 3 * sizeof(double)));
-  CK(cudaMalloc(&c->d_mov4, cap * sizeof(Moving4)));
-  CK(cudaMalloc(&c->d_step_matched, cap));
+  CK(cudaMalloc(c->d_moving.put(), cap * 3 * sizeof(double)));
+  CK(cudaMalloc(c->d_mov4.put(), cap * sizeof(Moving4)));
+  CK(cudaMalloc(c->d_step_matched.put(), cap));
   c->cap_moving = cap;
   return MADICP_OK;
 }
@@ -1095,7 +1024,7 @@ static int launch_search(madicp_ctx* c, const ModelView& mv, const double* d_X, 
   rc = prepare_moving(c);
   if (rc) return rc;
   k_search<<<grid_for(c, items), kStepBlock, 0, c->stream>>>(mv, c->d_mov4, c->L, d_X, c->d_hit,
-                                                            want_ord ? c->d_ord : nullptr);
+                                                            want_ord ? c->d_ord.get() : nullptr);
   c->launches++;
   CK(cudaGetLastError());
   return MADICP_OK;
@@ -1233,20 +1162,12 @@ static int register_enqueue(madicp_ctx* c, int iters, const double X0[12], int c
     const size_t need = stride * size_t(c->gn_grid);
     if (need > c->cap_memo) {
       CK(cudaStreamSynchronize(c->stream));
-      cudaFree(c->d_memo_leaf);
-      cudaFree(c->d_memo_margin);
-      cudaFree(c->d_memo_ckpt);
-      cudaFree(c->d_memo_ckpt_up);
-      c->d_memo_leaf = nullptr;
-      c->d_memo_margin = nullptr;
-      c->d_memo_ckpt = nullptr;
-      c->d_memo_ckpt_up = nullptr;
       c->cap_memo = 0;
       const size_t cap = need + need / 4;
-      CK(cudaMalloc(&c->d_memo_leaf, cap * sizeof(int)));
-      CK(cudaMalloc(&c->d_memo_margin, cap * sizeof(float)));
-      CK(cudaMalloc(&c->d_memo_ckpt, cap * sizeof(unsigned)));
-      CK(cudaMalloc(&c->d_memo_ckpt_up, cap * sizeof(float)));
+      CK(cudaMalloc(c->d_memo_leaf.put(), cap * sizeof(int)));
+      CK(cudaMalloc(c->d_memo_margin.put(), cap * sizeof(float)));
+      CK(cudaMalloc(c->d_memo_ckpt.put(), cap * sizeof(unsigned)));
+      CK(cudaMalloc(c->d_memo_ckpt_up.put(), cap * sizeof(float)));
       c->cap_memo = cap;
     }
     A.memo_leaf = c->d_memo_leaf;
@@ -1259,7 +1180,7 @@ static int register_enqueue(madicp_ctx* c, int iters, const double X0[12], int c
   }
   A.st = c->d_state;
   A.dbg = c->d_dbg;
-  A.dbg_cta = c->d_dbg ? c->d_dbg_cta : nullptr;
+  A.dbg_cta = c->d_dbg ? c->d_dbg_cta.get() : nullptr;
   c->epoch += uint32_t(iters);
   A.pose_epoch = c->pose_epoch;
   c->pose_epoch += uint32_t(iters);
@@ -1384,14 +1305,10 @@ int madicp_search_cloud(madicp_ctx_t* c, int slot, const double* q, int64_t n, i
   CK(cudaSetDevice(c->device));
   if (size_t(n) > c->cap_cloud) {  // scratch lives with the context and only grows
     CK(cudaStreamSynchronize(c->stream));
-    cudaFree(c->d_cloud_q);
-    cudaFree(c->d_cloud_o);
-    c->d_cloud_q = nullptr;
-    c->d_cloud_o = nullptr;
     c->cap_cloud = 0;
     const size_t cap = size_t(n) + size_t(n) / 4 + 1024;
-    CK(cudaMalloc(&c->d_cloud_q, cap * 10 * sizeof(double)));
-    CK(cudaMalloc(&c->d_cloud_o, cap * sizeof(int)));
+    CK(cudaMalloc(c->d_cloud_q.put(), cap * 10 * sizeof(double)));
+    CK(cudaMalloc(c->d_cloud_o.put(), cap * sizeof(int)));
     c->cap_cloud = cap;
   }
   double* d_q = c->d_cloud_q;
@@ -1491,34 +1408,37 @@ int madicp_calibrate(madicp_ctx_t* c, const double X0[12]) {
   if (rc) return rc;
   if (!X0 || c->world > 1) return MADICP_ERR_INVALID;
   CK(cudaSetDevice(c->device));
-  const bool was_auto = c->gn_auto;
   const int64_t items = int64_t(madicp_num_keyframes(c)) * c->L;
   const double per_sm = double((items + 31) / 32) / double(c->sm_count);
-  cudaEvent_t e0, e1;
-  CK(cudaEventCreate(&e0));
-  CK(cudaEventCreate(&e1));
-  c->gn_auto = false;
   int measured = 0;
-  for (int i = 0; i < madicp_ctx::kNumAutoShapes; ++i) {
-    if (configure_gn(c, madicp_ctx::kAutoShapes[i], 1)) continue;
-    const int rounds = 4;
-    for (int rep = 0; rep < 2; ++rep) {  // the second repetition is the timed one (warm L2, configured kernel)
-      CK(cudaEventRecord(e0, c->stream));
-      rc = register_enqueue(c, rounds, X0, rounds - 1);
+  {
+    struct KeepAuto {  // the shapes are measured with the automatic choice off; it comes back on every exit
+      madicp_ctx* c;
+      bool was;
+      ~KeepAuto() { c->gn_auto = was; }
+    } keep{c, c->gn_auto};
+    Event e0, e1;
+    CK(cudaEventCreate(e0.put()));
+    CK(cudaEventCreate(e1.put()));
+    c->gn_auto = false;
+    for (int i = 0; i < madicp_ctx::kNumAutoShapes; ++i) {
+      if (configure_gn(c, madicp_ctx::kAutoShapes[i], 1)) continue;
+      const int rounds = 4;
+      for (int rep = 0; rep < 2; ++rep) {  // the second repetition is the timed one (warm L2, configured kernel)
+        CK(cudaEventRecord(e0, c->stream));
+        rc = register_enqueue(c, rounds, X0, rounds - 1);
+        if (rc) break;
+        CK(cudaEventRecord(e1, c->stream));
+        CK(cudaEventSynchronize(e1));
+      }
       if (rc) break;
-      CK(cudaEventRecord(e1, c->stream));
-      CK(cudaEventSynchronize(e1));
+      float ms = 0;
+      CK(cudaEventElapsedTime(&ms, e0, e1));
+      const double passes = ceil(per_sm / double(madicp_ctx::kAutoShapes[i] / 32));
+      c->pass_cost[i] = double(ms) / double(rounds) / passes;  // any unit: only ratios matter
+      ++measured;
     }
-    if (rc) break;
-    float ms = 0;
-    CK(cudaEventElapsedTime(&ms, e0, e1));
-    const double passes = ceil(per_sm / double(madicp_ctx::kAutoShapes[i] / 32));
-    c->pass_cost[i] = double(ms) / double(rounds) / passes;  // any unit: only ratios matter
-    ++measured;
   }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  c->gn_auto = was_auto;
   if (rc) return rc;
   c->calibrated = true;
   if (c->gn_auto) {
@@ -1539,15 +1459,13 @@ int madicp_debug_timing(madicp_ctx_t* c, int enable, int64_t* out, int max_round
     CK(cudaMemcpy(out, c->d_dbg, size_t(rows) * 8 * sizeof(long long), cudaMemcpyDeviceToHost));
   }
   if (enable && !c->d_dbg) {
-    CK(cudaMalloc(&c->d_dbg, MADICP_MAX_ITERS * 8 * sizeof(long long)));
+    CK(cudaMalloc(c->d_dbg.put(), MADICP_MAX_ITERS * 8 * sizeof(long long)));
     CK(cudaMemset(c->d_dbg, 0, MADICP_MAX_ITERS * 8 * sizeof(long long)));
-    CK(cudaMalloc(&c->d_dbg_cta, size_t(MADICP_MAX_ITERS) * c->sm_count * 8 * 4 * sizeof(long long)));  // 4 planes, <= 8 CTAs/SM
+    CK(cudaMalloc(c->d_dbg_cta.put(), size_t(MADICP_MAX_ITERS) * c->sm_count * 8 * 4 * sizeof(long long)));  // 4 planes, <= 8 CTAs/SM
     CK(cudaMemset(c->d_dbg_cta, 0, size_t(MADICP_MAX_ITERS) * c->sm_count * 8 * 4 * sizeof(long long)));
   } else if (!enable && c->d_dbg) {
-    cudaFree(c->d_dbg);
-    cudaFree(c->d_dbg_cta);
-    c->d_dbg = nullptr;
-    c->d_dbg_cta = nullptr;
+    c->d_dbg.reset();
+    c->d_dbg_cta.reset();
   }
   return rows;
 }

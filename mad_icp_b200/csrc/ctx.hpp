@@ -12,6 +12,7 @@
 #include <string>
 #include <vector>
 
+#include "cuda_owned.hpp"
 #include "kernels.cuh"
 
 namespace madicp {
@@ -35,9 +36,9 @@ struct CommBlock {
 // every point.  One buffer per build (a forest's trees share it, each its own slice); back to the context's cache once
 // the last tree holding a slice lets it go.
 struct CloudBuf {
-  size_t cap = 0;           // points
-  double* xyz = nullptr;    // cap x 3
-  int32_t* idx = nullptr;   // cap
+  size_t cap = 0;       // points
+  DevPtr<double> xyz;   // cap x 3
+  DevPtr<int32_t> idx;  // cap
 };
 }  // namespace madicp
 
@@ -65,82 +66,86 @@ struct madtree_gpu {
 };
 
 struct madicp_ctx {
+  // waits for the stream and closes the peer mappings, then frees what the members do not own (the build and plan
+  // lanes, cached trees and kept clouds); the members free the rest
+  ~madicp_ctx();
   int device = 0;
   int max_keyframes = 0;
-  cudaStream_t own_stream = nullptr, stream = nullptr;
+  madicp::Stream own_stream;
+  cudaStream_t stream = nullptr;  // own_stream or the caller's (madicp_set_stream)
   int sm_count = 0;
   std::vector<madicp::Slot> slots;
   // keyframe pool: parallel arrays, pool_cap nodes per slot (kernels.cuh: ModelView)
   size_t pool_cap = 0;
-  madtree_rec_t* d_pool_recs = nullptr;
-  int* d_pool_child0 = nullptr;    // per node: first quad record of the grandchildren (even-depth internal nodes)
-  int* d_pool_rec_of = nullptr;    // per node: its quad record (even-depth nodes)
-  int* d_pool_lvl = nullptr;       // per slot: level table, kMaxLevels + 1 entries
-  size_t quad_cap = 0;             // 4-ary records per slot (= 2 * pool_cap)
-  madicp::QuadRec* d_quad = nullptr;
-  double* d_pool_ww = nullptr;     // per node: planarity weight of a leaf (what the quad leaf codes also carry)
+  madicp::DevPtr<madtree_rec_t> d_pool_recs;
+  madicp::DevPtr<int> d_pool_child0;  // per node: first quad record of the grandchildren (even-depth internal nodes)
+  madicp::DevPtr<int> d_pool_rec_of;  // per node: its quad record (even-depth nodes)
+  madicp::DevPtr<int> d_pool_lvl;     // per slot: level table, kMaxLevels + 1 entries
+  size_t quad_cap = 0;                // 4-ary records per slot (= 2 * pool_cap)
+  madicp::DevPtr<madicp::QuadRec> d_quad;
+  madicp::DevPtr<double> d_pool_ww;   // per node: planarity weight of a leaf (what the quad leaf codes also carry)
   // pinned staging rings for the small stream-ordered uploads of a promotion (pose, level table)
   static constexpr int kXformRing = 64;
-  double* d_xform = nullptr;
-  double* h_xform = nullptr;
-  int* h_lvl = nullptr;
-  cudaEvent_t xform_done[kXformRing] = {};
+  madicp::DevPtr<double> d_xform;
+  madicp::HostPtr<double> h_xform;
+  madicp::HostPtr<int> h_lvl;
+  madicp::Event xform_done[kXformRing];
   uint32_t xform_seq = 0;
   // leaf-mean gathers (madtree_gpu_leaf_means*): their tree tables go up through a pinned ring (kGatherRing tables of
   // cap_gather entries) into as many device tables, stream-ordered; the host form's means come back through h_leaves
   static constexpr int kGatherRing = 8;
-  madicp::LeafGather* h_gather = nullptr;
-  madicp::LeafGather* d_gather = nullptr;
+  madicp::HostPtr<madicp::LeafGather> h_gather;
+  madicp::DevPtr<madicp::LeafGather> d_gather;
   size_t cap_gather = 0;
-  cudaEvent_t gather_done[kGatherRing] = {};
+  madicp::Event gather_done[kGatherRing];
   uint32_t gather_seq = 0;
-  double* d_leaves = nullptr;  // host form: L x 3 on the device, then in pinned memory
-  double* h_leaves = nullptr;
+  madicp::DevPtr<double> d_leaves;  // host form: L x 3 on the device, then in pinned memory
+  madicp::HostPtr<double> h_leaves;
   size_t cap_leaves = 0;
-  std::vector<madtree_gpu*> tree_cache;  // freed device trees keep their memory for the next scan
-  std::vector<void*> tree_slabs;         // the allocations the trees are carved from
-  cudaEvent_t tree_free_ev = nullptr;    // recorded on the context's stream at every madtree_gpu_free
-  cudaEvent_t xstream_ev = nullptr;      // hand-overs with a caller's stream (madicp_stream_wait)
-  std::mutex tree_mu;                    // ... builders on other host threads allocate from it too
+  std::vector<madtree_gpu*> tree_cache;          // freed device trees keep their memory for the next scan
+  std::vector<madicp::DevPtr<void>> tree_slabs;  // the allocations the trees are carved from
+  madicp::Event tree_free_ev;                    // recorded on the context's stream at every madtree_gpu_free
+  madicp::Event xstream_ev;                      // hand-overs with a caller's stream (madicp_stream_wait)
+  std::mutex tree_mu;                            // ... builders on other host threads allocate from it too
   // kept clouds (madicp_set_keep_cloud): trees built from now on keep their input cloud; released buffers are cached
   bool keep_cloud = false;
   std::vector<madicp::CloudBuf*> cloud_cache;
   std::mutex cloud_mu;
-  int64_t* h_cloud_idx = nullptr;  // mapped staging of madtree_gpu_cloud (host form)
-  double* h_cloud_xyz = nullptr;
+  madicp::HostPtr<int64_t> h_cloud_idx;  // mapped staging of madtree_gpu_cloud (host form)
+  madicp::HostPtr<double> h_cloud_xyz;
   size_t cap_cloud_out = 0;
-  void* build_state = nullptr;           // gpu_tree.cu: working memory of the device build (lazily created)
-  void* plan_state = nullptr;            // gpu_tree.cu: buffers and threads of look-ahead plans (lazily created)
-  long long* d_dbg_cta = nullptr;  // MADICP_MAX_ITERS x grid item-phase cycles when debug timing is on
+  void* build_state = nullptr;  // gpu_tree.cu: working memory of the device build (lazily created)
+  void* plan_state = nullptr;   // gpu_tree.cu: buffers and threads of look-ahead plans (lazily created)
+  madicp::DevPtr<long long> d_dbg_cta;  // MADICP_MAX_ITERS x grid item-phase cycles when debug timing is on
   madicp::IcpParams P{0.2, 0.31622776601683794, 0.02};
-  double* d_moving = nullptr;               // raw L x 3 means as uploaded / gathered
-  madicp::Moving4* d_mov4 = nullptr;        // prepared (mean, gate radius) records the kernels read
-  bool mov4_stale = true;                   // params changed / new means since the last preparation
-  unsigned char* d_step_matched = nullptr;  // matched flags of the step API (madicp_linearize)
+  madicp::DevPtr<double> d_moving;               // raw L x 3 means as uploaded / gathered
+  madicp::DevPtr<madicp::Moving4> d_mov4;        // prepared (mean, gate radius) records the kernels read
+  bool mov4_stale = true;                        // params changed / new means since the last preparation
+  madicp::DevPtr<unsigned char> d_step_matched;  // matched flags of the step API (madicp_linearize)
   int L = 0;
   size_t cap_moving = 0;
   uint32_t call_seq = 0;  // registrations enqueued so far (selects the matched buffer)
-  int* d_hit = nullptr;
-  int* d_ord = nullptr;
+  madicp::DevPtr<int> d_hit;
+  madicp::DevPtr<int> d_ord;
   size_t cap_items = 0;
-  double* d_cloud_q = nullptr;  // madicp_search_cloud scratch: queries (3n) + outputs (7n), ordinals
-  int* d_cloud_o = nullptr;
+  madicp::DevPtr<double> d_cloud_q;  // madicp_search_cloud scratch: queries (3n) + outputs (7n), ordinals
+  madicp::DevPtr<int> d_cloud_o;
   size_t cap_cloud = 0;
-  double* d_partial = nullptr;      // per-CTA tiles of the step kernel (k_linearize)
-  madicp::LLCell* d_tiles = nullptr;  // per-CTA tiles of the persistent kernel, epoch-tagged (cap_partial cells)
+  madicp::DevPtr<double> d_partial;        // per-CTA tiles of the step kernel (k_linearize)
+  madicp::DevPtr<madicp::LLCell> d_tiles;  // per-CTA tiles of the persistent kernel, epoch-tagged (cap_partial cells)
   size_t cap_partial = 0;
-  int* d_memo_leaf = nullptr;      // path memo of the persistent kernel (GnArgs), grid x item_stride each
-  float* d_memo_margin = nullptr;
-  unsigned* d_memo_ckpt = nullptr;
-  float* d_memo_ckpt_up = nullptr;
+  madicp::DevPtr<int> d_memo_leaf;  // path memo of the persistent kernel (GnArgs), grid x item_stride each
+  madicp::DevPtr<float> d_memo_margin;
+  madicp::DevPtr<unsigned> d_memo_ckpt;
+  madicp::DevPtr<float> d_memo_ckpt_up;
   size_t cap_memo = 0;
   int memo_mode = 2;               // madicp_debug_set_memo; MADICP_NO_MEMO=1: 0 (walk every item from the root in every round)
-  madicp::GnState* d_state = nullptr;
-  double* d_X = nullptr;  // 12 (step API pose) + 36 + 6 scratch
-  madicp::CommBlock* d_comm = nullptr;
-  double* h_pinned = nullptr;       // 12 + 36 + 6 + ... staging
-  madicp::GnState* h_state = nullptr;  // pinned mirror (results)
-  unsigned char* h_matched = nullptr;
+  madicp::DevPtr<madicp::GnState> d_state;
+  madicp::DevPtr<double> d_X;  // 12 (step API pose) + 36 + 6 scratch
+  madicp::DevPtr<madicp::CommBlock> d_comm;
+  madicp::HostPtr<double> h_pinned;          // 12 + 36 + 6 + ... staging
+  madicp::HostPtr<madicp::GnState> h_state;  // pinned mirror (results)
+  madicp::HostPtr<unsigned char> h_matched;
   int gn_grid = 0;
   bool gn_auto = true;  // pick the shape per launch from the item count (pick_shape)
   int gn_threads = 1024;
@@ -154,7 +159,7 @@ struct madicp_ctx {
   double pass_cost[kNumAutoShapes] = {5570.0, 8260.0, 7480.0, 5650.0, 5325.0, 4650.0};
   bool calibrated = false;
   int last_iters = 0;
-  long long* d_dbg = nullptr;  // MADICP_MAX_ITERS x 8 clock stamps when debug timing is on
+  madicp::DevPtr<long long> d_dbg;  // MADICP_MAX_ITERS x 8 clock stamps when debug timing is on
   std::atomic<int64_t> launches{0};
   // peers
   int rank = 0, world = 1;

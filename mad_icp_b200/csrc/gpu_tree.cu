@@ -62,60 +62,67 @@ struct Resident {
 };
 
 struct BuildState {
+  // waits for what may still read the lane's memory: the background sums of staged scans and the copy stream
+  ~BuildState() {
+    for (const Staged& sg : staged) sg.root.wait();
+    if (copy_stream) cudaStreamSynchronize(copy_stream);
+  }
   size_t cap = 0;  // points
-  double* P[2] = {nullptr, nullptr};
-  int* owner[2] = {nullptr, nullptr};
-  unsigned char* flag = nullptr;
-  int *G = nullptr, *tile = nullptr, *XF = nullptr, *BP = nullptr;
+  DevPtr<double> P[2];
+  DevPtr<int> owner[2];
+  DevPtr<unsigned char> flag;
+  DevPtr<int> G, tile, XF, BP;
   // level-local
-  double* S = nullptr;
-  Eig3Mid* mid = nullptr;
-  long long* box = nullptr;
-  int *cnt = nullptr, *imin = nullptr, *child_of = nullptr, *dtile = nullptr;
-  double* dres = nullptr;
-  unsigned long long* dmin = nullptr;
-  // whole build
+  DevPtr<double> S;
+  DevPtr<Eig3Mid> mid;
+  DevPtr<long long> box;
+  DevPtr<int> cnt, imin, child_of, dtile;
+  DevPtr<double> dres;
+  DevPtr<unsigned long long> dmin;
+  // whole build: the node arrays (Nodes, by value in N)
+  DevPtr<int> n_lo, n_hi, n_parent, n_pp, n_anc, n_link, n_tree;
+  DevPtr<double> n_full;
   Nodes N{};
-  int* d_count = nullptr;  // nodes per level (kMaxLevels + 2)
-  Lvl* d_lvl = nullptr;    // level-loop state (gpu_tree_kernels.cuh)
+  DevPtr<int> d_count;  // nodes per level (kMaxLevels + 2)
+  DevPtr<Lvl> d_lvl;    // level-loop state (gpu_tree_kernels.cuh)
   // forest bookkeeping (a batch of scans is built as one forest): per tree and level
-  int* d_offs = nullptr;   // kMaxBatch + 1: first point of every tree
-  int* d_flvl = nullptr;   // forest level table (kMaxLevels + 2)
-  int *d_tcnt = nullptr, *d_tleaf = nullptr, *d_F = nullptr, *d_Loff = nullptr;
-  TreeOut* d_out = nullptr;
-  int *h_tcnt = nullptr, *h_tleaf = nullptr, *h_F = nullptr, *h_Loff = nullptr, *h_offs = nullptr;
-  TreeOut* h_out = nullptr;
+  DevPtr<int> d_offs;   // kMaxBatch + 1: first point of every tree
+  DevPtr<int> d_flvl;   // forest level table (kMaxLevels + 2)
+  DevPtr<int> d_tcnt, d_tleaf, d_F, d_Loff;
+  DevPtr<TreeOut> d_out;
+  HostPtr<int> h_tcnt, h_tleaf, h_F, h_Loff, h_offs;
+  HostPtr<TreeOut> h_out;
   Work W{};                // every pointer above, by value for the kernels
-  cudaGraphExec_t level_graph = nullptr;  // the fourteen kernels of one level
+  GraphExec level_graph;   // the fourteen kernels of one level
   // mapped pinned host memory
-  double *h_args = nullptr, *h_res = nullptr;
-  Ctl* h_ctl = nullptr;
-  int* h_lvl = nullptr;
+  HostPtr<double> h_args, h_res;
+  HostPtr<Ctl> h_ctl;
+  HostPtr<int> h_lvl;
   // ingest staging
-  void* d_raw = nullptr;  // the raw scans as uploaded (packed float32 or records), raw_cap bytes
+  DevPtr<char> d_raw;  // the raw scans as uploaded (packed float32 or records), raw_cap bytes
   size_t raw_cap = 0;
-  int* h_kept = nullptr;  // mapped: kept points of every scan, counted by the device's compaction (k_compact)
+  HostPtr<int> h_kept;  // mapped: kept points of every scan, counted by the device's compaction (k_compact)
   // vertical correction (vertical_correction.h): one table per distinct angle, kept while the lane lives.  The host
   // copy of slot k is written once, before its upload is queued, and never again until every upload has run.
-  VcorrTable* d_vtab = nullptr;
-  VcorrTable* h_vtab = nullptr;        // pinned
+  DevPtr<VcorrTable> d_vtab;
+  HostPtr<VcorrTable> h_vtab;          // pinned
   std::vector<double> vtab_angle;      // angle of slot k
-  int* h_vc_err = nullptr;             // mapped: a corrected point's rotation angle fell outside its table
+  HostPtr<int> h_vc_err;               // mapped: a corrected point's rotation angle fell outside its table
   // time-stamp deskew (time_deskew.h): the largest kept stamp's key, and a kept stamp that is NaN or infinite (mapped)
-  unsigned long long* d_tmax = nullptr;
-  int* h_t_err = nullptr;
-  int* d_perm = nullptr;
-  unsigned short* d_chunk = nullptr;
-  double* d_poses = nullptr;
-  int32_t* h_perm = nullptr;
-  uint16_t* h_chunk = nullptr;
-  double* h_poses = nullptr;
-  double* h_packed = nullptr;  // pinned, 3 x cap, at first use: a deskewed device scan's kept points for the host's order
+  DevPtr<unsigned long long> d_tmax;
+  HostPtr<int> h_t_err;
+  DevPtr<int> d_perm;
+  DevPtr<unsigned short> d_chunk;
+  DevPtr<double> d_poses;
+  HostPtr<int32_t> h_perm;
+  HostPtr<uint16_t> h_chunk;
+  HostPtr<double> h_poses;
+  HostPtr<double> h_packed;  // pinned, 3 x cap, at first use: a deskewed device scan's kept points for the host's order
   // kept clouds (madicp_set_keep_cloud), at first use: the record index of every point of the cloud in P[0] (valid when
   // res.idx_ok), and the records of a compaction's kept ranks before a deskew order is composed with them
-  int* d_idx = nullptr;
-  int* d_rec = nullptr;
-  double* h_root = nullptr;  // pinned: the root's sums when the host computes them
+  DevPtr<int> d_idx;
+  DevPtr<int> d_rec;
+  HostPtr<double> h_root;  // pinned: the root's sums when the host computes them
   double root_S[9];          // ... of the resident cloud (valid when res.has_root_S)
   Resident res;
   uint64_t seq = 0;        // builds so far (madtree_gpu_export is valid for the latest one only)
@@ -131,59 +138,32 @@ struct BuildState {
   int64_t staged_points = 0;  // records
   size_t staged_bytes = 0;    // end of the last staged scan in d_raw
   bool staged_raw = false, stage_closed = false;
-  cudaStream_t copy_stream = nullptr;
-  cudaEvent_t copy_ev = nullptr, idle_ev = nullptr;  // copies done / the working buffers are free again
-  std::vector<void*> dev_allocs, host_allocs;
+  Stream copy_stream;
+  Event copy_ev, idle_ev;  // copies done / the working buffers are free again
 };
 
 template <class T>
-int dev_alloc(BuildState* bs, T** p, size_t count) {
-  CK(cudaMalloc(p, count * sizeof(T)));
-  bs->dev_allocs.push_back(*p);
-  return MADICP_OK;
+cudaError_t dev_alloc(DevPtr<T>& p, size_t count) {
+  return cudaMalloc(p.put(), count * sizeof(T));
 }
 template <class T>
-int host_alloc(BuildState* bs, T** p, size_t count) {
-  CK(cudaHostAlloc(p, count * sizeof(T), cudaHostAllocMapped));
-  bs->host_allocs.push_back(*p);
-  return MADICP_OK;
-}
-
-void release(BuildState* bs) {
-  for (const BuildState::Staged& sg : bs->staged) sg.root.wait();  // (background sums still reading staged clouds)
-  bs->staged.clear();
-  if (bs->level_graph) cudaGraphExecDestroy(bs->level_graph);
-  bs->level_graph = nullptr;
-  if (bs->copy_stream) {
-    cudaStreamSynchronize(bs->copy_stream);
-    cudaStreamDestroy(bs->copy_stream);
-  }
-  if (bs->copy_ev) cudaEventDestroy(bs->copy_ev);
-  if (bs->idle_ev) cudaEventDestroy(bs->idle_ev);
-  bs->copy_stream = nullptr;
-  bs->copy_ev = bs->idle_ev = nullptr;
-  for (void* p : bs->dev_allocs) cudaFree(p);
-  for (void* p : bs->host_allocs) cudaFreeHost(p);
-  bs->dev_allocs.clear();
-  bs->host_allocs.clear();
+cudaError_t host_alloc(HostPtr<T>& p, size_t count) {  // mapped: the kernels read and write it in place
+  return cudaHostAlloc(p.put(), count * sizeof(T), cudaHostAllocMapped);
 }
 
 // `slot`: where the lane keeps its working memory (the context's own lane, or a builder's)
 // n: records (every per-point array is indexed by record before the compaction), raw_bytes: the raw buffer
 int ensure_state(void** slot, cudaStream_t stream, size_t n, size_t raw_bytes, BuildState** out) {
-  BuildState* bs = static_cast<BuildState*>(*slot);
-  if (bs && bs->cap >= n && bs->raw_cap >= raw_bytes) {
-    *out = bs;
+  BuildState* old = static_cast<BuildState*>(*slot);
+  if (old && old->cap >= n && old->raw_cap >= raw_bytes) {
+    *out = old;
     return MADICP_OK;
   }
   CK(cudaStreamSynchronize(stream));
-  const uint64_t seq = bs ? bs->seq : 0;
-  if (bs) {
-    release(bs);
-    delete bs;
-    *slot = nullptr;
-  }
-  bs = new BuildState;
+  const uint64_t seq = old ? old->seq : 0;
+  delete old;
+  *slot = nullptr;
+  std::unique_ptr<BuildState> bs(new BuildState);
   bs->seq = seq;
   size_t cap = size_t(1) << 17;
   while (cap < n) cap <<= 1;
@@ -200,79 +180,70 @@ int ensure_state(void** slot, cudaStream_t stream, size_t n, size_t raw_bytes, B
     if (const char* e = getenv("MADICP_HOST_THREADS")) bs->threads = std::max(1, atoi(e));
   }
   const size_t nodes = 2 * cap + 2, lvl = cap + 2;
-  int rc = 0;
-  for (int k = 0; k < 2 && !rc; ++k) {
-    rc = dev_alloc(bs, &bs->P[k], 3 * cap);
-    if (!rc) rc = dev_alloc(bs, &bs->owner[k], cap);
+  for (int k = 0; k < 2; ++k) {
+    CK(dev_alloc(bs->P[k], 3 * cap));
+    CK(dev_alloc(bs->owner[k], cap));
   }
-  if (!rc) rc = dev_alloc(bs, &bs->flag, cap);
-  if (!rc) rc = dev_alloc(bs, &bs->G, cap);
-  if (!rc) rc = dev_alloc(bs, &bs->tile, cap / kTile + 2);
-  if (!rc) rc = dev_alloc(bs, &bs->XF, cap);
-  if (!rc) rc = dev_alloc(bs, &bs->BP, cap);
-  if (!rc) rc = dev_alloc(bs, &bs->S, 9 * lvl);
-  if (!rc) rc = dev_alloc(bs, &bs->mid, lvl);
-  if (!rc) rc = dev_alloc(bs, &bs->box, 6 * lvl);
-  if (!rc) rc = dev_alloc(bs, &bs->cnt, lvl);
-  if (!rc) rc = dev_alloc(bs, &bs->imin, lvl);
-  if (!rc) rc = dev_alloc(bs, &bs->child_of, lvl);
-  if (!rc) rc = dev_alloc(bs, &bs->dtile, lvl / 1024 + 4);
-  if (!rc) rc = dev_alloc(bs, &bs->dres, 2 * lvl);
-  if (!rc) rc = dev_alloc(bs, &bs->dmin, lvl);
-  if (!rc) rc = dev_alloc(bs, &bs->N.lo, nodes);
-  if (!rc) rc = dev_alloc(bs, &bs->N.hi, nodes);
-  if (!rc) rc = dev_alloc(bs, &bs->N.parent, nodes);
-  if (!rc) rc = dev_alloc(bs, &bs->N.pp, nodes);
-  if (!rc) rc = dev_alloc(bs, &bs->N.anc, nodes);
-  if (!rc) rc = dev_alloc(bs, &bs->N.link, nodes);
-  if (!rc) rc = dev_alloc(bs, &bs->N.tree, nodes);
-  if (!rc) rc = dev_alloc(bs, &bs->N.full, 16 * nodes);
-  if (!rc) rc = dev_alloc(bs, &bs->d_count, size_t(kMaxLevels) + 2);
-  if (!rc) rc = dev_alloc(bs, &bs->d_lvl, 1);
+  CK(dev_alloc(bs->flag, cap));
+  CK(dev_alloc(bs->G, cap));
+  CK(dev_alloc(bs->tile, cap / kTile + 2));
+  CK(dev_alloc(bs->XF, cap));
+  CK(dev_alloc(bs->BP, cap));
+  CK(dev_alloc(bs->S, 9 * lvl));
+  CK(dev_alloc(bs->mid, lvl));
+  CK(dev_alloc(bs->box, 6 * lvl));
+  CK(dev_alloc(bs->cnt, lvl));
+  CK(dev_alloc(bs->imin, lvl));
+  CK(dev_alloc(bs->child_of, lvl));
+  CK(dev_alloc(bs->dtile, lvl / 1024 + 4));
+  CK(dev_alloc(bs->dres, 2 * lvl));
+  CK(dev_alloc(bs->dmin, lvl));
+  CK(dev_alloc(bs->n_lo, nodes));
+  CK(dev_alloc(bs->n_hi, nodes));
+  CK(dev_alloc(bs->n_parent, nodes));
+  CK(dev_alloc(bs->n_pp, nodes));
+  CK(dev_alloc(bs->n_anc, nodes));
+  CK(dev_alloc(bs->n_link, nodes));
+  CK(dev_alloc(bs->n_tree, nodes));
+  CK(dev_alloc(bs->n_full, 16 * nodes));
+  CK(dev_alloc(bs->d_count, size_t(kMaxLevels) + 2));
+  CK(dev_alloc(bs->d_lvl, 1));
   const size_t tl = size_t(kMaxBatch) * (kMaxLevels + 2);
-  if (!rc) rc = dev_alloc(bs, &bs->d_offs, size_t(kMaxBatch) + 1);
-  if (!rc) rc = dev_alloc(bs, &bs->d_flvl, size_t(kMaxLevels) + 2);
-  if (!rc) rc = dev_alloc(bs, &bs->d_tcnt, tl);
-  if (!rc) rc = dev_alloc(bs, &bs->d_tleaf, size_t(kMaxBatch));
-  if (!rc) rc = dev_alloc(bs, &bs->d_F, tl);
-  if (!rc) rc = dev_alloc(bs, &bs->d_Loff, tl);
-  if (!rc) rc = dev_alloc(bs, &bs->d_out, size_t(kMaxBatch));
-  if (!rc) rc = host_alloc(bs, &bs->h_tcnt, tl);
-  if (!rc) rc = host_alloc(bs, &bs->h_tleaf, size_t(kMaxBatch));
-  if (!rc) rc = host_alloc(bs, &bs->h_F, tl);
-  if (!rc) rc = host_alloc(bs, &bs->h_Loff, tl);
-  if (!rc) rc = host_alloc(bs, &bs->h_offs, size_t(kMaxBatch) + 1);
-  if (!rc) rc = host_alloc(bs, &bs->h_out, size_t(kMaxBatch));
-  if (!rc) {
-    char* raw = nullptr;
-    rc = dev_alloc(bs, &raw, bs->raw_cap);
-    bs->d_raw = raw;
-  }
-  if (!rc) rc = host_alloc(bs, &bs->h_kept, size_t(kMaxBatch));
-  if (!rc) rc = dev_alloc(bs, &bs->d_vtab, size_t(kMaxBatch));
-  if (!rc) rc = host_alloc(bs, &bs->h_vtab, size_t(kMaxBatch));
-  if (!rc) rc = host_alloc(bs, &bs->h_vc_err, 1);
-  if (!rc) rc = dev_alloc(bs, &bs->d_tmax, 1);
-  if (!rc) rc = host_alloc(bs, &bs->h_t_err, 1);
-  if (!rc) rc = dev_alloc(bs, &bs->d_perm, cap);
-  if (!rc) rc = dev_alloc(bs, &bs->d_chunk, cap);
-  if (!rc) rc = dev_alloc(bs, &bs->d_poses, size_t(65536) * 12);
-  if (!rc) rc = host_alloc(bs, &bs->h_args, 2 * lvl);
-  if (!rc) rc = host_alloc(bs, &bs->h_res, 2 * lvl);
-  if (!rc) rc = host_alloc(bs, &bs->h_ctl, size_t(kMaxLevels) + 2);
-  if (!rc) rc = host_alloc(bs, &bs->h_lvl, size_t(kMaxLevels) + 2);
-  if (!rc) rc = host_alloc(bs, &bs->h_perm, cap);
-  if (!rc) rc = host_alloc(bs, &bs->h_chunk, cap);
-  if (!rc) rc = host_alloc(bs, &bs->h_poses, size_t(65536) * 12);
-  if (!rc) rc = host_alloc(bs, &bs->h_root, size_t(kMaxBatch) * 9);
-  if (!rc && cudaStreamCreateWithFlags(&bs->copy_stream, cudaStreamNonBlocking) != cudaSuccess) rc = MADICP_ERR_CUDA;
-  if (!rc && cudaEventCreateWithFlags(&bs->copy_ev, cudaEventDisableTiming) != cudaSuccess) rc = MADICP_ERR_CUDA;
-  if (!rc && cudaEventCreateWithFlags(&bs->idle_ev, cudaEventDisableTiming) != cudaSuccess) rc = MADICP_ERR_CUDA;
-  if (rc) {
-    release(bs);
-    delete bs;
-    return rc;
-  }
+  CK(dev_alloc(bs->d_offs, size_t(kMaxBatch) + 1));
+  CK(dev_alloc(bs->d_flvl, size_t(kMaxLevels) + 2));
+  CK(dev_alloc(bs->d_tcnt, tl));
+  CK(dev_alloc(bs->d_tleaf, size_t(kMaxBatch)));
+  CK(dev_alloc(bs->d_F, tl));
+  CK(dev_alloc(bs->d_Loff, tl));
+  CK(dev_alloc(bs->d_out, size_t(kMaxBatch)));
+  CK(host_alloc(bs->h_tcnt, tl));
+  CK(host_alloc(bs->h_tleaf, size_t(kMaxBatch)));
+  CK(host_alloc(bs->h_F, tl));
+  CK(host_alloc(bs->h_Loff, tl));
+  CK(host_alloc(bs->h_offs, size_t(kMaxBatch) + 1));
+  CK(host_alloc(bs->h_out, size_t(kMaxBatch)));
+  CK(dev_alloc(bs->d_raw, bs->raw_cap));
+  CK(host_alloc(bs->h_kept, size_t(kMaxBatch)));
+  CK(dev_alloc(bs->d_vtab, size_t(kMaxBatch)));
+  CK(host_alloc(bs->h_vtab, size_t(kMaxBatch)));
+  CK(host_alloc(bs->h_vc_err, 1));
+  CK(dev_alloc(bs->d_tmax, 1));
+  CK(host_alloc(bs->h_t_err, 1));
+  CK(dev_alloc(bs->d_perm, cap));
+  CK(dev_alloc(bs->d_chunk, cap));
+  CK(dev_alloc(bs->d_poses, size_t(65536) * 12));
+  CK(host_alloc(bs->h_args, 2 * lvl));
+  CK(host_alloc(bs->h_res, 2 * lvl));
+  CK(host_alloc(bs->h_ctl, size_t(kMaxLevels) + 2));
+  CK(host_alloc(bs->h_lvl, size_t(kMaxLevels) + 2));
+  CK(host_alloc(bs->h_perm, cap));
+  CK(host_alloc(bs->h_chunk, cap));
+  CK(host_alloc(bs->h_poses, size_t(65536) * 12));
+  CK(host_alloc(bs->h_root, size_t(kMaxBatch) * 9));
+  CK(cudaStreamCreateWithFlags(bs->copy_stream.put(), cudaStreamNonBlocking));
+  CK(cudaEventCreateWithFlags(bs->copy_ev.put(), cudaEventDisableTiming));
+  CK(cudaEventCreateWithFlags(bs->idle_ev.put(), cudaEventDisableTiming));
+  bs->N = Nodes{bs->n_lo, bs->n_hi, bs->n_parent, bs->n_pp, bs->n_anc, bs->n_link, bs->n_tree, bs->n_full};
   Work& W = bs->W;
   W.P[0] = bs->P[0]; W.P[1] = bs->P[1];
   W.owner[0] = bs->owner[0]; W.owner[1] = bs->owner[1];
@@ -281,8 +252,8 @@ int ensure_state(void** slot, cudaStream_t stream, size_t n, size_t raw_bytes, B
   W.dtile = bs->dtile; W.dres = bs->dres;
   W.dmin = bs->dmin; W.N = bs->N; W.count = bs->d_count; W.lvl = bs->d_lvl;
   W.args = bs->h_args; W.res = bs->h_res; W.ctl = bs->h_ctl;
-  *slot = bs;
-  *out = bs;
+  *out = bs.get();
+  *slot = bs.release();
   return MADICP_OK;
 }
 int ensure_state(madicp_ctx* c, size_t n, size_t raw_bytes, BuildState** out) {
@@ -439,15 +410,13 @@ int blocks(int64_t n, int per = kBlock) { return int(std::max<int64_t>(1, (n + p
 
 // ---- record indices of kept clouds (madicp_set_keep_cloud): nothing below runs unless the context keeps clouds
 int ensure_idx(BuildState* bs) {
-  if (!bs->d_idx)
-    if (int e = dev_alloc(bs, &bs->d_idx, bs->cap)) return e;
-  if (!bs->d_rec)
-    if (int e = dev_alloc(bs, &bs->d_rec, bs->cap)) return e;
+  if (!bs->d_idx) CK(dev_alloc(bs->d_idx, bs->cap));
+  if (!bs->d_rec) CK(dev_alloc(bs->d_rec, bs->cap));
   return MADICP_OK;
 }
 // rec_of[rank] for the records of B (k_kept_records): gated, over the flags and scan of the compaction just launched
 int keep_records(madicp_ctx* c, cudaStream_t st, BuildState* bs, const RecBatch& B, bool gated, int* rec_of) {
-  k_kept_records<<<blocks(B.n_rec), kBlock, 0, st>>>(B, gated ? bs->flag : nullptr, bs->G, bs->tile, rec_of);
+  k_kept_records<<<blocks(B.n_rec), kBlock, 0, st>>>(B, gated ? bs->flag.get() : nullptr, bs->G, bs->tile, rec_of);
   c->launches++;
   CK(cudaGetLastError());
   return MADICP_OK;
@@ -546,7 +515,7 @@ int build_forest(madicp_ctx* c, BuildState* bs, cudaStream_t st, int n_trees, co
       set_error(std::string("madtree_gpu_build: graph capture: ") + cudaGetErrorString(e));
       return MADICP_ERR_CUDA;
     }
-    e = cudaGraphInstantiate(&bs->level_graph, g, 0);
+    e = cudaGraphInstantiate(bs->level_graph.put(), g, 0);
     cudaGraphDestroy(g);
     if (e != cudaSuccess) {
       set_error(std::string("madtree_gpu_build: graph instantiate: ") + cudaGetErrorString(e));
@@ -702,10 +671,7 @@ void madicp_gpu_build_release(madicp_ctx* c) {
     release_plan_lane(static_cast<PlanLane*>(c->plan_state));
     c->plan_state = nullptr;
   }
-  BuildState* bs = static_cast<BuildState*>(c->build_state);
-  if (!bs) return;
-  release(bs);
-  delete bs;
+  delete static_cast<BuildState*>(c->build_state);
   c->build_state = nullptr;
 }
 
@@ -1010,45 +976,31 @@ int stage(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, int
 // device and pinned buffers of one plan, recycled through the lane's cache (as device trees are)
 struct PlanBuf {
   size_t cap = 0, raw_cap = 0;  // records, bytes
-  char* d_raw = nullptr;        // the records as uploaded
-  int32_t* d_perm = nullptr;
-  uint16_t* d_chunk = nullptr;
-  int32_t* h_perm = nullptr;  // pinned: what the order half writes
-  uint16_t* h_chunk = nullptr;
-  cudaEvent_t ready = nullptr;    // lane stream: records, perm and chunk are on the device
-  cudaEvent_t free_ev = nullptr;  // context stream: the last ingest that read the device buffers has run
+  DevPtr<char> d_raw;           // the records as uploaded
+  DevPtr<int32_t> d_perm;
+  DevPtr<uint16_t> d_chunk;
+  HostPtr<int32_t> h_perm;  // pinned: what the order half writes
+  HostPtr<uint16_t> h_chunk;
+  Event ready;    // lane stream: records, perm and chunk are on the device
+  Event free_ev;  // context stream: the last ingest that read the device buffers has run
   // a plan of device records (madicp_plan_points_dev): d_raw holds its kept points, compacted and corrected as packed
   // float64 on the context's stream; the order half reads them back
-  int* h_cnt = nullptr;              // mapped: [0] kept points, [1] a correction fell outside its table, [2] a kept time
+  HostPtr<int> h_cnt;                // mapped: [0] kept points, [1] a correction fell outside its table, [2] a kept time
                                      // stamp is NaN or infinite
-  double* h_pts = nullptr;           // pinned, 3 x cap, at first use: the kept points for the order half
-  cudaEvent_t compacted = nullptr;   // context stream: the compaction has run
+  HostPtr<double> h_pts;             // pinned, 3 x cap, at first use: the kept points for the order half
+  Event compacted;                   // context stream: the compaction has run
   // a plan with a time field (madicp_plan_points_t): its kept points, corrected, and their stamps, compacted on the
   // context's stream; d_tmax: the largest kept stamp's key.  At first use.
-  double* d_pts = nullptr;
-  double* d_tau = nullptr;
-  unsigned long long* d_tmax = nullptr;
+  DevPtr<double> d_pts;
+  DevPtr<double> d_tau;
+  DevPtr<unsigned long long> d_tmax;
   // kept clouds (madicp_set_keep_cloud), at first use: the record of every kept rank of a compaction done at hand-over
-  int* d_rec = nullptr;
+  DevPtr<int> d_rec;
 };
 void free_buf(PlanBuf* b) {
   if (b->ready) cudaEventSynchronize(b->ready);
   if (b->free_ev) cudaEventSynchronize(b->free_ev);
   if (b->compacted) cudaEventSynchronize(b->compacted);
-  cudaFree(b->d_pts);
-  cudaFree(b->d_tau);
-  cudaFree(b->d_tmax);
-  cudaFree(b->d_rec);
-  cudaFree(b->d_raw);
-  cudaFree(b->d_perm);
-  cudaFree(b->d_chunk);
-  cudaFreeHost(b->h_perm);
-  cudaFreeHost(b->h_chunk);
-  cudaFreeHost(b->h_cnt);
-  cudaFreeHost(b->h_pts);
-  if (b->ready) cudaEventDestroy(b->ready);
-  if (b->free_ev) cudaEventDestroy(b->free_ev);
-  if (b->compacted) cudaEventDestroy(b->compacted);
   delete b;
 }
 
@@ -1056,9 +1008,9 @@ struct PlanLane {
   static constexpr int kRing = 8;                // chunk-pose tables in flight
   static constexpr int kRingPoses = 2 * 1024;    // per table: the sweep makes at most 1024 chunks (+1 on rounding)
   int device = 0;
-  cudaStream_t stream = nullptr;  // uploads of the plans
-  double* h_poses = nullptr;      // pinned ring of chunk-pose tables: kRing x kRingPoses x 12
-  cudaEvent_t ring_done[kRing] = {};
+  Stream stream;             // uploads of the plans
+  HostPtr<double> h_poses;   // pinned ring of chunk-pose tables: kRing x kRingPoses x 12
+  Event ring_done[kRing];
   uint32_t ring_seq = 0;
   std::mutex mu;  // everything below
   std::condition_variable cv;
@@ -1105,13 +1057,7 @@ void release_plan_lane(PlanLane* L) {
   L->cv.notify_all();
   for (std::thread& t : L->workers) t.join();
   for (PlanBuf* b : L->cache) free_buf(b);
-  if (L->stream) {
-    cudaStreamSynchronize(L->stream);
-    cudaStreamDestroy(L->stream);
-  }
-  for (cudaEvent_t e : L->ring_done)
-    if (e) cudaEventDestroy(e);
-  if (L->h_poses) cudaFreeHost(L->h_poses);
+  cudaStreamSynchronize(L->stream);
   delete L;
 }
 
@@ -1120,18 +1066,17 @@ int plan_lane(madicp_ctx* c, PlanLane** out) {
     *out = static_cast<PlanLane*>(c->plan_state);
     return MADICP_OK;
   }
-  PlanLane* L = new PlanLane;
+  std::unique_ptr<PlanLane> L(new PlanLane);
   L->device = c->device;
-  cudaError_t e = cudaStreamCreateWithFlags(&L->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaHostAlloc(&L->h_poses, size_t(PlanLane::kRing) * PlanLane::kRingPoses * 12 * sizeof(double), 0);
-  for (int r = 0; r < PlanLane::kRing && e == cudaSuccess; ++r) e = cudaEventCreateWithFlags(&L->ring_done[r], cudaEventDisableTiming);
+  cudaError_t e = cudaStreamCreateWithFlags(L->stream.put(), cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaHostAlloc(L->h_poses.put(), size_t(PlanLane::kRing) * PlanLane::kRingPoses * 12 * sizeof(double), 0);
+  for (int r = 0; r < PlanLane::kRing && e == cudaSuccess; ++r) e = cudaEventCreateWithFlags(L->ring_done[r].put(), cudaEventDisableTiming);
   if (e != cudaSuccess) {
-    release_plan_lane(L);
     set_error(std::string("madicp_plan_points: ") + cudaGetErrorString(e));
     return MADICP_ERR_CUDA;
   }
-  c->plan_state = L;
-  *out = L;
+  *out = L.get();
+  c->plan_state = L.release();
   return MADICP_OK;
 }
 
@@ -1146,26 +1091,25 @@ int plan_buf(PlanLane* L, size_t n, size_t bytes, PlanBuf** out) {
         return MADICP_OK;
       }
   }
-  PlanBuf* b = new PlanBuf;
+  std::unique_ptr<PlanBuf> b(new PlanBuf);  // (new: nothing reads it yet)
   b->cap = size_t(1) << 17;
   while (b->cap < n) b->cap <<= 1;
   b->raw_cap = size_t(1) << 21;
   while (b->raw_cap < bytes) b->raw_cap <<= 1;
-  cudaError_t e = cudaMalloc(&b->d_raw, b->raw_cap);
-  if (e == cudaSuccess) e = cudaMalloc(&b->d_perm, b->cap * sizeof(int32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&b->d_chunk, b->cap * sizeof(uint16_t));
-  if (e == cudaSuccess) e = cudaHostAlloc(&b->h_perm, b->cap * sizeof(int32_t), 0);
-  if (e == cudaSuccess) e = cudaHostAlloc(&b->h_chunk, b->cap * sizeof(uint16_t), 0);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->ready, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->free_ev, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaHostAlloc(&b->h_cnt, 4 * sizeof(int), cudaHostAllocMapped);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->compacted, cudaEventDisableTiming);
+  cudaError_t e = cudaMalloc(b->d_raw.put(), b->raw_cap);
+  if (e == cudaSuccess) e = cudaMalloc(b->d_perm.put(), b->cap * sizeof(int32_t));
+  if (e == cudaSuccess) e = cudaMalloc(b->d_chunk.put(), b->cap * sizeof(uint16_t));
+  if (e == cudaSuccess) e = cudaHostAlloc(b->h_perm.put(), b->cap * sizeof(int32_t), 0);
+  if (e == cudaSuccess) e = cudaHostAlloc(b->h_chunk.put(), b->cap * sizeof(uint16_t), 0);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(b->ready.put(), cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(b->free_ev.put(), cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaHostAlloc(b->h_cnt.put(), 4 * sizeof(int), cudaHostAllocMapped);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(b->compacted.put(), cudaEventDisableTiming);
   if (e != cudaSuccess) {
-    free_buf(b);
     set_error(std::string("madicp_plan_points: ") + cudaGetErrorString(e));
     return MADICP_ERR_CUDA;
   }
-  *out = b;
+  *out = b.release();
   return MADICP_OK;
 }
 void return_buf(PlanLane* L, PlanBuf* b) {
@@ -1215,7 +1159,7 @@ void plan_order(madicp_plan* p) {
     if (!rc && b->h_cnt[1]) rc = MADICP_ERR_STATE;
     if (!rc) p->kept = b->h_cnt[0];
     if (!rc && p->kept > 0) {
-      if (!b->h_pts) cuda(cudaHostAlloc(&b->h_pts, b->cap * 3 * sizeof(double), 0), "cudaHostAlloc");
+      if (!b->h_pts) cuda(cudaHostAlloc(b->h_pts.put(), b->cap * 3 * sizeof(double), 0), "cudaHostAlloc");
       if (!rc) cuda(cudaMemcpyAsync(b->h_pts, b->d_raw, size_t(p->kept) * 24, cudaMemcpyDeviceToHost, st), "kept points");
       if (!rc) cuda(cudaEventRecord(b->ready, st), "cudaEventRecord");
       if (!rc) cuda(cudaEventSynchronize(b->ready), "cudaEventSynchronize");
@@ -1412,7 +1356,7 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, co
     base = static_cast<const char*>(bs->d_raw);
   }
   if (compacted) {  // the plan's kept points, packed float64 (and their stamps)
-    const double* pts = plan->tm.type != kTimeNone ? pb->d_pts : reinterpret_cast<const double*>(pb->d_raw);
+    const double* pts = plan->tm.type != kTimeNone ? pb->d_pts.get() : reinterpret_cast<const double*>(pb->d_raw.get());
     if (k.on)
       if (int e = stage_chunk_poses(plan->lane, st, k.T_prev, k.T_now, k.hz, timed ? kTimeChunks : plan->n_chunks,
                                     bs->d_poses))
@@ -1480,8 +1424,7 @@ int ingest(madicp_ctx* c, const madicp_points_t& d, const madicp_vcorr_t& vc, co
       }
       kept = bs->h_kept[0];
       if (k.on && !timed && kept > 0) {  // the kept points come back for the host's order: a packed, plain cloud
-        if (!bs->h_packed)
-          if (int e = host_alloc(bs, &bs->h_packed, 3 * bs->cap)) return e;
+        if (!bs->h_packed) CK(host_alloc(bs->h_packed, 3 * bs->cap));
         CK(cudaMemcpyAsync(bs->h_packed, bs->P[1], size_t(kept) * 24, cudaMemcpyDeviceToHost, st));
         int64_t n_sorted = 0;
         if (int e = host_order(bs, st, packed_points(bs->h_packed, kept, 0), madicp_vcorr_t{}, k, fn, &n_sorted)) return e;
@@ -1516,9 +1459,9 @@ int hand_over(madicp_ctx* c, madicp_plan* p) {
     if (!timed) return MADICP_OK;
   }
   if (timed && !b->d_pts) {
-    CK(cudaMalloc(&b->d_pts, b->cap * 3 * sizeof(double)));
-    CK(cudaMalloc(&b->d_tau, b->cap * sizeof(double)));
-    CK(cudaMalloc(&b->d_tmax, sizeof(unsigned long long)));
+    CK(cudaMalloc(b->d_pts.put(), b->cap * 3 * sizeof(double)));
+    CK(cudaMalloc(b->d_tau.put(), b->cap * sizeof(double)));
+    CK(cudaMalloc(b->d_tmax.put(), sizeof(unsigned long long)));
   }
   BuildState* bs = static_cast<BuildState*>(c->build_state);
   if (bs && bs->cap < size_t(d.n))  // the lane is about to be re-allocated: early uploads are lost
@@ -1537,12 +1480,12 @@ int hand_over(madicp_ctx* c, madicp_plan* p) {
   if (timed) {
     const TimeArgs T = time_args(p->tm, base, 0.0, b->d_tmax, b->h_cnt + 2, nullptr, b->d_tau);
     if (int e = launch_compaction_time(c, bs, st, B, T, b->d_pts, b->h_cnt, b->h_cnt + 1, p->vc.enabled)) return e;
-  } else if (int e = launch_compaction(c, bs, st, B, reinterpret_cast<double*>(b->d_raw), b->h_cnt, b->h_cnt + 1,
+  } else if (int e = launch_compaction(c, bs, st, B, reinterpret_cast<double*>(b->d_raw.get()), b->h_cnt, b->h_cnt + 1,
                                        p->vc.enabled)) {
     return e;
   }
   if (p->keep) {  // (madicp_set_keep_cloud: the records of the kept ranks)
-    if (!b->d_rec) CK(cudaMalloc(&b->d_rec, b->cap * sizeof(int)));
+    if (!b->d_rec) CK(cudaMalloc(b->d_rec.put(), b->cap * sizeof(int)));
     if (int e = keep_records(c, st, bs, B, true, b->d_rec)) return e;
   }
   CK(cudaEventRecord(b->compacted, st));

@@ -25,6 +25,17 @@ namespace madicp_b200 {
 struct DevScan {
   void* stream = nullptr;
 };
+// One scan as the Pipeline hands it to the library.  A packed N x 3 cloud is records without a gate
+// (madicp::packed_points), so every scan is one descriptor with its correction and time field.
+struct Scan {
+  madicp_points_t pts{};
+  madicp_vcorr_t vc{};    // disabled: none
+  madicp_times_t tm{};    // the records' time field (kTimeNone: none, the azimuth deskew)
+  bool dev = false;       // device memory, ready on `stream` (DevScan)
+  void* stream = nullptr;
+  bool records = false;   // handed over as records (computeRecords, prefetchRecords), not as a packed cloud
+  std::shared_ptr<void> keepalive;  // a queued scan's memory, which pts.data points into: the caller's buffer or a copy
+};
 namespace detail {
 
 using madicp_pose::Pose;
@@ -95,7 +106,7 @@ struct VelocityEstimator {
 }  // namespace detail
 
 // Look-ahead tree builds: scans handed to Pipeline::prefetch are queued; when compute() needs the tree of the oldest
-// one, the trees of ALL queued scans (up to `batch`) are built in one go, as one forest (madtree_gpu_build_batch) --
+// one, the trees of ALL queued scans (up to `batch`) are built in one go, as one forest (madtree_gpu_build_batch_points) --
 // the build's latency is that of its dependent-add chains, which a batch runs side by side -- and compute() then
 // consumes them in FIFO order.  Possible because a scan's tree depends on the pose estimates only when the scan is
 // deskewed (pipeline.cpp:137-141).  No threads: the batch is built by the thread that calls compute().
@@ -105,21 +116,9 @@ struct VelocityEstimator {
 class Lookahead {
  public:
   struct Job {
-    std::vector<double> f64;  // private copies of the cloud ...
-    std::vector<float> f32;
-    const void* ext = nullptr;        // ... or the caller's buffer, kept alive by `keepalive` until its tree is built
-    bool is_f32 = false;
-    bool records = false;             // raw sensor records (Pipeline::prefetchRecords): `pts` describes them, `vc` is
-    madicp_points_t pts{};            // their vertical correction (disabled: none)
-    madicp_vcorr_t vc{};
-    madicp_times_t tm{};              // a deskewed scan's time field (none: the azimuth deskew)
-    bool dev = false;                 // records in device memory, ready on `stream` (DevScan): never staged
-    void* stream = nullptr;
-    std::shared_ptr<void> keepalive;
-    size_t n = 0;
+    Scan scan;  // kept alive until its tree is built or its plan consumed; device scans are never staged
     madtree_gpu_t* tree = nullptr;
     madicp_plan_t* plan = nullptr;  // a deskewed scan's look-ahead plan (pushPlan)
-    const void* data() const { return ext ? ext : (is_f32 ? static_cast<const void*>(f32.data()) : static_cast<const void*>(f64.data())); }
   };
   Lookahead(madicp_ctx_t* ctx, double b_max, double b_min, int batch) : ctx_(ctx), b_max_(b_max), b_min_(b_min), batch_(batch) {}
   ~Lookahead() {
@@ -129,19 +128,17 @@ class Lookahead {
       if (j.plan) madicp_plan_free(j.plan);  // (returns once nothing reads the scan's buffer)
     }
   }
-  void push(Job&& j) {
-    fifo_.push_back(std::move(j));
+  void push(Scan&& s) {
+    fifo_.push_back(Job{std::move(s)});
     stageQueued();
   }
-  // a deskewed scan: planned at once, over its records or its packed cloud, with at most num_threads plans' order
-  // halves running at a time
-  void pushPlan(Job&& j, int num_threads) {
-    fifo_.push_back(std::move(j));
-    Job& q = fifo_.back();  // (planned where its private copy, if any, will stay)
-    const madicp_points_t d = q.records ? q.pts : madicp::packed_points(q.data(), int64_t(q.n), q.is_f32 ? 1 : 0);
-    const int rc = q.dev ? madicp_plan_points_dev_t(ctx_, &d, &q.vc, &q.tm, num_threads, q.stream, &q.plan)
-                         : madicp_plan_points_t(ctx_, &d, q.records ? &q.vc : nullptr, q.records ? &q.tm : nullptr,
-                                                num_threads, &q.plan);
+  // a deskewed scan: planned at once, with at most num_threads plans' order halves running at a time
+  void pushPlan(Scan&& scan, int num_threads) {
+    fifo_.push_back(Job{std::move(scan)});
+    Job& q = fifo_.back();
+    const Scan& s = q.scan;
+    const int rc = s.dev ? madicp_plan_points_dev_t(ctx_, &s.pts, &s.vc, &s.tm, num_threads, s.stream, &q.plan)
+                         : madicp_plan_points_t(ctx_, &s.pts, &s.vc, &s.tm, num_threads, &q.plan);
     if (rc < 0) {
       const std::string msg = "madicp_plan_points failed (" + std::to_string(rc) + "): " + madicp_last_error();
       fifo_.pop_back();
@@ -171,8 +168,9 @@ class Lookahead {
   // scans that can share one batch call: packed clouds of one element type, or records (each with its own correction:
   // the batch call takes one per scan) -- host records, or device records ready on one stream
   static bool sameKind(const Job& a, const Job& b) {
-    return !a.plan && !b.plan && a.records == b.records && (a.records || a.is_f32 == b.is_f32) && a.dev == b.dev &&
-           (!a.dev || a.stream == b.stream);
+    const Scan &x = a.scan, &y = b.scan;
+    return !a.plan && !b.plan && x.records == y.records && (x.records || x.pts.is_f32 == y.pts.is_f32) && x.dev == y.dev &&
+           (!x.dev || x.stream == y.stream);
   }
   // Builds the trees of the longest run of queued scans of the front's kind, up to the batch size.  A scan whose tree
   // cannot be built (records the range gate leaves empty) fails the batch call as a whole: the run is then halved until
@@ -180,33 +178,25 @@ class Lookahead {
   // error is raised -- in the compute() call that reaches that scan.  The scans after it stay queued.
   void buildBatch() {
     size_t k = 0;
-    const Job& front = fifo_.front();
+    const Scan& front = fifo_.front().scan;
     for (const Job& j : fifo_) {
-      if (int(k) == batch_ || j.tree || !sameKind(j, front)) break;
+      if (int(k) == batch_ || j.tree || !sameKind(j, fifo_.front())) break;
       ++k;
     }
     std::vector<madtree_gpu_t*> out;
     for (;;) {
-      std::vector<const void*> ptr;
-      std::vector<int64_t> n;
       std::vector<madicp_points_t> pts;
       std::vector<madicp_vcorr_t> vc;
       for (size_t i = 0; i < k; ++i) {
-        ptr.push_back(fifo_[i].data());
-        n.push_back(int64_t(fifo_[i].n));
-        pts.push_back(fifo_[i].pts);
-        vc.push_back(fifo_[i].vc);
+        pts.push_back(fifo_[i].scan.pts);
+        vc.push_back(fifo_[i].scan.vc);
       }
       out.assign(k, nullptr);
-      const int rc =
-          front.dev ? madtree_gpu_build_batch_points_dev(ctx_, pts.data(), vc.data(), int(k), b_max_, b_min_, front.stream,
-                                                         out.data())
-          : front.records ? madtree_gpu_build_batch_points_ex(ctx_, pts.data(), vc.data(), int(k), b_max_, b_min_, out.data())
-                          : madtree_gpu_build_batch(ctx_, ptr.data(), n.data(), front.is_f32 ? 1 : 0, int(k), b_max_, b_min_,
-                                                    out.data());
+      const int rc = front.dev ? madtree_gpu_build_batch_points_dev(ctx_, pts.data(), vc.data(), int(k), b_max_, b_min_,
+                                                                    front.stream, out.data())
+                               : madtree_gpu_build_batch_points_ex(ctx_, pts.data(), vc.data(), int(k), b_max_, b_min_, out.data());
       if (rc >= 0) break;
-      const std::string msg = std::string(front.records ? "madtree_gpu_build_batch_points" : "madtree_gpu_build_batch") +
-                              " failed (" + std::to_string(rc) + "): " + madicp_last_error();
+      const std::string msg = "madtree_gpu_build_batch_points failed (" + std::to_string(rc) + "): " + madicp_last_error();
       madicp_stage_discard(ctx_);  // (the failed call consumed the early uploads, or they are given up here)
       staged_ = 0;
       if (k == 1) {
@@ -221,23 +211,17 @@ class Lookahead {
     for (size_t i = 0; i < out.size(); ++i) {
       Job& j = fifo_[i];
       j.tree = out[i];
-      j.keepalive.reset();  // (the clouds have been copied to the device: pageable copies are staged before the call returns)
-      j.f64 = std::vector<double>();
-      j.f32 = std::vector<float>();
+      j.scan.keepalive.reset();  // (the scans have been copied to the device: pageable copies are staged before the call returns)
     }
     stageQueued();
   }
-  // Early upload (madicp_stage_cloud) of the queued scans whose trees are not built yet, oldest first, up to one
+  // Early upload (madicp_stage_points_ex) of the queued scans whose trees are not built yet, oldest first, up to one
   // batch: the copies run while the device registers the scans before them.
   void stageQueued() {
     while (staged_ < size_t(batch_) && built_ + staged_ < fifo_.size()) {
       const Job& j = fifo_[built_ + staged_];
-      if (j.plan || j.dev || !sameKind(j, fifo_[built_])) break;
-      if (j.records)
-        check(madicp_stage_points_ex(ctx_, &j.pts, &j.vc, int64_t(batch_) * int64_t(j.n)), "madicp_stage_points");
-      else
-        check(madicp_stage_cloud(ctx_, j.data(), int64_t(j.n), j.is_f32 ? 1 : 0, int64_t(batch_) * int64_t(j.n)),
-              "madicp_stage_cloud");
+      if (j.plan || j.scan.dev || !sameKind(j, fifo_[built_])) break;
+      check(madicp_stage_points_ex(ctx_, &j.scan.pts, &j.scan.vc, int64_t(batch_) * j.scan.pts.n), "madicp_stage_points");
       ++staged_;
     }
   }
@@ -332,21 +316,12 @@ class Pipeline {
   // pipeline.cpp:125-265; reference signature (pipeline.h:71): the cloud by value
   void compute(double stamp, ContainerType cloud) {
     if (cloud.empty()) throw Error("Pipeline.compute: empty cloud");
-    computeRaw(stamp, cloud[0].data(), cloud.size(), false);
+    computeScan(stamp, packedScan(cloud[0].data(), cloud.size(), false));
   }
   // the same without taking ownership: N x 3 doubles read in place
-  void compute(double stamp, const double* xyz, size_t n) { computeRaw(stamp, xyz, n, false); }
+  void compute(double stamp, const double* xyz, size_t n) { computeScan(stamp, packedScan(xyz, n, false)); }
   // float32 scans as the dataset readers produce them (the conversion to float64 runs on the device)
-  void computeF32(double stamp, const float* xyz, size_t n) {
-    if (!gpu_build_) {
-      ContainerType cloud(n);
-      for (size_t i = 0; i < n; ++i)
-        for (int a = 0; a < 3; ++a) cloud[i][size_t(a)] = double(xyz[3 * i + size_t(a)]);
-      compute(stamp, std::move(cloud));
-      return;
-    }
-    computeRaw(stamp, xyz, n, true);
-  }
+  void computeF32(double stamp, const float* xyz, size_t n) { computeScan(stamp, packedScan(xyz, n, true)); }
   // Raw sensor records with the dataset readers' range gate (include/madicp_b200.h, madicp_points_t), read in place:
   // the same result as compute() on the reader's filtered array -- corrected by `vc` (nullable: none) like KITTI's
   // reader with apply_correction.  MADICP_GPU_BUILD=0: the kept points are packed (and corrected) on the host with the
@@ -363,18 +338,9 @@ class Pipeline {
       check(madicp::check_points(&pts, "Pipeline.computeRecords"), "Pipeline.computeRecords");
       check(madicp::check_times(tm, &pts, "Pipeline.computeRecords"), "Pipeline.computeRecords");
     }
-    const madicp_times_t t = madicp::times_of(tm);
-    if (!gpu_build_) {
-      std::vector<int32_t> idx;
-      const ContainerType cloud = packRecords(pts, vc, keep_cloud_ ? &idx : nullptr);
-      const madicp_vcorr_t v = madicp::vcorr_of(vc);
-      computeRaw(stamp, cloud[0].data(), cloud.size(), false, t.type ? &pts : nullptr, &v, nullptr, t.type ? &t : nullptr,
-                 keep_cloud_ ? idx.data() : nullptr);
-      return;
-    }
-    if (!pts.data || pts.n <= 0) throw Error("Pipeline.computeRecords: empty scan");
-    const madicp_vcorr_t v = madicp::vcorr_of(vc);
-    computeRaw(stamp, pts.data, size_t(pts.n), pts.is_f32 != 0, &pts, &v, dev, t.type ? &t : nullptr);
+    if (!gpu_build_) check(madicp::check_points(&pts, "Pipeline.computeRecords"), "Pipeline.computeRecords");
+    else if (!pts.data || pts.n <= 0) throw Error("Pipeline.computeRecords: empty scan");
+    computeScan(stamp, recordsScan(pts, vc, dev, tm));
   }
   bool gpuBuild() const { return gpu_build_; }
   int lastIcpIterations() const { return last_iters_; }  // rounds the realtime budget allowed for the last scan
@@ -402,32 +368,28 @@ class Pipeline {
       if (batch < 1) return false;
       lookahead_.reset(new Lookahead(icp_.context(), b_max_, b_min_, std::min(batch, 64)));
     }
-    Lookahead::Job j;
-    j.n = n;
-    j.is_f32 = is_f32;
+    Scan s;
     if (records) {  // (read in place: the caller must hand over a keepalive)
       if (!keepalive) throw Error("Pipeline.prefetchRecords: the records must be kept alive");
       // a descriptor the library would reject must not enter the queue (every later batch would fail on it)
       check(madicp::check_points(records, "Pipeline.prefetchRecords"), "Pipeline.prefetchRecords");
       check(madicp::check_vcorr(vc, "Pipeline.prefetchRecords"), "Pipeline.prefetchRecords");
       check(madicp::check_times(tm, records, "Pipeline.prefetchRecords"), "Pipeline.prefetchRecords");
-      j.records = true;
-      if (deskew_) j.tm = madicp::times_of(tm);  // (a scan that is not deskewed goes into a batch build: no time field)
-      j.pts = *records;
-      j.vc = madicp::vcorr_of(vc);
-      j.dev = dev != nullptr;
-      j.stream = dev ? dev->stream : nullptr;
+      // (a scan that is not deskewed goes into a batch build: no time field)
+      s = recordsScan(*records, vc, dev, deskew_ ? tm : nullptr);
+    } else {
+      s.pts = madicp::packed_points(xyz, int64_t(n), is_f32 ? 1 : 0);
     }
     if (keepalive) {
-      j.ext = xyz;
-      j.keepalive = std::move(keepalive);
-    } else if (is_f32) {
-      j.f32.assign(static_cast<const float*>(xyz), static_cast<const float*>(xyz) + 3 * n);
-    } else {
-      j.f64.assign(static_cast<const double*>(xyz), static_cast<const double*>(xyz) + 3 * n);
+      s.keepalive = std::move(keepalive);
+    } else {  // a private copy of the packed cloud
+      const char* p = static_cast<const char*>(xyz);
+      auto copy = std::make_shared<std::vector<char>>(p, p + 3 * n * (is_f32 ? sizeof(float) : sizeof(double)));
+      s.pts.data = copy->data();
+      s.keepalive = std::move(copy);
     }
-    if (deskew_) lookahead_->pushPlan(std::move(j), num_threads_);
-    else lookahead_->push(std::move(j));
+    if (deskew_) lookahead_->pushPlan(std::move(s), num_threads_);
+    else lookahead_->push(std::move(s));
     return true;
   }
   bool prefetchRecords(const madicp_points_t& pts, std::shared_ptr<void> keepalive, const madicp_vcorr_t* vc = nullptr,
@@ -438,6 +400,24 @@ class Pipeline {
   size_t prefetched() { return lookahead_ ? lookahead_->size() : 0; }
 
  private:
+  // a packed N x 3 cloud, read in place
+  static Scan packedScan(const void* xyz, size_t n, bool is_f32) {
+    if (!xyz || n == 0) throw Error("Pipeline.compute: empty cloud");
+    Scan s;
+    s.pts = madicp::packed_points(xyz, int64_t(n), is_f32 ? 1 : 0);
+    return s;
+  }
+  // records with their correction and time field (both nullable: none), in device memory when `dev` is given
+  static Scan recordsScan(const madicp_points_t& pts, const madicp_vcorr_t* vc, const DevScan* dev, const madicp_times_t* tm) {
+    Scan s;
+    s.pts = pts;
+    s.vc = madicp::vcorr_of(vc);
+    s.tm = madicp::times_of(tm);
+    s.dev = dev != nullptr;
+    s.stream = dev ? dev->stream : nullptr;
+    s.records = true;
+    return s;
+  }
   // whether there is a current scan whose cloud can be read (throws without keep_cloud)
   bool requireCloud() const {
     if (!keep_cloud_) throw Error("Pipeline.currentCloud: the pipeline keeps no cloud (construct it with keep_cloud=True)");
@@ -452,12 +432,31 @@ class Pipeline {
       trees.push_back(current_->tree.get());
     return trees;
   }
+  // Host-built trees: the scan's kept points as a packed float64 cloud (a packed float64 scan is read in place, any
+  // other goes through packRecords) and, with keep_cloud, the record index of every point
+  struct HostCloud {
+    const double* xyz = nullptr;
+    size_t n = 0;
+    std::vector<int32_t> idx;
+    ContainerType packed;
+  };
+  HostCloud hostCloud(const Scan& s) const {
+    HostCloud h;
+    if (s.records || s.pts.is_f32) {
+      h.packed = packRecords(s.pts, &s.vc, keep_cloud_ ? &h.idx : nullptr);
+      h.xyz = h.packed[0].data();
+      h.n = h.packed.size();
+      return h;
+    }
+    h.xyz = static_cast<const double*>(s.pts.data);
+    h.n = size_t(s.pts.n);
+    if (keep_cloud_)
+      for (size_t i = 0; i < h.n; ++i) h.idx.push_back(int32_t(i));
+    return h;
+  }
+
   // the scan's MAD-tree: ingest (+ deskew, pipeline.cpp:137-138) and build, on the device or on the host
-  // tm (nullable): the records' time field.  Host-built trees (MADICP_GPU_BUILD=0): xyz is the packed kept cloud and
-  // `records` the scan it came from, for the stamps.
-  std::unique_ptr<MADtree> makeTree(const void* xyz, size_t n, bool is_f32, const madicp_points_t* records,
-                                    const madicp_vcorr_t* vc, const DevScan* dev, const madicp_times_t* tm,
-                                    const int32_t* rec_idx) {
+  std::unique_ptr<MADtree> makeTree(const Scan& s) {
     const bool dsk = deskew_ && is_initialized_ && trajectory_.size() > 1;
     const double* Ta = dsk ? trajectory_[trajectory_.size() - 2].m : nullptr;
     const double* Tb = dsk ? trajectory_[trajectory_.size() - 1].m : nullptr;
@@ -468,39 +467,27 @@ class Pipeline {
     }
     if (lookahead_ && !lookahead_->empty())  // built ahead of time by a worker lane
       return std::unique_ptr<MADtree>(new MADtree(icp_.context(), lookahead_->pop(), b_max_));
-    if (gpu_build_ && records && dev) {
-      check(madicp_ingest_points_dev_t(icp_.context(), records, vc, tm, dsk ? 1 : 0, Ta, Tb, sensor_hz_,
-                                       std::max(1 << max_parallel_levels_, 1), dev->stream, nullptr, nullptr),
-            "madicp_ingest_points_dev");
-      return std::unique_ptr<MADtree>(new MADtree(icp_.context(), b_max_, b_min_));
-    }
-    if (gpu_build_ && records) {
-      check(madicp_ingest_points_t(icp_.context(), records, vc, tm, dsk ? 1 : 0, Ta, Tb, sensor_hz_,
-                                   std::max(1 << max_parallel_levels_, 1), nullptr, nullptr), "madicp_ingest_points");
-      return std::unique_ptr<MADtree>(new MADtree(icp_.context(), b_max_, b_min_));
-    }
     if (gpu_build_) {
-      check(madicp_ingest(icp_.context(), xyz, int64_t(n), is_f32 ? 1 : 0, dsk ? 1 : 0, Ta, Tb, sensor_hz_,
-                          std::max(1 << max_parallel_levels_, 1), nullptr), "madicp_ingest");
+      const int threads = std::max(1 << max_parallel_levels_, 1);
+      check(s.dev ? madicp_ingest_points_dev_t(icp_.context(), &s.pts, &s.vc, &s.tm, dsk ? 1 : 0, Ta, Tb, sensor_hz_, threads,
+                                               s.stream, nullptr, nullptr)
+                  : madicp_ingest_points_t(icp_.context(), &s.pts, &s.vc, &s.tm, dsk ? 1 : 0, Ta, Tb, sensor_hz_, threads,
+                                           nullptr, nullptr),
+            s.dev ? "madicp_ingest_points_dev" : "madicp_ingest_points");
       return std::unique_ptr<MADtree>(new MADtree(icp_.context(), b_max_, b_min_));
     }
-    const double* pts = static_cast<const double*>(xyz);
-    // keep_cloud: the record of every point of the tree's cloud (rec_idx: of every point of xyz; nullptr: xyz is the
-    // array the caller handed over)
-    std::vector<int32_t> idx;
+    HostCloud h = hostCloud(s);
+    const double* pts = h.xyz;
+    const size_t n = h.n;
     auto tree = [&](const double* cloud) {
       std::unique_ptr<MADtree> t(new MADtree(cloud, n, b_max_, b_min_, max_parallel_levels_));
-      if (keep_cloud_) t->keepHostCloud(cloud, n, std::move(idx));
+      if (keep_cloud_) t->keepHostCloud(cloud, n, std::move(h.idx));
       return t;
     };
-    if (keep_cloud_ && !(dsk && !(tm && records))) {  // (the azimuth deskew reorders: its indices come with its order)
-      idx.resize(n);
-      for (size_t i = 0; i < n; ++i) idx[i] = rec_idx ? rec_idx[i] : int32_t(i);
-    }
-    if (dsk && tm && records) {  // the host restatement of the time-stamp deskew (madicp_debug_time_chunks)
-      std::vector<uint16_t> chunk(size_t(records->n));
+    if (dsk && s.tm.type != madicp::kTimeNone) {  // the host restatement of the time-stamp deskew (madicp_debug_time_chunks)
+      std::vector<uint16_t> chunk(size_t(s.pts.n));
       int64_t kept = 0;
-      check(madicp_debug_time_chunks(records, vc, tm, sensor_hz_, chunk.data(), &kept), "madicp_debug_time_chunks");
+      check(madicp_debug_time_chunks(&s.pts, &s.vc, &s.tm, sensor_hz_, chunk.data(), &kept), "madicp_debug_time_chunks");
       if (size_t(kept) != n) throw Error("Pipeline.computeRecords: internal error (kept count)");
       std::vector<detail::Pose> poses(kChunks);
       check(madicp_debug_chunk_poses(Ta, Tb, sensor_hz_, kChunks, poses[0].m), "madicp_debug_chunk_poses");
@@ -519,11 +506,12 @@ class Pipeline {
       check(madicp_debug_deskew_plan(&d, nullptr, Ta, Tb, sensor_hz_, 0, 1 << max_parallel_levels_, perm.data(), chunk.data(),
                                      poses[0].m, &n_poses, &kept), "madicp_debug_deskew_plan");
       ContainerType cloud(n);
-      idx.resize(n);
+      std::vector<int32_t> idx(n);
       for (size_t i = 0; i < n; ++i) {
         madicp_pose::poseApply(poses[chunk[i]], pts + 3 * size_t(perm[i]), cloud[i].data());
-        idx[i] = rec_idx ? rec_idx[perm[i]] : perm[i];
+        idx[i] = h.idx[size_t(perm[i])];
       }
+      h.idx = std::move(idx);
       return tree(cloud[0].data());
     }
     if (dsk) {
@@ -535,18 +523,14 @@ class Pipeline {
     return tree(pts);
   }
 
-  // rec_idx (host-built trees, nullable): the record index of every point of xyz
-  void computeRaw(double stamp, const void* xyz, size_t n, bool is_f32, const madicp_points_t* records = nullptr,
-                  const madicp_vcorr_t* vc = nullptr, const DevScan* dev = nullptr, const madicp_times_t* tm = nullptr,
-                  const int32_t* rec_idx = nullptr) {
-    if (!xyz || n == 0) throw Error("Pipeline.compute: empty cloud");
+  void computeScan(double stamp, const Scan& s) {
     is_map_updated_ = false;
     if (!is_initialized_) {  // pipeline.cpp:267-284
       auto f = std::make_shared<FrameB>();
       f->frame = int(seq_);
       f->to_map = frame_to_map_;
       f->stamp = stamp;
-      f->tree = makeTree(xyz, n, is_f32, records, vc, dev, tm, rec_idx);
+      f->tree = makeTree(s);
       keyframes_.push_back(f);
       current_ = f;
       trajectory_.push_back(detail::poseIdentity());
@@ -557,7 +541,7 @@ class Pipeline {
     const auto c0 = clk();
     const auto c1 = c0;
     auto cur = std::make_shared<FrameB>();
-    cur->tree = makeTree(xyz, n, is_f32, records, vc, dev, tm, rec_idx);
+    cur->tree = makeTree(s);
     const auto c2 = clk();
     double t[3], w[3];
     for (int a = 0; a < 3; ++a) {
@@ -637,7 +621,7 @@ class Pipeline {
     return M;
   }
   // pipeline.cpp:79-123 on the host (madicp_deskew: threaded, same permutation and poses); the device path is
-  // madicp_ingest
+  // madicp_ingest_points_t
   static void deskew(ContainerType& cloud, const detail::Pose& T_prev, const detail::Pose& T_now, double sensor_hz,
                      int num_threads) {
     if (cloud.empty()) return;
@@ -647,7 +631,6 @@ class Pipeline {
   // the kept points of `pts` as a packed float64 cloud, corrected by `vc` (nullable), with the predicate and the
   // restatement the device applies (records.hpp); idx (nullable) receives the record index of every kept point
   static ContainerType packRecords(const madicp_points_t& pts, const madicp_vcorr_t* vc, std::vector<int32_t>* idx = nullptr) {
-    check(madicp::check_points(&pts, "Pipeline.computeRecords"), "Pipeline.computeRecords");
     madicp::VcorrTable table;
     const bool corrected = madicp::vcorr_of(vc).enabled != 0;
     if (corrected) madicp::vcorr_table_fill(vc->angle, &table);

@@ -10,47 +10,86 @@ static bool on_device(const py::object& o) { return py::hasattr(o, "__cuda_array
 // a device array copied to the host once (records.to_host), for host-built trees (MADICP_GPU_BUILD=0)
 static py::object to_host(const py::object& o) { return py::module_::import("mad_icp_b200.records").attr("to_host")(o); }
 
-// records (2-D float array with >= 3 columns, or 1-D structured with x/y/z; host or device memory) -> madicp_points_t, by
-// records.layout; dev receives the producer stream of device records (and is left alone for host records)
-static madicp_points_t records_arg(const py::object& records, double min_range, double max_range, bool inclusive,
-                                   bool drop_nan, mb::DevScan* dev = nullptr, bool* is_dev = nullptr) {
-  const py::tuple t = py::module_::import("mad_icp_b200.records")
-                          .attr("layout")(records, min_range, max_range, inclusive, drop_nan)
-                          .cast<py::tuple>();
-  if (is_dev) *is_dev = t[11].cast<bool>();
-  if (dev && t[11].cast<bool>()) dev->stream = reinterpret_cast<void*>(t[12].cast<uintptr_t>());
+// keeps a Python object alive until a queued scan is done with it (dropped on the thread that calls compute, with the
+// GIL held)
+static std::shared_ptr<void> keepalive(const py::object& o) {
+  return std::shared_ptr<void>(new py::object(o), [](void* q) { delete static_cast<py::object*>(q); });
+}
+
+// A scan as a Pipeline call takes it, and the Python object that keeps its memory alive
+struct ScanArg {
   madicp_points_t d{};
-  d.data = reinterpret_cast<const void*>(t[0].cast<uintptr_t>());
-  d.n = t[1].cast<int64_t>();
-  d.stride = t[2].cast<int64_t>();
-  for (int c = 0; c < 3; ++c) d.offset[c] = t[size_t(3 + c)].cast<int32_t>();
-  d.is_f32 = t[6].cast<int32_t>();
-  d.min_range = t[7].cast<double>();
-  d.max_range = t[8].cast<double>();
-  d.range_mode = t[9].cast<int32_t>();
-  d.drop_nan = t[10].cast<int32_t>();
-  return d;
-}
-
-// time_field / time_scale / time_end -> madicp_times_t (records.time_layout; type MADICP_TIME_NONE without a field)
-static madicp_times_t times_arg(const py::object& records, const py::object& field, double scale, const py::object& t_end) {
-  madicp_times_t t{};
-  if (field.is_none()) return t;
-  const py::tuple l = py::module_::import("mad_icp_b200.records").attr("time_layout")(records, field, scale, t_end).cast<py::tuple>();
-  t.offset = l[0].cast<int32_t>();
-  t.type = l[1].cast<int32_t>();
-  t.scale = l[2].cast<double>();
-  t.t_end = l[3].cast<double>();
-  t.has_t_end = l[4].cast<int32_t>();
-  return t;
-}
-
-// apply_correction / vertical_angle_offset (KittiReader's names) -> madicp_vcorr_t
-static madicp_vcorr_t vcorr_arg(bool apply_correction, double vertical_angle_offset) {
   madicp_vcorr_t v{};
-  v.angle = vertical_angle_offset;
-  v.enabled = apply_correction ? 1 : 0;
-  return v;
+  madicp_times_t t{};  // type MADICP_TIME_NONE without a time field
+  bool on_dev = false;
+  mb::DevScan dev;     // device records: the stream they are ready on
+  py::object hold;
+  const mb::DevScan* devScan() const { return on_dev ? &dev : nullptr; }
+  const madicp_times_t* times() const { return t.type ? &t : nullptr; }
+};
+
+// records (2-D float array with >= 3 columns, or 1-D structured with x/y/z; host or device memory) -> madicp_points_t, by
+// records.layout; apply_correction / vertical_angle_offset (KittiReader's names) -> madicp_vcorr_t; time_field /
+// time_scale / time_end -> madicp_times_t, by records.time_layout
+static ScanArg records_arg(const py::object& records, double min_range, double max_range, bool inclusive, bool drop_nan,
+                           bool apply_correction = false, double vertical_angle_offset = 0.0,
+                           const py::object& time_field = py::none(), double time_scale = 1.0,
+                           const py::object& time_end = py::none()) {
+  const py::module_ rec = py::module_::import("mad_icp_b200.records");
+  const py::tuple l = rec.attr("layout")(records, min_range, max_range, inclusive, drop_nan).cast<py::tuple>();
+  ScanArg r;
+  r.d.data = reinterpret_cast<const void*>(l[0].cast<uintptr_t>());
+  r.d.n = l[1].cast<int64_t>();
+  r.d.stride = l[2].cast<int64_t>();
+  for (int c = 0; c < 3; ++c) r.d.offset[c] = l[size_t(3 + c)].cast<int32_t>();
+  r.d.is_f32 = l[6].cast<int32_t>();
+  r.d.min_range = l[7].cast<double>();
+  r.d.max_range = l[8].cast<double>();
+  r.d.range_mode = l[9].cast<int32_t>();
+  r.d.drop_nan = l[10].cast<int32_t>();
+  r.on_dev = l[11].cast<bool>();
+  if (r.on_dev) r.dev.stream = reinterpret_cast<void*>(l[12].cast<uintptr_t>());
+  r.v.angle = vertical_angle_offset;
+  r.v.enabled = apply_correction ? 1 : 0;
+  if (!time_field.is_none()) {
+    const py::tuple t = rec.attr("time_layout")(records, time_field, time_scale, time_end).cast<py::tuple>();
+    r.t.offset = t[0].cast<int32_t>();
+    r.t.type = t[1].cast<int32_t>();
+    r.t.scale = t[2].cast<double>();
+    r.t.t_end = t[3].cast<double>();
+    r.t.has_t_end = t[4].cast<int32_t>();
+  }
+  r.hold = records;
+  return r;
+}
+
+// A compute / prefetch cloud, read where it is: a device array as records without a gate (for host-built trees it is
+// copied to the host first); in host memory a packed N x 3 cloud -- a bound VectorEigen3d by reference, a float32 array
+// as the dataset readers deliver it (the conversion to float64 runs on the device), any other array as C-contiguous
+// float64 (a view when it already is one)
+static ScanArg scan_arg(py::object cloud, bool gpu_build) {
+  if (on_device(cloud)) {
+    if (gpu_build) {
+      ScanArg r = records_arg(cloud, 0.0, std::numeric_limits<double>::infinity(), true, false);
+      r.d.range_mode = MADICP_RANGE_NONE;
+      return r;
+    }
+    cloud = to_host(cloud);
+  }
+  ScanArg r;
+  if (py::isinstance<mb::ContainerType>(cloud)) {
+    const mb::ContainerType& v = cloud.cast<const mb::ContainerType&>();
+    r.d = madicp::packed_points(v.empty() ? nullptr : v[0].data(), int64_t(v.size()), 0);
+    r.hold = cloud;
+    return r;
+  }
+  const bool f32 = py::isinstance<py::array>(cloud) && py::array::ensure(cloud).dtype().is(py::dtype::of<float>());
+  const py::array a = f32 ? py::array(cloud.cast<py::array_t<float, py::array::c_style | py::array::forcecast>>())
+                          : py::array(cloud.cast<NpArr>());
+  if (a.ndim() != 2 || a.shape(1) != 3) throw py::cast_error();
+  r.d = madicp::packed_points(a.shape(0) ? a.data() : nullptr, a.shape(0), f32 ? 1 : 0);
+  r.hold = a;
+  return r;
 }
 
 // currentLeaves (model == false) / modelLeaves as an (N, 3) float64 numpy array, or with `device` as a float64 CUDA tensor
@@ -139,32 +178,11 @@ PYBIND11_MODULE(pypeline, m) {
       .def("_leafMeansDev", [](const mb::Pipeline& p, bool model, uintptr_t out, uintptr_t stream) {
         p.leafMeansDev(model, reinterpret_cast<double*>(out), reinterpret_cast<void*>(stream));
       })
-      .def("compute", [](mb::Pipeline& p, double stamp, py::object cloud) {
-        // read the points where they are: a bound VectorEigen3d by reference, a numpy array through its buffer, a device
-        // array in place (as records without a gate)
-        if (on_device(cloud)) {
-          if (p.gpuBuild()) {
-            mb::DevScan dev;
-            madicp_points_t d = records_arg(cloud, 0.0, std::numeric_limits<double>::infinity(), true, false, &dev);
-            d.range_mode = MADICP_RANGE_NONE;
-            p.computeRecords(stamp, d, nullptr, &dev);
-            return;
-          }
-          cloud = to_host(cloud);
-        }
-        if (py::isinstance<mb::ContainerType>(cloud)) {
-          const mb::ContainerType& v = cloud.cast<const mb::ContainerType&>();
-          p.compute(stamp, v.empty() ? nullptr : v[0].data(), v.size());
-        } else if (py::isinstance<py::array>(cloud) && py::array::ensure(cloud).dtype().is(py::dtype::of<float>())) {
-          // float32 as the dataset readers deliver it: converted on the device (no host copy in float64)
-          const auto a = cloud.cast<py::array_t<float, py::array::c_style | py::array::forcecast>>();
-          if (a.ndim() != 2 || a.shape(1) != 3) throw py::cast_error();
-          p.computeF32(stamp, a.shape(0) ? a.data() : nullptr, size_t(a.shape(0)));
-        } else {
-          const NpArr a = cloud.cast<NpArr>();  // a view when the array already is C-contiguous float64
-          if (a.ndim() != 2 || a.shape(1) != 3) throw py::cast_error();
-          p.compute(stamp, a.shape(0) ? a.data() : nullptr, size_t(a.shape(0)));
-        }
+      .def("compute", [](mb::Pipeline& p, double stamp, const py::object& cloud) {
+        const ScanArg c = scan_arg(cloud, p.gpuBuild());
+        if (c.on_dev) p.computeRecords(stamp, c.d, nullptr, &c.dev);
+        else if (c.d.is_f32) p.computeF32(stamp, static_cast<const float*>(c.d.data), size_t(c.d.n));
+        else p.compute(stamp, static_cast<const double*>(c.d.data), size_t(c.d.n));
       })
       // additions (not in the reference): diagnostics
       .def_static("_deskewOnly", [](const py::object& cloud, const NpArr& a, const NpArr& b, double sensor_hz, int num_threads) {
@@ -172,30 +190,10 @@ PYBIND11_MODULE(pypeline, m) {
       }, py::arg("cloud"), py::arg("T_prev"), py::arg("T_now"), py::arg("sensor_hz"), py::arg("num_threads") = 1)
       .def("prefetch", [](mb::Pipeline& p, const py::object& cloud, bool deskew_ahead) {
         // the array is read in place when the batch is built (inside a later compute()): a reference keeps it alive
-        // until then (it is dropped there, on the calling thread, with the GIL held)
-        auto hold = [](const py::object& o) {
-          py::object* ref = new py::object(o);
-          return std::shared_ptr<void>(ref, [](void* q) { delete static_cast<py::object*>(q); });
-        };
-        if (on_device(cloud)) {  // (host-built trees: no look-ahead, as for host arrays)
-          if (!p.gpuBuild()) return false;
-          mb::DevScan dev;
-          madicp_points_t d = records_arg(cloud, 0.0, std::numeric_limits<double>::infinity(), true, false, &dev);
-          d.range_mode = MADICP_RANGE_NONE;
-          return p.prefetchRecords(d, hold(cloud), nullptr, deskew_ahead, &dev);
-        }
-        if (py::isinstance<mb::ContainerType>(cloud)) {
-          const mb::ContainerType& v = cloud.cast<const mb::ContainerType&>();
-          return p.prefetch(v.empty() ? nullptr : v[0].data(), v.size(), false, hold(cloud), nullptr, nullptr, deskew_ahead);
-        }
-        if (py::isinstance<py::array>(cloud) && py::array::ensure(cloud).dtype().is(py::dtype::of<float>())) {
-          const auto a = cloud.cast<py::array_t<float, py::array::c_style | py::array::forcecast>>();
-          if (a.ndim() != 2 || a.shape(1) != 3) throw py::cast_error();
-          return p.prefetch(a.data(), size_t(a.shape(0)), true, hold(a), nullptr, nullptr, deskew_ahead);
-        }
-        const NpArr a = cloud.cast<NpArr>();
-        if (a.ndim() != 2 || a.shape(1) != 3) throw py::cast_error();
-        return p.prefetch(a.data(), size_t(a.shape(0)), false, hold(a), nullptr, nullptr, deskew_ahead);
+        if (on_device(cloud) && !p.gpuBuild()) return false;  // (host-built trees: no look-ahead, as for host arrays)
+        const ScanArg c = scan_arg(cloud, true);
+        if (c.on_dev) return p.prefetchRecords(c.d, keepalive(c.hold), nullptr, deskew_ahead, &c.dev);
+        return p.prefetch(c.d.data, size_t(c.d.n), c.d.is_f32 != 0, keepalive(c.hold), nullptr, nullptr, deskew_ahead);
       }, py::arg("cloud"), py::arg("deskew_ahead") = false)
       // additions (not in the reference): raw sensor records, filtered on the way in like the dataset readers do
       // (mad_icp_b200/records.py describes the array; it is read in place); apply_correction: KITTI's vertical-angle
@@ -206,13 +204,10 @@ PYBIND11_MODULE(pypeline, m) {
       .def("computeRecords", [](mb::Pipeline& p, double stamp, const py::object& records, double min_range, double max_range,
                                 bool inclusive, bool drop_nan, bool apply_correction, double vertical_angle_offset,
                                 const py::object& time_field, double time_scale, const py::object& time_end) {
-        const madicp_vcorr_t v = vcorr_arg(apply_correction, vertical_angle_offset);
         const py::object recs = (on_device(records) && !p.gpuBuild()) ? to_host(records) : records;
-        mb::DevScan dev;
-        bool is_dev = false;
-        const madicp_points_t d = records_arg(recs, min_range, max_range, inclusive, drop_nan, &dev, &is_dev);
-        const madicp_times_t t = times_arg(recs, time_field, time_scale, time_end);
-        p.computeRecords(stamp, d, &v, is_dev ? &dev : nullptr, t.type ? &t : nullptr);
+        const ScanArg r = records_arg(recs, min_range, max_range, inclusive, drop_nan, apply_correction,
+                                      vertical_angle_offset, time_field, time_scale, time_end);
+        p.computeRecords(stamp, r.d, &r.v, r.devScan(), r.times());
       }, py::arg("stamp"), py::arg("records"), py::arg("min_range") = 0.0,
          py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false,
          py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle, py::arg("time_field") = py::none(),
@@ -223,14 +218,9 @@ PYBIND11_MODULE(pypeline, m) {
                                  bool inclusive, bool drop_nan, bool apply_correction, double vertical_angle_offset,
                                  bool deskew_ahead, const py::object& time_field, double time_scale, const py::object& time_end) {
         if (on_device(records) && !p.gpuBuild()) return false;  // (host-built trees: no look-ahead)
-        mb::DevScan dev;
-        bool is_dev = false;
-        const madicp_points_t d = records_arg(records, min_range, max_range, inclusive, drop_nan, &dev, &is_dev);
-        const madicp_vcorr_t v = vcorr_arg(apply_correction, vertical_angle_offset);
-        const madicp_times_t t = times_arg(records, time_field, time_scale, time_end);
-        py::object* ref = new py::object(records);  // dropped once the scan's tree is built (see prefetch)
-        return p.prefetchRecords(d, std::shared_ptr<void>(ref, [](void* q) { delete static_cast<py::object*>(q); }), &v,
-                                 deskew_ahead, is_dev ? &dev : nullptr, t.type ? &t : nullptr);
+        const ScanArg r = records_arg(records, min_range, max_range, inclusive, drop_nan, apply_correction,
+                                      vertical_angle_offset, time_field, time_scale, time_end);
+        return p.prefetchRecords(r.d, keepalive(r.hold), &r.v, deskew_ahead, r.devScan(), r.times());
       }, py::arg("records"), py::arg("min_range") = 0.0,
          py::arg("max_range") = std::numeric_limits<double>::infinity(), py::arg("inclusive") = true, py::arg("drop_nan") = false,
          py::arg("apply_correction") = false, py::arg("vertical_angle_offset") = kVerticalAngle, py::arg("deskew_ahead") = false,

@@ -188,6 +188,8 @@ static int configure_gn(madicp_ctx* c, int threads, int ctas) {
                               int((t[i].smem * size_t(ctas) + 2048) * 100 / (228 * 1024)) + 1));
       int per_sm = 0;
       CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, t[i].fn, threads, t[i].smem));
+      cudaFuncAttributes fa;
+      CK(cudaFuncGetAttributes(&fa, t[i].fn));
       if (per_sm < ctas) {
         set_error("persistent kernel shape does not fit on an SM");
         return MADICP_ERR_CUDA;
@@ -196,6 +198,7 @@ static int configure_gn(madicp_ctx* c, int threads, int ctas) {
       c->gn_grid = ctas * c->sm_count;
       c->gn_kernel = t[i].fn;
       c->gn_smem = t[i].smem;
+      c->gn_static_smem = fa.sharedSizeBytes;
       return MADICP_OK;
     }
   set_error("unsupported persistent-kernel shape (threads per CTA, CTAs per SM)");
@@ -1144,14 +1147,15 @@ static int register_enqueue(madicp_ctx* c, int iters, const double X0[12], int c
   size_t map_bytes = 0;
   {
     const size_t per_cta = gn_map_bytes(unsigned(madicp_num_keyframes(c)), unsigned(c->L), unsigned(c->gn_grid));
-    auto bucket = [](size_t bytes) {
+    const size_t ctas = size_t(c->gn_grid / c->sm_count);
+    auto bucket = [&](size_t dynamic) {  // every CTA of an SM: its dynamic and static shared memory + the 1 KB reserved per CTA
+      const size_t bytes = ctas * (dynamic + c->gn_static_smem + 1024);
       const size_t kb[] = {8, 16, 32, 64, 100, 132, 164, 196, 228};
       for (size_t b : kb)
-        if (bytes + 1024 <= b * 1024) return b;  // 1 KB of static shared memory + system reserve
+        if (bytes <= b * 1024) return b;
       return size_t(1 << 20);
     };
-    const size_t ctas = size_t(c->gn_grid / c->sm_count);
-    if (per_cta && bucket((c->gn_smem + per_cta) * ctas) == bucket(c->gn_smem * ctas)) map_bytes = per_cta;
+    if (per_cta && bucket(c->gn_smem + per_cta) == bucket(c->gn_smem)) map_bytes = per_cta;
   }
   A.map_in_smem = map_bytes ? 1 : 0;
   {  // path memo: one entry per CTA-local item

@@ -150,13 +150,17 @@ struct madicp_ctx {
   bool gn_auto = true;  // pick the shape per launch from the item count (pick_shape)
   int gn_threads = 1024;
   const void* gn_kernel = nullptr;
-  size_t gn_smem = 0;
+  size_t gn_smem = 0;         // dynamic shared memory of the shape (staging tiles), without the item map
+  size_t gn_static_smem = 0;  // static shared memory of its kernel
   // one-CTA-per-SM shapes the automatic choice considers, with the cost of one full pass of each (any unit):
   // a prior until madicp_calibrate measures them on the resident workload.  The prior: 10-round registrations of the
-  // bench workload (16 keyframes, 19 202 moving leaves) on an H100 SXM at a 400 W limit, time / passes, in 10 ns
-  static constexpr int kNumAutoShapes = 6;
-  static constexpr int kAutoShapes[kNumAutoShapes] = {768, 1024, 896, 704, 640, 512};
-  double pass_cost[kNumAutoShapes] = {5570.0, 8260.0, 7480.0, 5650.0, 5325.0, 4650.0};
+  // bench workload (16 keyframes, 19 202 moving leaves: 72.7 warp-items per SM) with L2 flushed before each, on an H100
+  // 80GB HBM3 (SXM) at a 700 W limit and 1980 MHz SM clock, median time / passes, in 10 ns (scripts/memo_probe.py).
+  // Only shapes without local-memory traffic in the item loop are listed (tests/test_gn_sass.py): 1024 x 1 keeps its
+  // DMMA accumulators in local memory at 64 registers, and ran at 6915 per pass.
+  static constexpr int kNumAutoShapes = 5;
+  static constexpr int kAutoShapes[kNumAutoShapes] = {768, 896, 704, 640, 512};
+  double pass_cost[kNumAutoShapes] = {4935.0, 6195.0, 5060.0, 4925.0, 4165.0};
   bool calibrated = false;
   int last_iters = 0;
   madicp::DevPtr<long long> d_dbg;  // MADICP_MAX_ITERS x 8 clock stamps when debug timing is on

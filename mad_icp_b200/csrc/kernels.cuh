@@ -42,7 +42,7 @@ namespace madicp {
 constexpr int kMaxSlots = 64;     // keyframe slots addressable by one launch
 constexpr int kStepBlock = 256;   // threads per CTA of the step-API kernels (K1, K2, tools)
 constexpr int kAcc = 48;          // 6 rows x 8 cols accumulator tile: H(r,c) at r*8+c, b(r) at r*8+6
-constexpr int kStage = 13;        // doubles staged per correspondence: sJ[6], J[6], e
+constexpr int kStage = 8;         // doubles staged per correspondence: J[6], e, scale
 constexpr int kStageItems = 16;   // correspondences staged per DMMA pass (half a warp)
 constexpr int kStagePitch = 20;   // doubles per staged value row (16 items + 4 padding: conflict-free)
 constexpr int kStageTile = kStage * kStagePitch;  // doubles of shared memory per warp
@@ -365,8 +365,8 @@ __device__ __forceinline__ int descend(const ModelView& M, int k, double qx, dou
 }
 
 // One correspondence (reference: odometry/mad_icp.cpp:81-101): gate, error, Jacobian, Huber scale,
-// planarity weight.  Fills v = {sJ[0..5] = scale*J, J[0..5], e}; returns false (v untouched) when
-// the gate rejects the pair.
+// planarity weight.  Fills v = {J[0..5], e, scale}; returns false (v untouched) when the gate rejects the pair.
+// scale*J is formed where warp_accumulate loads the A fragment: the same single product, ten fewer live doubles.
 //   * The gate `|ml - f.mean| > ball` decides a flag (matched_) and a discontinuous contribution, so
 //     it is evaluated exactly as the reference does (FP64, no FMA); the square root is only taken
 //     when d^2 is within 1e-14 (relative) of ball^2, where the comparison of squares could disagree
@@ -394,28 +394,27 @@ __device__ __forceinline__ bool linearize_one(const double* __restrict__ X, doub
   const double chi = fabs(e);
   if (chi > rho) scale = (rho / chi) * ww;
 #pragma unroll
-  for (int i = 0; i < 6; ++i) {
-    v[i] = scale * J[i];
-    v[6 + i] = J[i];
-  }
-  v[12] = e;
+  for (int i = 0; i < 6; ++i) v[i] = J[i];
+  v[6] = e;
+  v[7] = scale;
   return true;
 }
 
 // H += sJ^T J, b += sJ^T e for the 32 correspondences a warp holds, on the FP64 tensor pipe:
-// D(8x8) += A(8x4) * B(4x8) with A[r][k] = sJ_r(item k), B[k][c] = J_c(item k) (c<6), e(item k)
+// D(8x8) += A(8x4) * B(4x8) with A[r][k] = scale(item k) * J_r(item k), B[k][c] = J_c(item k) (c<6), e(item k)
 // (c==6), zero padding elsewhere -- 8 DMMA.8x8x4 per 32 items, staged through shared memory in two
 // half-warp passes.  The point is not FLOPs (there are few) but registers: the running sums are the
 // 2-double C fragment instead of 42 scalars per thread, which keeps the kernel at 64 registers
 // (1024 resident threads per SM for the latency-bound walk).  H(r,c) = sum (scale*J_r)*J_c is
 // formed for both triangles independently, like the reference's `scale * J.transpose() * J`.
-// stage: this warp's [kStageItems][kStage] doubles.  v: this lane's 13 values (zeros if none).
+// stage: this warp's [kStage][kStagePitch] doubles.  v: this lane's kStage values (zeros if none).
 __device__ __forceinline__ void warp_accumulate(double* stage, const double* v, double& c0, double& c1) {
   const int lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
-  // tile layout [value 0..12][item 0..15, padded to kStagePitch]: value-major with a pitch of 20
-  // doubles makes both the stores (lanes = consecutive items) and the fragment loads
-  // (bank = 4g + t + 4s mod 16) conflict-free.
+  // tile layout [value 0..7][item 0..15, padded to kStagePitch]: value-major with a pitch of 20
+  // doubles makes both the stores (lanes = consecutive items) and the fragment loads conflict-free: a
+  // 64-bit access is served per half-warp, and lanes (g, t) of one half (g = 0..3 or 4..7) hit the
+  // 8-byte bank 4g + t + 4s mod 16 -- sixteen distinct banks; the scale row is one broadcast per t.
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     if ((lane >> 4) == h) {
@@ -426,8 +425,8 @@ __device__ __forceinline__ void warp_accumulate(double* stage, const double* v, 
 #pragma unroll
     for (int s = 0; s < 4; ++s) {
       const double* it = stage + (4 * s + t);
-      const double a = (g < 6) ? it[g * kStagePitch] : 0.0;                          // rows 6,7 of A are padding
-      const double b = (g < 7) ? it[(6 + (g < 7 ? g : 6)) * kStagePitch] : 0.0;      // col 6 of B = e, col 7 padding
+      const double b = (g < 7) ? it[g * kStagePitch] : 0.0;           // col 6 of B = e, col 7 padding
+      const double a = (g < 6) ? it[7 * kStagePitch] * b : 0.0;        // scale * J_g; rows 6,7 of A are padding
       asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
                    : "+d"(c0), "+d"(c1)
                    : "d"(a), "d"(b));

@@ -194,6 +194,39 @@ int64_t madtree_gpu_cloud_dev(const madtree_gpu_t* t, const double X[12], double
                               void* consumer_stream);
 /* Gives the tree's kept cloud back to the context's cache (no-op without one).  Freeing the tree does too. */
 int madtree_gpu_release_cloud(madtree_gpu_t* t);
+
+/* ---------------- voxel map of the kept clouds (not in the reference) ---------------------------------------------
+ * A map of every inserted scan, built on the device of one context.  Voxel of a point p: (floor(p.x / v), floor(p.y / v),
+ * floor(p.z / v)) in IEEE float64; each component must lie in (-2^20, 2^20).  A voxel keeps the first points_per_voxel
+ * (K, 1..32) points that reach it: scans count in insertion order, points within a scan in kept-cloud order, later ones
+ * are discarded.  Points with a key out of range or a non-finite coordinate are skipped and counted (`dropped`).  The
+ * map's rows are in acceptance order (by insert, then by kept-cloud position), each with (scan, record): the caller's
+ * scan number and the point's record index (madtree_gpu_cloud's idx_out).  Nothing observable depends on hash-slot
+ * placement or on the order of atomics: the same inserts give the same bits. */
+typedef struct madicp_map madicp_map_t;
+/* Not in the reference.  voxel_size v: finite and > 0; reserve_points: rows (and voxels) to allocate up front (0: sized
+ * by the first insert).  The map grows by doubling; the table is rehashed on the device without changing any row. */
+int madicp_map_create(madicp_ctx_t* ctx, double voxel_size, int points_per_voxel, int64_t reserve_points,
+                      madicp_map_t** out);
+/* Not in the reference.  Waits for the context's stream, then frees the map.  Free maps before their context. */
+int madicp_map_free(madicp_map_t* map);
+/* Not in the reference.  Inserts the kept cloud of `tree` (a tree of the map's context, built with madicp_set_keep_cloud
+ * on), posed by X as madtree_gpu_cloud poses it (NULL: untouched, -0.0 stays -0.0), its points tagged with `scan`.  Runs
+ * on the context's stream and never waits on the host, except to grow the map.  MADICP_ERR_STATE for a tree that kept
+ * no cloud; MADICP_ERR_INVALID for a tree of another context. */
+int madicp_map_insert(madicp_map_t* map, const madtree_gpu_t* tree, const double X[12], int64_t scan);
+/* Not in the reference.  Waits for the context's stream; returns the number of rows M, and the skipped points in
+ * *dropped (nullable). */
+int64_t madicp_map_size(madicp_map_t* map, int64_t* dropped);
+/* Not in the reference.  The rows into host memory: xyz M x 3 doubles, scan_record M x 2 int64 (scan, record); either may
+ * be NULL, not both.  Synchronises.  Returns M. */
+int64_t madicp_map_points(madicp_map_t* map, double* xyz, int64_t* scan_record);
+/* Not in the reference.  The same into device memory of the map's device (8-byte aligned), ordered like
+ * madtree_gpu_cloud_dev: the context's stream waits for consumer_stream, the rows are ready on consumer_stream with no
+ * host sync.  Learning M waits for the context's stream unless madicp_map_size already did. */
+int64_t madicp_map_points_dev(madicp_map_t* map, double* xyz, int64_t* scan_record, void* consumer_stream);
+/* Not in the reference.  Empties the map (keeping its memory); later inserts start a new one.  Synchronises. */
+int madicp_map_clear(madicp_map_t* map);
 /* Audit dump of a DEVICE-BUILT tree in breadth-first order: mean n x 3, eigenvectors n x 9 (column-major), bbox
  * n x 3, num_points n (any may be NULL).  Valid for the most recently built tree of the context.  Synchronises. */
 int madtree_gpu_export(const madtree_gpu_t* t, double* mean, double* eigenvectors, double* bbox, int32_t* num_points);

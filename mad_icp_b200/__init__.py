@@ -5,6 +5,6 @@ classes and pybind modules with the reference's names: pymadtree, pymadicp, pype
 csrc/adapter/ (backend TU the reference's own Pipeline links against), engine.py (ctypes handles used by the
 tests and bench.py), distributed.py (multi-GPU plumbing), synth.py (synthetic inputs).
 """
-from .engine import DeskewPlan, DeviceTree, FlatTree, Registrar, MadIcpError  # noqa: F401
+from .engine import DeskewPlan, DeviceTree, FlatTree, Registrar, MadIcpError, VoxelMap  # noqa: F401
 
 __version__ = "0.1.0"

@@ -117,6 +117,13 @@ SYMBOLS = {
     "madtree_gpu_cloud": (C.c_int64, [vp, dp, dp, C.POINTER(C.c_int64)]),
     "madtree_gpu_cloud_dev": (C.c_int64, [vp, dp, vp, vp, vp]),
     "madtree_gpu_release_cloud": (C.c_int, [vp]),
+    "madicp_map_create": (C.c_int, [vp, C.c_double, C.c_int, C.c_int64, C.POINTER(vp)]),
+    "madicp_map_free": (C.c_int, [vp]),
+    "madicp_map_insert": (C.c_int, [vp, vp, dp, C.c_int64]),
+    "madicp_map_size": (C.c_int64, [vp, C.POINTER(C.c_int64)]),
+    "madicp_map_points": (C.c_int64, [vp, dp, C.POINTER(C.c_int64)]),
+    "madicp_map_points_dev": (C.c_int64, [vp, vp, vp, vp]),
+    "madicp_map_clear": (C.c_int, [vp]),
     "madicp_debug_deskew_plan": (C.c_int, [pts_p, vc_p, dp, dp, C.c_double, C.c_int, C.c_int, ip,
                                            C.POINTER(C.c_uint16), dp, C.POINTER(C.c_int), C.POINTER(C.c_int64)]),
     "madicp_register_fetch_weight": (C.c_int, [vp, dp, dp, dp, bp, C.POINTER(C.c_int), dp]),

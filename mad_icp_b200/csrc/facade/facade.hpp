@@ -229,6 +229,41 @@ class MADtree {
   std::vector<int32_t> host_idx_;
 };
 
+// A voxel map of kept clouds on one context (madicp_map_*, not in the reference): owns the map and frees it.  Trees must be
+// device trees of that context, built with madicp_set_keep_cloud on.
+class VoxelMap {
+ public:
+  VoxelMap(madicp_ctx_t* ctx, double voxel_size, int points_per_voxel, int64_t reserve_points = 0) {
+    check(madicp_map_create(ctx, voxel_size, points_per_voxel, reserve_points, &m_), "madicp_map_create");
+  }
+  ~VoxelMap() { madicp_map_free(m_); }
+  VoxelMap(const VoxelMap&) = delete;
+  VoxelMap& operator=(const VoxelMap&) = delete;
+
+  // the tree's kept cloud, posed by its pose (none: untouched), its points tagged with `scan`
+  void insert(const MADtree& t, int64_t scan) {
+    if (!t.deviceHandle()) throw Error("VoxelMap.insert: the map takes device trees");
+    check(int(std::min<int64_t>(0, madicp_map_insert(m_, t.deviceHandle(), t.pose(), scan))), "madicp_map_insert");
+  }
+  size_t size(int64_t* dropped = nullptr) {
+    const int64_t n = madicp_map_size(m_, dropped);
+    check(int(std::min<int64_t>(0, n)), "madicp_map_size");
+    return size_t(n);
+  }
+  // host output (either nullable): size() x 3 doubles, size() x 2 int64 (scan, record)
+  void points(double* xyz, int64_t* scan_record) {
+    check(int(std::min<int64_t>(0, madicp_map_points(m_, xyz, scan_record))), "madicp_map_points");
+  }
+  // device output of the context's device, ready on consumer_stream with no host sync
+  void pointsDev(double* xyz, int64_t* scan_record, void* consumer_stream) {
+    check(int(std::min<int64_t>(0, madicp_map_points_dev(m_, xyz, scan_record, consumer_stream))), "madicp_map_points_dev");
+  }
+  void clear() { check(madicp_map_clear(m_), "madicp_map_clear"); }
+
+ private:
+  madicp_map_t* m_ = nullptr;
+};
+
 // reference: class MADicp (odometry/mad_icp.h:41-79).  `update(tree)` under the reference's OpenMP loop
 // becomes "make this keyframe resident and part of the next round" (thread-safe); `updateState()` runs the round
 // on the device (search + linearise + reduce + solve).  `compute(iters)` is the whole loop in one launch.

@@ -237,7 +237,8 @@ class Pipeline {
   static constexpr int kMaxIcpIts = 15, kSmoothingT = 10, kFrameWindow = 10, kChunks = 1024;  // tools/constants.h
 
   Pipeline(double sensor_hz, bool deskew, double b_max, double rho_ker, double p_th, double b_min, double b_ratio,
-           int num_keyframes, int num_threads, bool realtime, int device = -1, bool keep_cloud = false)
+           int num_keyframes, int num_threads, bool realtime, int device = -1, bool keep_cloud = false,
+           double map_voxel_size = 0.0, int map_points_per_voxel = 1)
       : sensor_hz_(sensor_hz), deskew_(deskew), b_max_(b_max), p_th_(p_th), b_min_(b_min), num_keyframes_(num_keyframes),
         realtime_(realtime), keep_cloud_(keep_cloud),
         icp_(b_max, rho_ker, b_ratio, num_threads, resolveDevice(device), std::max(num_keyframes, 1)), vel_(sensor_hz) {
@@ -245,6 +246,14 @@ class Pipeline {
     device_ = resolveDevice(device);
     if (keep_cloud_) check(madicp_set_keep_cloud(icp_.context(), 1), "madicp_set_keep_cloud");
     if (const char* e = std::getenv("MADICP_GPU_BUILD")) gpu_build_ = std::atoi(e) != 0;
+    if (!(map_voxel_size >= 0.0) || !std::isfinite(map_voxel_size))
+      throw Error("Pipeline: map_voxel_size must be finite and >= 0 (0: no map)");
+    if (map_points_per_voxel < 1 || map_points_per_voxel > 32) throw Error("Pipeline: map_points_per_voxel must lie in [1, 32]");
+    if (map_voxel_size > 0.0) {  // the map inserts each scan's kept cloud: every tree keeps one
+      if (!gpu_build_) throw Error("Pipeline: a map (map_voxel_size > 0) needs device-built trees (MADICP_GPU_BUILD)");
+      check(madicp_set_keep_cloud(icp_.context(), 1), "madicp_set_keep_cloud");
+      map_.reset(new VoxelMap(icp_.context(), map_voxel_size, map_points_per_voxel));
+    }
     num_threads_ = std::max(num_threads, 1);
     int lvl = 0;
     while ((1 << (lvl + 1)) <= std::max(num_threads, 1)) ++lvl;
@@ -302,6 +311,21 @@ class Pipeline {
   void cloudDev(bool map, double* xyz_out, int64_t* idx_out, void* consumer_stream) const {
     if (requireCloud()) current_->tree->cloudDev(map, xyz_out, idx_out, consumer_stream);
   }
+  // The voxel map of every scan so far (map_voxel_size > 0; not in the reference): each scan's kept cloud in the map
+  // frame, the rows currentCloud(map) hands out, inserted once its pose is known; a voxel keeps the first
+  // map_points_per_voxel points that reach it.  Rows in acceptance order with (scan, record): the scan's currentID()
+  // before it was computed and the point's currentCloudIndices() value.
+  size_t mapSize() { return requireMap().size(); }
+  int64_t mapDropped() {
+    int64_t dropped = 0;
+    requireMap().size(&dropped);
+    return dropped;
+  }
+  void mapPoints(double* xyz, int64_t* scan_record) { requireMap().points(xyz, scan_record); }
+  void mapPointsDev(double* xyz, int64_t* scan_record, void* consumer_stream) {
+    requireMap().pointsDev(xyz, scan_record, consumer_stream);
+  }
+  void clearMap() { requireMap().clear(); }
 
   // test hook: the deskew step alone (poses 4x4 row-major)
   static ContainerType deskewOnly(ContainerType cloud, const Matrix4d& T_prev, const Matrix4d& T_now, double sensor_hz,
@@ -418,6 +442,10 @@ class Pipeline {
     s.records = true;
     return s;
   }
+  VoxelMap& requireMap() const {
+    if (!map_) throw Error("Pipeline.map: the pipeline builds no map (construct it with map_voxel_size > 0)");
+    return *map_;
+  }
   // whether there is a current scan whose cloud can be read (throws without keep_cloud)
   bool requireCloud() const {
     if (!keep_cloud_) throw Error("Pipeline.currentCloud: the pipeline keeps no cloud (construct it with keep_cloud=True)");
@@ -531,6 +559,7 @@ class Pipeline {
       f->to_map = frame_to_map_;
       f->stamp = stamp;
       f->tree = makeTree(s);
+      if (map_) map_->insert(*f->tree, int64_t(seq_));  // (no pose: the sensor frame is the map frame)
       keyframes_.push_back(f);
       current_ = f;
       trajectory_.push_back(detail::poseIdentity());
@@ -581,7 +610,8 @@ class Pipeline {
     cur->weight = (iters > 0 && iters <= MADICP_MAX_ITERS) ? icp_.weight()                        // :223, from the device
                                                            : detail::inverseDeterminant(icp_.H_adder_);
     cur->tree->applyTransform(toM(frame_to_map_));             // :224
-    if (current_ && keep_cloud_) current_->tree->releaseCloud();  // (only the current scan's cloud is kept)
+    if (map_) map_->insert(*cur->tree, int64_t(seq_));
+    if (current_ && (keep_cloud_ || map_)) current_->tree->releaseCloud();  // (only the current scan's cloud is kept)
     current_ = cur;
     frames_.push_back(cur);
     if (frames_.size() > size_t(kFrameWindow)) frames_.pop_front();
@@ -673,6 +703,7 @@ class Pipeline {
   double round_ms_ = 0.0;   // duration of one GN round on the previous scan (realtime budget)
   MADicp icp_;
   std::unique_ptr<Lookahead> lookahead_;  // declared after icp_: destroyed first (its lanes use icp_'s context)
+  std::unique_ptr<VoxelMap> map_;         // (map_voxel_size > 0) likewise after icp_
   detail::VelocityEstimator vel_;
   detail::Pose frame_to_map_, keyframe_to_map_;
   std::deque<std::shared_ptr<FrameB>> keyframes_, frames_;

@@ -127,6 +127,19 @@ static py::object cloud_indices(const py::object& self, bool device) {
   return std::move(out);
 }
 
+// mapArray / mapIndices as numpy arrays, or with `device` as CUDA tensors on the pipeline's device, ready on torch's current
+// stream (records.map_array_dev)
+static py::object map_array(const py::object& self, bool device, bool indices) {
+  if (device) return py::module_::import("mad_icp_b200.records").attr("map_array_dev")(self, indices);
+  mb::Pipeline& p = self.cast<mb::Pipeline&>();
+  const size_t n = p.mapSize();
+  py::array_t<double> xyz({indices ? size_t(0) : n, size_t(3)});
+  py::array_t<int64_t> sr({indices ? n : size_t(0), size_t(2)});
+  if (n) p.mapPoints(indices ? nullptr : xyz.mutable_data(), indices ? sr.mutable_data() : nullptr);
+  if (indices) return std::move(sr);
+  return std::move(xyz);
+}
+
 PYBIND11_MODULE(pypeline, m) {
   bind_vector_eigen3d(m);
   // KittiReader.vertical_angle_offset, np.radians(0.205), as records.py computes it: the default bit for bit
@@ -134,14 +147,17 @@ PYBIND11_MODULE(pypeline, m) {
   py::class_<mb::Pipeline>(m, "Pipeline")
       // keep_cloud (not in the reference): the current scan's deskewed cloud and its record indices stay available
       // (currentCloudArray / currentCloudIndices)
+      // map_voxel_size > 0 (not in the reference): a voxel map of every scan builds itself on the device, keeping the
+      // first map_points_per_voxel points of each voxel (mapArray / mapIndices)
       .def(py::init([](double sensor_hz, bool deskew, double b_max, double rho_ker, double p_th, double b_min, double b_ratio,
-                       int num_keyframes, int num_threads, bool realtime, bool keep_cloud) {
+                       int num_keyframes, int num_threads, bool realtime, bool keep_cloud, double map_voxel_size,
+                       int map_points_per_voxel) {
              return new mb::Pipeline(sensor_hz, deskew, b_max, rho_ker, p_th, b_min, b_ratio, num_keyframes, num_threads,
-                                     realtime, -1, keep_cloud);
+                                     realtime, -1, keep_cloud, map_voxel_size, map_points_per_voxel);
            }),
            py::arg("sensor_hz"), py::arg("deskew"), py::arg("b_max"), py::arg("rho_ker"), py::arg("p_th"), py::arg("b_min"),
            py::arg("b_ratio"), py::arg("num_keyframes"), py::arg("num_threads"), py::arg("realtime"),
-           py::arg("keep_cloud") = false)
+           py::arg("keep_cloud") = false, py::arg("map_voxel_size") = 0.0, py::arg("map_points_per_voxel") = 1)
       .def("currentPose", [](const mb::Pipeline& p) { return pose_to_numpy(p.currentPose()); })
       .def("trajectory",
            [](const mb::Pipeline& p) {
@@ -168,6 +184,18 @@ PYBIND11_MODULE(pypeline, m) {
            }, py::arg("device") = false, py::arg("frame") = "map")
       .def("currentCloudIndices", [](const py::object& self, bool device) { return cloud_indices(self, device); },
            py::arg("device") = false)
+      // the voxel map (map_voxel_size > 0): its points in the map frame (M, 3) float64, and (scan, record) per point
+      // (M, 2) int64 -- scan: currentID() before that scan was computed, record: its currentCloudIndices() value
+      .def("mapSize", &mb::Pipeline::mapSize)
+      .def("mapArray", [](const py::object& self, bool device) { return map_array(self, device, false); },
+           py::arg("device") = false)
+      .def("mapIndices", [](const py::object& self, bool device) { return map_array(self, device, true); },
+           py::arg("device") = false)
+      .def("mapDropped", &mb::Pipeline::mapDropped)
+      .def("clearMap", &mb::Pipeline::clearMap)
+      .def("_mapDev", [](mb::Pipeline& p, uintptr_t xyz, uintptr_t sr, uintptr_t stream) {
+        p.mapPointsDev(reinterpret_cast<double*>(xyz), reinterpret_cast<int64_t*>(sr), reinterpret_cast<void*>(stream));
+      })
       .def("_numCloudPoints", &mb::Pipeline::numCloudPoints)
       .def("_kernelLaunches", &mb::Pipeline::kernelLaunches)
       .def("_cloudDev", [](const mb::Pipeline& p, bool map, uintptr_t xyz, uintptr_t idx, uintptr_t stream) {

@@ -22,6 +22,7 @@
 #include "../../include/madicp_b200.h"
 #include "arith.h"
 #include "eig3.h"
+#include "tile_scan.cuh"
 #include "range_gate.h"
 #include "time_deskew.h"
 #include "vertical_correction.h"
@@ -33,7 +34,6 @@ constexpr int kBlock = 256;
 // The in-order sums are the long-running kernels of a build (one dependent FP64 add per point and chain): small CTAs,
 // many per SM, so that every node (k_sums_big) / every four nodes (k_sums_small) of a level have a CTA of their own.
 constexpr int kSumsBlock = 128;
-constexpr int kTile = 1024;  // positions per CTA of the flag scan
 
 // per-node data kept for the whole build (index = breadth-first node id)
 struct Nodes {
@@ -567,75 +567,13 @@ __global__ void k_advance(const Work W) {
   }
 }
 
-// (7) exclusive prefix of the side flags over the whole array: per-tile scan + scan of the tile totals
-__device__ __forceinline__ void scan_tiles_body(const unsigned char* __restrict__ flag, int n, int* __restrict__ G,
-                                                int* __restrict__ tile_sum) {
-  __shared__ int s_warp[32];
-  const int i = blockIdx.x * kTile + threadIdx.x;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int f = (i < n) ? int(flag[i]) : 0;
-  int incl = f;
-#pragma unroll
-  for (int off = 1; off < 32; off <<= 1) {
-    const int v = __shfl_up_sync(0xffffffffu, incl, off);
-    if (lane >= off) incl += v;
-  }
-  if (lane == 31) s_warp[warp] = incl;
-  __syncthreads();
-  if (warp == 0) {
-    int w = s_warp[lane];
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int v = __shfl_up_sync(0xffffffffu, w, off);
-      if (lane >= off) w += v;
-    }
-    s_warp[lane] = w;
-  }
-  __syncthreads();
-  const int excl = (warp ? s_warp[warp - 1] : 0) + incl - f;
-  if (i < n) G[i] = excl;
-  if (threadIdx.x == kTile - 1) tile_sum[blockIdx.x] = excl + f;
-}
+// (7) exclusive prefix of the side flags over the whole array: per-tile scan + scan of the tile totals (tile_scan.cuh)
 __global__ void __launch_bounds__(kTile)
 k_scan_tiles(const unsigned char* __restrict__ flag, int n, int* __restrict__ G, int* __restrict__ tile_sum) {
   scan_tiles_body(flag, n, G, tile_sum);
 }
 __global__ void __launch_bounds__(kTile) k_scan_tiles_lvl(const Work W) { scan_tiles_body(W.flag, W.lvl->n_points, W.G, W.tile); }
 
-__device__ __forceinline__ void scan_tile_sums_body(int* __restrict__ tile_sum, int n_tiles) {  // in place: exclusive; one CTA
-  __shared__ int s_warp[32];
-  __shared__ int s_carry;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) s_carry = 0;
-  __syncthreads();
-  for (int base = 0; base < n_tiles; base += 1024) {
-    const int t = base + threadIdx.x;
-    const int v0 = (t < n_tiles) ? tile_sum[t] : 0;
-    int incl = v0;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int v = __shfl_up_sync(0xffffffffu, incl, off);
-      if (lane >= off) incl += v;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      int w = s_warp[lane];
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const int v = __shfl_up_sync(0xffffffffu, w, off);
-        if (lane >= off) w += v;
-      }
-      s_warp[lane] = w;
-    }
-    __syncthreads();
-    const int excl = s_carry + (warp ? s_warp[warp - 1] : 0) + incl - v0;
-    if (t < n_tiles) tile_sum[t] = excl;
-    __syncthreads();
-    if (threadIdx.x == 1023) s_carry = excl + v0;
-    __syncthreads();
-  }
-}
 __global__ void __launch_bounds__(1024) k_scan_tile_sums(int* __restrict__ tile_sum, int n_tiles) {
   scan_tile_sums_body(tile_sum, n_tiles);
 }

@@ -1,0 +1,318 @@
+// voxel_map.cu -- madicp_map_* (include/madicp_b200.h): a voxel map of every inserted kept cloud, built on the device.
+// The kernels and the acceptance rule are in voxel_map_kernels.cuh.  An insert runs on the context's stream and never
+// waits on the host: the capacity it needs is bounded from the counters the previous inserts left in mapped memory, and
+// the host synchronises only when that bound outgrows the allocations (the map then grows by doubling).
+#include <cuda_runtime.h>
+
+#include <atomic>
+#include <cmath>
+#include <cstring>
+#include <string>
+
+#include "ctx.hpp"
+#include "voxel_map_kernels.cuh"
+
+using namespace madicp;
+
+struct madicp_map {
+  madicp_ctx* ctx = nullptr;
+  double v = 0.0;
+  int K = 1;
+  // the hash table: packed keys, accepted points per voxel, round words (K > 1: two arrays, by round parity)
+  size_t slots = 0;
+  DevPtr<unsigned long long> keys, win;
+  DevPtr<int> cnt;
+  // dense rows in acceptance order
+  size_t cap_points = 0;
+  DevPtr<double> xyz;
+  DevPtr<long long> sr;
+  // per-point scratch of one insert
+  size_t cap_scratch = 0;
+  DevPtr<int> slot, G, tile;
+  DevPtr<unsigned char> flag;
+  DevPtr<vmap::State> st;
+  HostPtr<vmap::Mirror> mirror;  // mapped
+  vmap::Mirror* d_mirror = nullptr;
+  uint64_t inserts = 0;  // inserts enqueued
+  int64_t points_in = 0;  // points handed to them
+  // the counters as of the last insert the host has seen complete, and points_in at that time
+  int64_t known_M = 0, known_V = 0, known_dropped = 0, known_in = 0;
+  uint32_t rounds = 0;  // acceptance rounds so far (tags 0xFFFFFFFF - round)
+};
+
+namespace {
+
+int map_error(const char* fn, const std::string& msg) {
+  set_error(std::string(fn) + ": " + msg);
+  return MADICP_ERR_INVALID;
+}
+
+// takes the mirror's counters when they belong to the last insert enqueued
+void refresh(madicp_map* m) {
+  const volatile vmap::Mirror* h = m->mirror.get();
+  if (h->seq != m->inserts) return;
+  std::atomic_thread_fence(std::memory_order_acquire);
+  m->known_M = h->M;
+  m->known_V = h->V;
+  m->known_dropped = h->dropped;
+  m->known_in = m->points_in;
+}
+
+// the map's counters exactly: waits for the context's stream when the last insert may still run
+int settle(madicp_map* m) {
+  refresh(m);
+  if (m->known_in != m->points_in) {
+    CK(cudaStreamSynchronize(m->ctx->stream));
+    refresh(m);
+  }
+  if (m->known_in != m->points_in) {
+    set_error("voxel map: the counters of the last insert did not arrive");
+    return MADICP_ERR_CUDA;
+  }
+  return MADICP_OK;
+}
+
+size_t pow2_at_least(size_t n) {
+  size_t p = 1;
+  while (p < n) p <<= 1;
+  return p;
+}
+
+// an empty table of `slots` slots (a power of two), with the round words reset
+int alloc_table(madicp_map* m, size_t slots, DevPtr<unsigned long long>* keys, DevPtr<int>* cnt,
+                DevPtr<unsigned long long>* win) {
+  cudaStream_t s = m->ctx->stream;
+  const size_t words = slots * (m->K > 1 ? 2 : 1);
+  CK(cudaMalloc(keys->put(), slots * sizeof(unsigned long long)));
+  CK(cudaMalloc(cnt->put(), slots * sizeof(int)));
+  CK(cudaMalloc(win->put(), words * sizeof(unsigned long long)));
+  CK(cudaMemsetAsync(keys->get(), 0xff, slots * sizeof(unsigned long long), s));
+  CK(cudaMemsetAsync(cnt->get(), 0, slots * sizeof(int), s));
+  CK(cudaMemsetAsync(win->get(), 0xff, words * sizeof(unsigned long long), s));
+  return MADICP_OK;
+}
+
+// Room for `points` more rows and voxels after everything enqueued so far: a bound from the last counters the host has
+// seen, exact after a synchronisation that only a growth needs.  Growth doubles; the table is rehashed on the device.
+int reserve(madicp_map* m, int64_t points) {
+  refresh(m);
+  auto fits = [&] {
+    const int64_t pending = m->points_in - m->known_in + points;
+    return size_t(m->known_M + pending) <= m->cap_points && 2 * size_t(m->known_V + pending) <= m->slots &&
+           size_t(points) <= m->cap_scratch;
+  };
+  if (fits()) return MADICP_OK;
+  cudaStream_t s = m->ctx->stream;
+  if (int rc = settle(m)) return rc;  // (the stream is idle from here on: buffers can be replaced)
+  const size_t need_M = size_t(m->known_M + points), need_V = size_t(m->known_V + points);
+  if (need_M > m->cap_points) {
+    size_t cap = m->cap_points ? m->cap_points : size_t(points);
+    while (cap < need_M) cap <<= 1;
+    DevPtr<double> xyz;
+    DevPtr<long long> sr;
+    CK(cudaMalloc(xyz.put(), cap * 3 * sizeof(double)));
+    CK(cudaMalloc(sr.put(), cap * 2 * sizeof(long long)));
+    if (m->known_M) {
+      CK(cudaMemcpyAsync(xyz.get(), m->xyz.get(), size_t(m->known_M) * 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+      CK(cudaMemcpyAsync(sr.get(), m->sr.get(), size_t(m->known_M) * 2 * sizeof(long long), cudaMemcpyDeviceToDevice, s));
+    }
+    CK(cudaStreamSynchronize(s));
+    m->xyz = std::move(xyz);
+    m->sr = std::move(sr);
+    m->cap_points = cap;
+  }
+  if (2 * need_V > m->slots) {
+    size_t slots = m->slots ? m->slots : pow2_at_least(2 * need_V);
+    while (slots < 2 * need_V) slots <<= 1;
+    DevPtr<unsigned long long> keys, win;
+    DevPtr<int> cnt;
+    if (int rc = alloc_table(m, slots, &keys, &cnt, &win)) return rc;
+    if (m->slots) {
+      vmap::k_map_rehash<<<unsigned((m->slots + vmap::kBlock - 1) / vmap::kBlock), vmap::kBlock, 0, s>>>(
+          m->keys, m->cnt, m->slots, keys, cnt, slots - 1);
+      m->ctx->launches++;
+      CK(cudaGetLastError());
+    }
+    CK(cudaStreamSynchronize(s));
+    m->keys = std::move(keys);
+    m->cnt = std::move(cnt);
+    m->win = std::move(win);
+    m->slots = slots;
+    m->rounds = 0;  // (fresh round words)
+  }
+  if (size_t(points) > m->cap_scratch) {
+    const size_t cap = size_t(points);
+    const size_t tiles = (cap + gtb::kTile - 1) / gtb::kTile + 1;
+    CK(cudaMalloc(m->slot.put(), cap * sizeof(int)));
+    CK(cudaMalloc(m->G.put(), cap * sizeof(int)));
+    CK(cudaMalloc(m->flag.put(), cap));
+    CK(cudaMalloc(m->tile.put(), tiles * sizeof(int)));
+    m->cap_scratch = cap;
+  }
+  return MADICP_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int madicp_map_create(madicp_ctx_t* c, double voxel_size, int points_per_voxel, int64_t reserve_points, madicp_map_t** out) {
+  const char* fn = "madicp_map_create";
+  if (!c || !out) return map_error(fn, "null context or output");
+  if (!(voxel_size > 0.0) || !std::isfinite(voxel_size))
+    return map_error(fn, "voxel_size must be finite and > 0 (got " + std::to_string(voxel_size) + ")");
+  if (points_per_voxel < 1 || points_per_voxel > 32)
+    return map_error(fn, "points_per_voxel must lie in [1, 32] (got " + std::to_string(points_per_voxel) + ")");
+  if (reserve_points < 0 || reserve_points > (int64_t(1) << 40)) return map_error(fn, "reserve_points out of range");
+  *out = nullptr;
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  std::unique_ptr<madicp_map> m(new madicp_map);
+  m->ctx = c;
+  m->v = voxel_size;
+  m->K = points_per_voxel;
+  CK(cudaMalloc(m->st.put(), sizeof(vmap::State)));
+  CK(cudaMemsetAsync(m->st.get(), 0, sizeof(vmap::State), c->stream));
+  CK(cudaHostAlloc(m->mirror.put(), sizeof(vmap::Mirror), cudaHostAllocMapped));
+  std::memset(m->mirror.get(), 0, sizeof(vmap::Mirror));
+  CK(cudaHostGetDevicePointer(reinterpret_cast<void**>(&m->d_mirror), m->mirror.get(), 0));
+  if (reserve_points > 0)
+    if (int rc = reserve(m.get(), reserve_points)) return rc;
+  *out = m.release();
+  return MADICP_OK;
+  MADICP_CATCH(fn)
+}
+
+int madicp_map_free(madicp_map_t* m) {
+  if (!m) return map_error("madicp_map_free", "null map");
+  cudaSetDevice(m->ctx->device);
+  cudaStreamSynchronize(m->ctx->stream);  // (inserts may still read and write the buffers)
+  delete m;
+  return MADICP_OK;
+}
+
+int madicp_map_insert(madicp_map_t* m, const madtree_gpu_t* t, const double X[12], int64_t scan) {
+  const char* fn = "madicp_map_insert";
+  if (!m || !t) return map_error(fn, "null map or tree");
+  if (t->ctx != m->ctx) return map_error(fn, "the tree lives on another context than the map");
+  if (!t->cloud) {
+    set_error(std::string(fn) + ": the tree kept no cloud (madicp_set_keep_cloud was off when it was built, or the cloud "
+              "was released)");
+    return MADICP_ERR_STATE;
+  }
+  const int64_t n = t->n_points;
+  if (n == 0) return MADICP_OK;
+  madicp_ctx* c = m->ctx;
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  if (int rc = reserve(m, n)) return rc;
+  if (m->rounds > 0xFFFFFF00u - uint32_t(m->K)) {  // tags about to run out: fresh round words
+    CK(cudaMemsetAsync(m->win.get(), 0xff, m->slots * (m->K > 1 ? 2 : 1) * sizeof(unsigned long long), c->stream));
+    m->rounds = 0;
+  }
+  vmap::InsertArgs a{};
+  a.xyz = t->cloud->xyz + 3 * size_t(t->cloud_off);
+  a.idx = t->cloud->idx + size_t(t->cloud_off);
+  a.n = int(n);
+  a.has_pose = X ? 1 : 0;
+  if (X) std::memcpy(a.X, X, 12 * sizeof(double));
+  a.v = m->v;
+  a.K = m->K;
+  a.tag0 = 0xFFFFFFFFu - (m->rounds + 1);
+  a.keys = m->keys;
+  a.cnt = m->cnt;
+  a.win[0] = m->win;
+  a.win[1] = m->K > 1 ? m->win + m->slots : m->win.get();
+  a.mask = m->slots - 1;
+  a.slot = m->slot;
+  a.flag = m->flag;
+  a.G = m->G;
+  a.tile = m->tile;
+  a.n_tiles = int((n + gtb::kTile - 1) / gtb::kTile);
+  a.st = m->st;
+  a.mirror = m->d_mirror;
+  a.seq = m->inserts + 1;
+  a.out_xyz = m->xyz;
+  a.out_sr = m->sr;
+  a.scan = scan;
+  const unsigned blocks = unsigned((n + vmap::kBlock - 1) / vmap::kBlock);
+  cudaStream_t s = c->stream;
+  vmap::k_map_claim<<<blocks, vmap::kBlock, 0, s>>>(a);
+  for (int r = 1; r < m->K; ++r) vmap::k_map_round<<<blocks, vmap::kBlock, 0, s>>>(a, r);
+  vmap::k_map_flags<<<unsigned(a.n_tiles), gtb::kTile, 0, s>>>(a);
+  vmap::k_map_sums<<<1, 1024, 0, s>>>(a);
+  vmap::k_map_scatter<<<blocks, vmap::kBlock, 0, s>>>(a);
+  c->launches += m->K + 3;
+  CK(cudaGetLastError());
+  m->rounds += uint32_t(m->K);
+  m->inserts++;
+  m->points_in += n;
+  return MADICP_OK;
+  MADICP_CATCH(fn)
+}
+
+int64_t madicp_map_size(madicp_map_t* m, int64_t* dropped) {
+  if (!m) return map_error("madicp_map_size", "null map");
+  CK(cudaSetDevice(m->ctx->device));
+  if (int rc = settle(m)) return rc;
+  if (dropped) *dropped = m->known_dropped;
+  return m->known_M;
+}
+
+int64_t madicp_map_points(madicp_map_t* m, double* xyz, int64_t* scan_record) {
+  const char* fn = "madicp_map_points";
+  if (!m) return map_error(fn, "null map");
+  if (!xyz && !scan_record) return map_error(fn, "no output");
+  CK(cudaSetDevice(m->ctx->device));
+  if (int rc = settle(m)) return rc;
+  const size_t M = size_t(m->known_M);
+  if (M == 0) return 0;
+  cudaStream_t s = m->ctx->stream;
+  if (xyz) CK(cudaMemcpyAsync(xyz, m->xyz.get(), M * 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (scan_record) CK(cudaMemcpyAsync(scan_record, m->sr.get(), M * 2 * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return int64_t(M);
+}
+
+int64_t madicp_map_points_dev(madicp_map_t* m, double* xyz, int64_t* scan_record, void* consumer_stream) {
+  const char* fn = "madicp_map_points_dev";
+  if (!m) return map_error(fn, "null map");
+  if (!xyz && !scan_record) return map_error(fn, "no output");
+  madicp_ctx* c = m->ctx;
+  CK(cudaSetDevice(c->device));
+  if (xyz)
+    if (int rc = madicp_check_device_ptr(c, xyz, 8, "madicp_map_points_dev (points)")) return rc;
+  if (scan_record)
+    if (int rc = madicp_check_device_ptr(c, scan_record, 8, "madicp_map_points_dev (scan, record)")) return rc;
+  if (int rc = settle(m)) return rc;
+  const size_t M = size_t(m->known_M);
+  if (M == 0) return 0;
+  if (int rc = madicp_stream_wait(c, c->stream, consumer_stream)) return rc;  // the outputs are allocated there
+  if (xyz) CK(cudaMemcpyAsync(xyz, m->xyz.get(), M * 3 * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
+  if (scan_record)
+    CK(cudaMemcpyAsync(scan_record, m->sr.get(), M * 2 * sizeof(int64_t), cudaMemcpyDeviceToDevice, c->stream));
+  if (int rc = madicp_stream_wait(c, consumer_stream, c->stream)) return rc;
+  return int64_t(M);
+}
+
+int madicp_map_clear(madicp_map_t* m) {
+  if (!m) return map_error("madicp_map_clear", "null map");
+  cudaStream_t s = m->ctx->stream;
+  CK(cudaSetDevice(m->ctx->device));
+  CK(cudaStreamSynchronize(s));  // (no insert may publish counters after the reset)
+  if (m->slots) {
+    CK(cudaMemsetAsync(m->keys.get(), 0xff, m->slots * sizeof(unsigned long long), s));
+    CK(cudaMemsetAsync(m->cnt.get(), 0, m->slots * sizeof(int), s));
+    CK(cudaMemsetAsync(m->win.get(), 0xff, m->slots * (m->K > 1 ? 2 : 1) * sizeof(unsigned long long), s));
+  }
+  CK(cudaMemsetAsync(m->st.get(), 0, sizeof(vmap::State), s));
+  m->rounds = 0;
+  vmap::Mirror* h = m->mirror.get();
+  h->M = h->V = h->dropped = 0;
+  h->seq = m->inserts;
+  m->known_M = m->known_V = m->known_dropped = 0;
+  m->known_in = m->points_in;
+  return MADICP_OK;
+}
+
+}  // extern "C"

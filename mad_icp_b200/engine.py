@@ -196,6 +196,61 @@ class DeskewPlan:
     __del__ = free
 
 
+class VoxelMap:
+    """A voxel map of kept clouds on one Registrar (madicp_map_*, `Registrar.voxel_map`): each voxel keeps the first
+    points_per_voxel points that reach it, inserts in call order, points in kept-cloud order."""
+
+    def __init__(self, handle, registrar):
+        self._h, self._reg = handle, registrar  # the registrar must outlive the map
+
+    def free(self):
+        h = getattr(self, "_h", None)
+        if h and getattr(self._reg, "_h", None):
+            self._h = None
+            try:
+                capi.lib().madicp_map_free(h)
+            except TypeError:  # interpreter shutdown
+                pass
+
+    __del__ = free
+
+    def insert(self, tree, T=None, scan=0):
+        """The kept cloud of a DeviceTree (built with `Registrar.keep_cloud` on), posed by T (4x4 / 3x4, or None:
+        untouched), its points tagged with `scan`.  Asynchronous."""
+        X = None if T is None else pose12(T)
+        check(capi.lib().madicp_map_insert(self._h, tree._h, as_d(X), int(scan)), "madicp_map_insert")
+
+    def size(self):
+        return check(capi.lib().madicp_map_size(self._h, None), "madicp_map_size")
+
+    def dropped(self):
+        d = C.c_int64(0)
+        check(capi.lib().madicp_map_size(self._h, C.byref(d)), "madicp_map_size")
+        return d.value
+
+    def points(self, device=False):
+        """(xyz (M, 3) float64, scan_record (M, 2) int64) as numpy arrays, or with device=True torch tensors on the
+        registrar's device, ready on torch's current stream."""
+        n = self.size()
+        if not device:
+            xyz, sr = np.empty((n, 3)), np.empty((n, 2), np.int64)
+            check(capi.lib().madicp_map_points(self._h, as_d(xyz), sr.ctypes.data_as(C.POINTER(C.c_int64))),
+                  "madicp_map_points")
+            return xyz, sr
+        import torch
+        dev = torch.device("cuda", self._reg.device)
+        xyz = torch.empty((n, 3), dtype=torch.float64, device=dev)
+        sr = torch.empty((n, 2), dtype=torch.int64, device=dev)
+        if n:
+            check(capi.lib().madicp_map_points_dev(self._h, C.c_void_p(xyz.data_ptr()), C.c_void_p(sr.data_ptr()),
+                                                   C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                  "madicp_map_points_dev")
+        return xyz, sr
+
+    def clear(self):
+        check(capi.lib().madicp_map_clear(self._h), "madicp_map_clear")
+
+
 class Registrar:
     """One GPU's registration context (reference: class MADicp + Pipeline's keyframe deque)."""
 
@@ -226,6 +281,13 @@ class Registrar:
     def keep_cloud(self, keep=True):
         """Trees built from now on keep their input cloud and its record indices (`DeviceTree.cloud`)."""
         check(capi.lib().madicp_set_keep_cloud(self._h, int(bool(keep))), "madicp_set_keep_cloud")
+
+    def voxel_map(self, voxel_size, points_per_voxel=1, reserve_points=0):
+        """A VoxelMap on this context (madicp_map_create); it takes trees built with `keep_cloud` on."""
+        h = C.c_void_p()
+        check(capi.lib().madicp_map_create(self._h, float(voxel_size), int(points_per_voxel), int(reserve_points),
+                                           C.byref(h)), "madicp_map_create")
+        return VoxelMap(h, self)
 
     def set_stream(self, cuda_stream_ptr):
         check(capi.lib().madicp_set_stream(self._h, C.c_void_p(cuda_stream_ptr or 0)))

@@ -320,6 +320,24 @@ def cloud_array_dev(pipeline, indices, map_frame):
     return out
 
 
+def map_array_dev(pipeline, indices):
+    """Pipeline.mapArray / mapIndices(device=True): the voxel map's points as an (M, 3) float64 torch tensor, or its
+    (scan, record) pairs (indices=True) as an (M, 2) int64 tensor, on the pipeline's device, copied in place and ready on
+    torch's current stream.  Learning M waits once for the pipeline's stream (mapSize); the points never reach the
+    host."""
+    import torch
+    dev = torch.device("cuda", pipeline._device())
+    n = pipeline.mapSize()
+    out = torch.empty((n, 2) if indices else (n, 3), dtype=torch.int64 if indices else torch.float64, device=dev)
+    if n:
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        if indices:
+            pipeline._mapDev(0, out.data_ptr(), stream)
+        else:
+            pipeline._mapDev(out.data_ptr(), 0, stream)
+    return out
+
+
 def vcorr(apply_correction=False, vertical_angle_offset=VERTICAL_ANGLE_OFFSET):
     """madicp_vcorr_t of the reader's `apply_correction` / `vertical_angle_offset`, or None without a correction."""
     if not apply_correction:
@@ -357,5 +375,5 @@ def correct_vertical_angle(records, vertical_angle_offset=VERTICAL_ANGLE_OFFSET,
     return out[:kept]
 
 
-__all__ = ["pointcloud2_dtype", "describe", "describe_times", "time_layout", "time_chunks", "chunk_poses", "layout", "to_host", "search_cloud_arrays_dev", "leaves_array_dev", "cloud_array_dev", "range_mask", "vcorr", "correct_vertical_angle",
+__all__ = ["pointcloud2_dtype", "describe", "describe_times", "time_layout", "time_chunks", "chunk_poses", "layout", "to_host", "search_cloud_arrays_dev", "leaves_array_dev", "cloud_array_dev", "map_array_dev", "range_mask", "vcorr", "correct_vertical_angle",
            "VERTICAL_ANGLE_OFFSET", "RANGE_NONE", "RANGE_INCLUSIVE", "RANGE_STRICT"]

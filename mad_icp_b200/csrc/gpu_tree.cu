@@ -1591,7 +1591,7 @@ int madtree_gpu_build_batch(madicp_ctx_t* c, const void* const* clouds, const in
   madicp_points_t d[kMaxBatch];
   for (int b = 0; b < count; ++b) {
     if (!clouds[b] || n_points[b] <= 0 || n_points[b] > (int64_t(1) << 24)) {
-      set_error("madtree_gpu_build_batch: empty cloud, or more than 2^26 points in the batch");
+      set_error("madtree_gpu_build_batch: empty cloud, or a cloud of more than 2^24 points");
       return MADICP_ERR_INVALID;
     }
     d[b] = packed_points(clouds[b], n_points[b], is_f32);

@@ -15,15 +15,12 @@ pytestmark = pytest.mark.gpu
 
 def _bfs_order(e):
     """DFS pre-order export (left/right node ids) -> node ids in breadth-first order, siblings adjacent."""
-    order, level = [], [0]
-    while level:
-        order += level
-        nxt = []
-        for i in level:
-            if e["left"][i] >= 0:
-                nxt += [int(e["left"][i]), int(e["right"][i])]
-        level = nxt
-    return np.array(order)
+    order, level = [], np.zeros(1, np.int64)
+    while level.size:
+        order.append(level)
+        inner = level[e["left"][level] >= 0]
+        level = np.stack([e["left"][inner], e["right"][inner]], 1).ravel().astype(np.int64)
+    return np.concatenate(order)
 
 
 def _same_as_oracle(dt, otree, ft=None):

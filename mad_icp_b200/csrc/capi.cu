@@ -1414,6 +1414,7 @@ int madicp_calibrate(madicp_ctx_t* c, const double X0[12]) {
   CK(cudaSetDevice(c->device));
   const int64_t items = int64_t(madicp_num_keyframes(c)) * c->L;
   const double per_sm = double((items + 31) / 32) / double(c->sm_count);
+  const int kept_threads = c->gn_threads, kept_ctas = c->gn_grid / c->sm_count;  // an explicit shape outlives the calibration
   int measured = 0;
   {
     struct KeepAuto {  // the shapes are measured with the automatic choice off; it comes back on every exit
@@ -1442,6 +1443,10 @@ int madicp_calibrate(madicp_ctx_t* c, const double X0[12]) {
       c->pass_cost[i] = double(ms) / double(rounds) / passes;  // any unit: only ratios matter
       ++measured;
     }
+  }
+  if (!c->gn_auto) {  // the shape set through madicp_set_gn_grid (or MADICP_GN_SHAPE) stays in force
+    const int rc_shape = configure_gn(c, kept_threads, kept_ctas);
+    if (!rc) rc = rc_shape;
   }
   if (rc) return rc;
   c->calibrated = true;

@@ -227,6 +227,18 @@ int64_t madicp_map_points(madicp_map_t* map, double* xyz, int64_t* scan_record);
 int64_t madicp_map_points_dev(madicp_map_t* map, double* xyz, int64_t* scan_record, void* consumer_stream);
 /* Not in the reference.  Empties the map (keeping its memory); later inserts start a new one.  Synchronises. */
 int madicp_map_clear(madicp_map_t* map);
+/* Not in the reference.  Removes every voxel whose centre lies farther than max_distance from origin, with all its
+ * rows.  Voxel key k = floor(p / v) as the insert computes it, centre c = (k + 0.5) v per axis, and the voxel goes iff
+ * ((cx - ox)^2 + (cy - oy)^2) + (cz - oz)^2 > max_distance^2, every operation float64 round-to-nearest without FMA and
+ * max_distance^2 rounded on the host: a pure function of the key.  So every point within max_distance - v sqrt(3) / 2 of
+ * the origin survives.  The surviving rows keep their order and their (scan, record).  A removed voxel is forgotten:
+ * later points that reach it are accepted as in a new voxel, up to points_per_voxel again.  A removal is not a drop
+ * (`dropped` counts only what inserts skip).  max_distance: >= 0, not NaN (+inf removes nothing); origin: finite.
+ * Runs on the context's stream and never waits on the host; madicp_map_size counts it once enqueued.  The table keeps a
+ * removed voxel's slot as a tombstone until an insert that needs the room rebuilds it (synchronising, as growth does),
+ * sized from the live voxels; the row allocations stay at their peak (nothing shrinks), and the first removal
+ * allocates a row-sized scratch for the compaction.  MADICP_ERR_INVALID for a bad argument, before any device work. */
+int madicp_map_remove_far(madicp_map_t* map, const double origin[3], double max_distance);
 /* Audit dump of a DEVICE-BUILT tree in breadth-first order: mean n x 3, eigenvectors n x 9 (column-major), bbox
  * n x 3, num_points n (any may be NULL).  Valid for the most recently built tree of the context.  Synchronises. */
 int madtree_gpu_export(const madtree_gpu_t* t, double* mean, double* eigenvectors, double* bbox, int32_t* num_points);

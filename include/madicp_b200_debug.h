@@ -84,6 +84,10 @@ int madicp_debug_time_chunks(const madicp_points_t* desc, const madicp_vcorr_t* 
 int madicp_debug_chunk_poses(const double T_prev[12], const double T_now[12], double sensor_hz, int n_chunks,
                              double* poses);
 
+/* The voxel map's hash table (madicp_map_*): its slots, the occupied ones (live voxels and the tombstones of removed
+ * ones) and the live ones, counted from the table's keys (any output may be NULL).  Synchronises. */
+int madicp_debug_map_table(madicp_map_t* map, int64_t* slots, int64_t* occupied, int64_t* live);
+
 #ifdef __cplusplus
 }
 #endif

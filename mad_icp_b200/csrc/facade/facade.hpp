@@ -259,6 +259,10 @@ class VoxelMap {
     check(int(std::min<int64_t>(0, madicp_map_points_dev(m_, xyz, scan_record, consumer_stream))), "madicp_map_points_dev");
   }
   void clear() { check(madicp_map_clear(m_), "madicp_map_clear"); }
+  // every voxel whose centre lies farther than max_distance from origin goes, with its rows (asynchronous)
+  void removeFar(const double origin[3], double max_distance) {
+    check(madicp_map_remove_far(m_, origin, max_distance), "madicp_map_remove_far");
+  }
 
  private:
   madicp_map_t* m_ = nullptr;

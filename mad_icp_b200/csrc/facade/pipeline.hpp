@@ -238,9 +238,9 @@ class Pipeline {
 
   Pipeline(double sensor_hz, bool deskew, double b_max, double rho_ker, double p_th, double b_min, double b_ratio,
            int num_keyframes, int num_threads, bool realtime, int device = -1, bool keep_cloud = false,
-           double map_voxel_size = 0.0, int map_points_per_voxel = 1)
+           double map_voxel_size = 0.0, int map_points_per_voxel = 1, double map_max_distance = 0.0)
       : sensor_hz_(sensor_hz), deskew_(deskew), b_max_(b_max), p_th_(p_th), b_min_(b_min), num_keyframes_(num_keyframes),
-        realtime_(realtime), keep_cloud_(keep_cloud),
+        realtime_(realtime), keep_cloud_(keep_cloud), map_max_distance_(map_max_distance),
         icp_(b_max, rho_ker, b_ratio, num_threads, resolveDevice(device), std::max(num_keyframes, 1)), vel_(sensor_hz) {
     frame_to_map_ = keyframe_to_map_ = detail::poseIdentity();
     device_ = resolveDevice(device);
@@ -249,6 +249,10 @@ class Pipeline {
     if (!(map_voxel_size >= 0.0) || !std::isfinite(map_voxel_size))
       throw Error("Pipeline: map_voxel_size must be finite and >= 0 (0: no map)");
     if (map_points_per_voxel < 1 || map_points_per_voxel > 32) throw Error("Pipeline: map_points_per_voxel must lie in [1, 32]");
+    if (!(map_max_distance >= 0.0) || !std::isfinite(map_max_distance))
+      throw Error("Pipeline: map_max_distance must be finite and >= 0 (0: no window)");
+    if (map_max_distance > 0.0 && !(map_voxel_size > 0.0))
+      throw Error("Pipeline: map_max_distance > 0 needs a map (map_voxel_size > 0)");
     if (map_voxel_size > 0.0) {  // the map inserts each scan's kept cloud: every tree keeps one
       if (!gpu_build_) throw Error("Pipeline: a map (map_voxel_size > 0) needs device-built trees (MADICP_GPU_BUILD)");
       check(madicp_set_keep_cloud(icp_.context(), 1), "madicp_set_keep_cloud");
@@ -314,7 +318,8 @@ class Pipeline {
   // The voxel map of every scan so far (map_voxel_size > 0; not in the reference): each scan's kept cloud in the map
   // frame, the rows currentCloud(map) hands out, inserted once its pose is known; a voxel keeps the first
   // map_points_per_voxel points that reach it.  Rows in acceptance order with (scan, record): the scan's currentID()
-  // before it was computed and the point's currentCloudIndices() value.
+  // before it was computed and the point's currentCloudIndices() value.  With map_max_distance > 0 (a window), every
+  // insert is followed by the removal of the voxels whose centre lies farther than that from currentPose()'s translation.
   size_t mapSize() { return requireMap().size(); }
   int64_t mapDropped() {
     int64_t dropped = 0;
@@ -442,6 +447,15 @@ class Pipeline {
     s.records = true;
     return s;
   }
+  // the scan's kept cloud into the map; with a window, then every voxel farther than map_max_distance from the sensor
+  // (currentPose()'s translation) goes
+  void insertIntoMap(const MADtree& t) {
+    map_->insert(t, int64_t(seq_));
+    if (map_max_distance_ > 0.0) {
+      const double origin[3] = {frame_to_map_.m[3], frame_to_map_.m[7], frame_to_map_.m[11]};
+      map_->removeFar(origin, map_max_distance_);
+    }
+  }
   VoxelMap& requireMap() const {
     if (!map_) throw Error("Pipeline.map: the pipeline builds no map (construct it with map_voxel_size > 0)");
     return *map_;
@@ -559,7 +573,7 @@ class Pipeline {
       f->to_map = frame_to_map_;
       f->stamp = stamp;
       f->tree = makeTree(s);
-      if (map_) map_->insert(*f->tree, int64_t(seq_));  // (no pose: the sensor frame is the map frame)
+      if (map_) insertIntoMap(*f->tree);  // (no pose: the sensor frame is the map frame)
       keyframes_.push_back(f);
       current_ = f;
       trajectory_.push_back(detail::poseIdentity());
@@ -610,7 +624,7 @@ class Pipeline {
     cur->weight = (iters > 0 && iters <= MADICP_MAX_ITERS) ? icp_.weight()                        // :223, from the device
                                                            : detail::inverseDeterminant(icp_.H_adder_);
     cur->tree->applyTransform(toM(frame_to_map_));             // :224
-    if (map_) map_->insert(*cur->tree, int64_t(seq_));
+    if (map_) insertIntoMap(*cur->tree);
     if (current_ && (keep_cloud_ || map_)) current_->tree->releaseCloud();  // (only the current scan's cloud is kept)
     current_ = cur;
     frames_.push_back(cur);
@@ -696,6 +710,7 @@ class Pipeline {
   int num_keyframes_, max_parallel_levels_ = 0;
   bool realtime_;
   bool keep_cloud_ = false;  // the current scan's tree keeps its cloud and record indices (currentCloud)
+  double map_max_distance_ = 0.0;  // > 0: after each insert, the map drops the voxels farther than this from the sensor
   bool gpu_build_ = true;   // MADICP_GPU_BUILD=0: host-built trees
   int device_ = 0;
   int num_threads_ = 1;

@@ -148,16 +148,19 @@ PYBIND11_MODULE(pypeline, m) {
       // keep_cloud (not in the reference): the current scan's deskewed cloud and its record indices stay available
       // (currentCloudArray / currentCloudIndices)
       // map_voxel_size > 0 (not in the reference): a voxel map of every scan builds itself on the device, keeping the
-      // first map_points_per_voxel points of each voxel (mapArray / mapIndices)
+      // first map_points_per_voxel points of each voxel (mapArray / mapIndices); map_max_distance > 0 bounds it to the
+      // voxels whose centre lies within that distance of the sensor after each scan
       .def(py::init([](double sensor_hz, bool deskew, double b_max, double rho_ker, double p_th, double b_min, double b_ratio,
                        int num_keyframes, int num_threads, bool realtime, bool keep_cloud, double map_voxel_size,
-                       int map_points_per_voxel) {
+                       int map_points_per_voxel, double map_max_distance) {
              return new mb::Pipeline(sensor_hz, deskew, b_max, rho_ker, p_th, b_min, b_ratio, num_keyframes, num_threads,
-                                     realtime, -1, keep_cloud, map_voxel_size, map_points_per_voxel);
+                                     realtime, -1, keep_cloud, map_voxel_size, map_points_per_voxel,
+                                     map_max_distance);
            }),
            py::arg("sensor_hz"), py::arg("deskew"), py::arg("b_max"), py::arg("rho_ker"), py::arg("p_th"), py::arg("b_min"),
            py::arg("b_ratio"), py::arg("num_keyframes"), py::arg("num_threads"), py::arg("realtime"),
-           py::arg("keep_cloud") = false, py::arg("map_voxel_size") = 0.0, py::arg("map_points_per_voxel") = 1)
+           py::arg("keep_cloud") = false, py::arg("map_voxel_size") = 0.0, py::arg("map_points_per_voxel") = 1,
+           py::arg("map_max_distance") = 0.0)
       .def("currentPose", [](const mb::Pipeline& p) { return pose_to_numpy(p.currentPose()); })
       .def("trajectory",
            [](const mb::Pipeline& p) {

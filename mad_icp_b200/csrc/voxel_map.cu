@@ -1,14 +1,19 @@
 // voxel_map.cu -- madicp_map_* (include/madicp_b200.h): a voxel map of every inserted kept cloud, built on the device.
 // The kernels and the acceptance rule are in voxel_map_kernels.cuh.  An insert runs on the context's stream and never
-// waits on the host: the capacity it needs is bounded from the counters the previous inserts left in mapped memory, and
-// the host synchronises only when that bound outgrows the allocations (the map then grows by doubling).
+// waits on the host: the capacity it needs is bounded from the counters the previous operations left in mapped memory,
+// and the host synchronises only when that bound outgrows the allocations (the map then grows by doubling, or its table
+// is rebuilt without the tombstones of removed voxels).  A removal (madicp_map_remove_far) never waits on the host.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
 #include <cmath>
+#include <cstdint>
 #include <cstring>
 #include <string>
+#include <vector>
 
+#include "../../include/madicp_b200_debug.h"
 #include "ctx.hpp"
 #include "voxel_map_kernels.cuh"
 
@@ -30,13 +35,20 @@ struct madicp_map {
   size_t cap_scratch = 0;
   DevPtr<int> slot, G, tile;
   DevPtr<unsigned char> flag;
+  // row-sized scratch of a removal (allocated by the first one, then kept at the rows' capacity)
+  size_t cap_rows = 0;
+  DevPtr<double> tmp_xyz;
+  DevPtr<long long> tmp_sr;
+  DevPtr<int> row_G, row_tile;
+  DevPtr<unsigned char> row_flag;
   DevPtr<vmap::State> st;
   HostPtr<vmap::Mirror> mirror;  // mapped
   vmap::Mirror* d_mirror = nullptr;
-  uint64_t inserts = 0;  // inserts enqueued
-  int64_t points_in = 0;  // points handed to them
-  // the counters as of the last insert the host has seen complete, and points_in at that time
-  int64_t known_M = 0, known_V = 0, known_dropped = 0, known_in = 0;
+  uint64_t ops = 0;       // inserts and removals enqueued
+  int64_t points_in = 0;  // points handed to the inserts
+  // the counters as of the last operation the host has seen complete (known_ops), and points_in at that time
+  int64_t known_M = 0, known_V = 0, known_T = 0, known_dropped = 0, known_in = 0;
+  uint64_t known_ops = 0;
   uint32_t rounds = 0;  // acceptance rounds so far (tags 0xFFFFFFFF - round)
 };
 
@@ -47,26 +59,28 @@ int map_error(const char* fn, const std::string& msg) {
   return MADICP_ERR_INVALID;
 }
 
-// takes the mirror's counters when they belong to the last insert enqueued
+// takes the mirror's counters when they belong to the last operation enqueued
 void refresh(madicp_map* m) {
   const volatile vmap::Mirror* h = m->mirror.get();
-  if (h->seq != m->inserts) return;
+  if (h->seq != m->ops) return;
   std::atomic_thread_fence(std::memory_order_acquire);
   m->known_M = h->M;
   m->known_V = h->V;
+  m->known_T = h->T;
   m->known_dropped = h->dropped;
   m->known_in = m->points_in;
+  m->known_ops = m->ops;
 }
 
-// the map's counters exactly: waits for the context's stream when the last insert may still run
+// the map's counters exactly: waits for the context's stream when the last operation may still run
 int settle(madicp_map* m) {
   refresh(m);
-  if (m->known_in != m->points_in) {
+  if (m->known_ops != m->ops) {
     CK(cudaStreamSynchronize(m->ctx->stream));
     refresh(m);
   }
-  if (m->known_in != m->points_in) {
-    set_error("voxel map: the counters of the last insert did not arrive");
+  if (m->known_ops != m->ops) {
+    set_error("voxel map: the counters of the last operation did not arrive");
     return MADICP_ERR_CUDA;
   }
   return MADICP_OK;
@@ -93,13 +107,18 @@ int alloc_table(madicp_map* m, size_t slots, DevPtr<unsigned long long>* keys, D
 }
 
 // Room for `points` more rows and voxels after everything enqueued so far: a bound from the last counters the host has
-// seen, exact after a synchronisation that only a growth needs.  Growth doubles; the table is rehashed on the device.
+// seen, exact after a synchronisation that only a growth or a rebuild needs.  Rows grow by doubling.  The table's
+// occupied slots (live voxels and the tombstones of removed ones) stay at most half of it; past that the table is
+// rebuilt on the device, the tombstones left behind.  Without tombstones that is the growth: doubled until the live
+// voxels take at most half.  With them the rebuild is sized from the live voxels alone, to at most a quarter live: the
+// same size while they leave that room, else doubled, so the next rebuild is as many removed voxels away as there are
+// live ones and a map whose live voxels stay bounded keeps a bounded table.
 int reserve(madicp_map* m, int64_t points) {
   refresh(m);
   auto fits = [&] {
     const int64_t pending = m->points_in - m->known_in + points;
-    return size_t(m->known_M + pending) <= m->cap_points && 2 * size_t(m->known_V + pending) <= m->slots &&
-           size_t(points) <= m->cap_scratch;
+    return size_t(m->known_M + pending) <= m->cap_points &&
+           2 * size_t(m->known_V + m->known_T + pending) <= m->slots && size_t(points) <= m->cap_scratch;
   };
   if (fits()) return MADICP_OK;
   cudaStream_t s = m->ctx->stream;
@@ -121,9 +140,10 @@ int reserve(madicp_map* m, int64_t points) {
     m->sr = std::move(sr);
     m->cap_points = cap;
   }
-  if (2 * need_V > m->slots) {
+  if (2 * (need_V + size_t(m->known_T)) > m->slots) {
+    const size_t live_share = m->known_T ? 4 : 2;  // slots per live voxel after the rebuild, at least
     size_t slots = m->slots ? m->slots : pow2_at_least(2 * need_V);
-    while (slots < 2 * need_V) slots <<= 1;
+    while (slots < live_share * need_V) slots <<= 1;
     DevPtr<unsigned long long> keys, win;
     DevPtr<int> cnt;
     if (int rc = alloc_table(m, slots, &keys, &cnt, &win)) return rc;
@@ -133,12 +153,15 @@ int reserve(madicp_map* m, int64_t points) {
       m->ctx->launches++;
       CK(cudaGetLastError());
     }
+    if (m->known_T) CK(cudaMemsetAsync(&m->st.get()->T, 0, sizeof(unsigned long long), s));
     CK(cudaStreamSynchronize(s));
     m->keys = std::move(keys);
     m->cnt = std::move(cnt);
     m->win = std::move(win);
     m->slots = slots;
     m->rounds = 0;  // (fresh round words)
+    m->known_T = 0;
+    m->mirror.get()->T = 0;  // (the stream is idle: nothing writes the mirror before the next operation)
   }
   if (size_t(points) > m->cap_scratch) {
     const size_t cap = size_t(points);
@@ -186,7 +209,7 @@ int madicp_map_create(madicp_ctx_t* c, double voxel_size, int points_per_voxel, 
 int madicp_map_free(madicp_map_t* m) {
   if (!m) return map_error("madicp_map_free", "null map");
   cudaSetDevice(m->ctx->device);
-  cudaStreamSynchronize(m->ctx->stream);  // (inserts may still read and write the buffers)
+  cudaStreamSynchronize(m->ctx->stream);  // (inserts and removals may still read and write the buffers)
   delete m;
   return MADICP_OK;
 }
@@ -231,7 +254,7 @@ int madicp_map_insert(madicp_map_t* m, const madtree_gpu_t* t, const double X[12
   a.n_tiles = int((n + gtb::kTile - 1) / gtb::kTile);
   a.st = m->st;
   a.mirror = m->d_mirror;
-  a.seq = m->inserts + 1;
+  a.seq = m->ops + 1;
   a.out_xyz = m->xyz;
   a.out_sr = m->sr;
   a.scan = scan;
@@ -245,7 +268,7 @@ int madicp_map_insert(madicp_map_t* m, const madtree_gpu_t* t, const double X[12
   c->launches += m->K + 3;
   CK(cudaGetLastError());
   m->rounds += uint32_t(m->K);
-  m->inserts++;
+  m->ops++;
   m->points_in += n;
   return MADICP_OK;
   MADICP_CATCH(fn)
@@ -308,11 +331,91 @@ int madicp_map_clear(madicp_map_t* m) {
   CK(cudaMemsetAsync(m->st.get(), 0, sizeof(vmap::State), s));
   m->rounds = 0;
   vmap::Mirror* h = m->mirror.get();
-  h->M = h->V = h->dropped = 0;
-  h->seq = m->inserts;
-  m->known_M = m->known_V = m->known_dropped = 0;
+  h->M = h->V = h->dropped = h->T = 0;
+  h->seq = m->ops;
+  m->known_M = m->known_V = m->known_T = m->known_dropped = 0;
   m->known_in = m->points_in;
+  m->known_ops = m->ops;
   return MADICP_OK;
+}
+
+int madicp_map_remove_far(madicp_map_t* m, const double origin[3], double max_distance) {
+  const char* fn = "madicp_map_remove_far";
+  if (!m) return map_error(fn, "null map");
+  if (!origin) return map_error(fn, "null origin");
+  if (!(max_distance >= 0.0))
+    return map_error(fn, "max_distance must be >= 0 and not NaN (got " + std::to_string(max_distance) + ")");
+  for (int a = 0; a < 3; ++a)
+    if (!std::isfinite(origin[a]))
+      return map_error(fn, "origin must be finite (component " + std::to_string(a) + " is " + std::to_string(origin[a]) + ")");
+  madicp_ctx* c = m->ctx;
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  if (!m->slots) return MADICP_OK;  // nothing was ever inserted
+  cudaStream_t s = c->stream;
+  refresh(m);
+  const size_t rows = std::min(m->cap_points, size_t(m->known_M + m->points_in - m->known_in));  // >= the device's M
+  if (rows > size_t(INT32_MAX - gtb::kTile)) return map_error(fn, "the map holds more rows than a removal can scan");
+  if (m->cap_rows < m->cap_points) {  // (after a growth of the rows: earlier removals may still read the old scratch)
+    CK(cudaStreamSynchronize(s));
+    const size_t cap = m->cap_points;
+    CK(cudaMalloc(m->tmp_xyz.put(), cap * 3 * sizeof(double)));
+    CK(cudaMalloc(m->tmp_sr.put(), cap * 2 * sizeof(long long)));
+    CK(cudaMalloc(m->row_G.put(), cap * sizeof(int)));
+    CK(cudaMalloc(m->row_flag.put(), cap));
+    CK(cudaMalloc(m->row_tile.put(), ((cap + gtb::kTile - 1) / gtb::kTile + 1) * sizeof(int)));
+    m->cap_rows = cap;
+  }
+  vmap::RemoveArgs a{};
+  a.keys = m->keys;
+  a.slots = m->slots;
+  a.v = m->v;
+  for (int k = 0; k < 3; ++k) a.o[k] = origin[k];
+  a.D2 = max_distance * max_distance;
+  a.xyz = m->xyz;
+  a.sr = m->sr;
+  a.tmp_xyz = m->tmp_xyz;
+  a.tmp_sr = m->tmp_sr;
+  a.flag = m->row_flag;
+  a.G = m->row_G;
+  a.tile = m->row_tile;
+  a.st = m->st;
+  a.mirror = m->d_mirror;
+  a.seq = m->ops + 1;
+  const unsigned slot_blocks = unsigned((m->slots + vmap::kBlock - 1) / vmap::kBlock);
+  const unsigned tiles = unsigned(std::max<size_t>(1, (rows + gtb::kTile - 1) / gtb::kTile));
+  const unsigned row_blocks = unsigned(std::max<size_t>(1, (rows + vmap::kBlock - 1) / vmap::kBlock));
+  vmap::k_map_evict<<<slot_blocks, vmap::kBlock, 0, s>>>(a);
+  vmap::k_map_keep<<<tiles, gtb::kTile, 0, s>>>(a);
+  vmap::k_map_evict_sums<<<1, 1024, 0, s>>>(a);
+  vmap::k_map_compact<<<row_blocks, vmap::kBlock, 0, s>>>(a);
+  vmap::k_map_copy_back<<<row_blocks, vmap::kBlock, 0, s>>>(a);
+  c->launches += 5;
+  CK(cudaGetLastError());
+  m->ops++;
+  return MADICP_OK;
+  MADICP_CATCH(fn)
+}
+
+int madicp_debug_map_table(madicp_map_t* m, int64_t* slots, int64_t* occupied, int64_t* live) {
+  const char* fn = "madicp_debug_map_table";
+  if (!m) return map_error(fn, "null map");
+  MADICP_TRY
+  CK(cudaSetDevice(m->ctx->device));
+  CK(cudaStreamSynchronize(m->ctx->stream));
+  std::vector<unsigned long long> keys(m->slots);
+  if (m->slots)
+    CK(cudaMemcpy(keys.data(), m->keys.get(), m->slots * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  int64_t occ = 0, liv = 0;
+  for (unsigned long long k : keys) {
+    occ += k != vmap::kEmpty;
+    liv += k != vmap::kEmpty && k != vmap::kTomb;
+  }
+  if (slots) *slots = int64_t(m->slots);
+  if (occupied) *occupied = occ;
+  if (live) *live = liv;
+  return MADICP_OK;
+  MADICP_CATCH(fn)
 }
 
 }  // extern "C"

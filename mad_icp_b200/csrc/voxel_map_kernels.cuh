@@ -12,6 +12,16 @@
 //   k_map_scatter  winner i goes to row M + (winners before i): dense storage in acceptance order.
 // Round words carry a tag (0xFFFFFFFF - global round number) above the position, so a word left by any earlier round
 // is larger than every value of the current one and the words never need clearing.
+//
+// A removal (madicp_map_remove_far) drops every voxel whose centre lies farther than D from an origin, in 5 launches:
+//   k_map_evict          over the table's slots: a removed voxel's key becomes kTomb, and the removed voxels are counted;
+//   k_map_keep           over the rows: keep flag of every row from its own key (the posed xyz the insert keyed), flags
+//                        scanned per tile, the first removed row noted;
+//   k_map_evict_sums     the tile offsets, the new M, V and tombstone counts, the counters mirrored to mapped memory;
+//   k_map_compact        survivors from the first removed row on are scattered to a row-sized scratch, in order;
+//   k_map_copy_back      the scratch rows from the first removed row on go back to the map's rows.
+// The row kernels return at once when k_map_evict removed nothing.  Tombstones keep their slots (a claim passes over
+// them like any foreign key) until the host rebuilds the table (k_map_rehash skips them).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -23,15 +33,18 @@
 namespace madicp {
 namespace vmap {
 
-constexpr unsigned long long kEmpty = ~0ull;  // a free slot (packed keys stay below 2^63)
-constexpr double kKeyLimit = 1048576.0;       // |key| < 2^20 per axis: three 21-bit fields
+constexpr unsigned long long kEmpty = ~0ull;      // a free slot (packed keys stay below 2^63)
+constexpr unsigned long long kTomb = ~0ull - 1;   // the slot of a removed voxel: occupied, matches no key
+constexpr double kKeyLimit = 1048576.0;           // |key| < 2^20 per axis: three 21-bit fields
 constexpr int kBlock = 256;
 
-struct State {  // device: the map's counters (k_map_claim adds, k_map_sums publishes)
-  unsigned long long M, V, dropped, base;
+// device: the map's counters (k_map_claim adds, k_map_sums / k_map_evict_sums publish).  T: tombstones in the table;
+// removed: voxels the running removal took out (zeroed by its k_map_evict_sums); lo: its first removed row (~0: none)
+struct State {
+  unsigned long long M, V, dropped, base, T, removed, lo;
 };
-struct Mirror {  // mapped host memory: the counters after the insert numbered `seq` (written last)
-  long long M, V, dropped;
+struct Mirror {  // mapped host memory: the counters after the operation (insert or removal) numbered `seq` (written last)
+  long long M, V, dropped, T;
   unsigned long long seq;
 };
 
@@ -170,6 +183,7 @@ __global__ void __launch_bounds__(1024) k_map_sums(const __grid_constant__ Inser
     m->M = (long long) st->M;
     m->V = (long long) st->V;
     m->dropped = (long long) st->dropped;
+    m->T = (long long) st->T;
     __threadfence_system();
     m->seq = a.seq;
   }
@@ -189,17 +203,130 @@ __global__ void __launch_bounds__(kBlock) k_map_scatter(const __grid_constant__ 
   atomicAdd(a.cnt + a.slot[i], 1);
 }
 
-// growth: every key of the old table, with its count, into the new (larger, empty) one
+// growth or rebuild: every live key of the old table, with its count, into the new (empty) one; tombstones stay behind
 __global__ void __launch_bounds__(kBlock) k_map_rehash(const unsigned long long* __restrict__ old_keys,
                                                        const int* __restrict__ old_cnt, unsigned long long old_slots,
                                                        unsigned long long* keys, int* cnt, unsigned long long mask) {
   const unsigned long long j = (unsigned long long) blockIdx.x * kBlock + threadIdx.x;
   if (j >= old_slots) return;
   const unsigned long long key = old_keys[j];
-  if (key == kEmpty) return;
+  if (key == kEmpty || key == kTomb) return;
   unsigned long long s = mix64(key) & mask;
   while (atomicCAS(keys + s, kEmpty, key) != kEmpty) s = (s + 1) & mask;  // (keys are unique: the first free slot)
   cnt[s] = old_cnt[j];
+}
+
+struct RemoveArgs {
+  unsigned long long* keys;
+  unsigned long long slots;
+  double v;
+  double o[3];                    // the origin
+  double D2;                      // max_distance^2, rounded on the host
+  double* xyz;                    // the map's rows
+  long long* sr;
+  double* tmp_xyz;                // row-sized scratch of the compaction
+  long long* tmp_sr;
+  unsigned char* flag;            // per row: kept
+  int* G;                         // per row: kept rows before it in its tile
+  int* tile;                      // row tiles + 1: totals, then offsets; [n_tiles] ends as the new M
+  State* st;
+  Mirror* mirror;
+  unsigned long long seq;
+};
+
+// the voxel with key k (per axis, as a double) goes when its centre (k + 0.5) v lies farther than D from the origin:
+// ((dx dx + dy dy) + dz dz) > D^2, each operation rounded to nearest, no FMA
+__device__ __forceinline__ bool voxel_far(const RemoveArgs& a, double kx, double ky, double kz) {
+  const double dx = __dsub_rn(__dmul_rn(__dadd_rn(kx, 0.5), a.v), a.o[0]);
+  const double dy = __dsub_rn(__dmul_rn(__dadd_rn(ky, 0.5), a.v), a.o[1]);
+  const double dz = __dsub_rn(__dmul_rn(__dadd_rn(kz, 0.5), a.v), a.o[2]);
+  return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)) > a.D2;
+}
+
+// over the slots: a far voxel's key becomes a tombstone; the removed voxels are counted
+__global__ void __launch_bounds__(kBlock) k_map_evict(const __grid_constant__ RemoveArgs a) {
+  const unsigned long long s = (unsigned long long) blockIdx.x * kBlock + threadIdx.x;
+  if (s == 0) a.st->lo = ~0ull;  // (k_map_keep lowers it; nothing reads it before)
+  bool gone = false;
+  if (s < a.slots) {
+    const unsigned long long key = a.keys[s];
+    if (key != kEmpty && key != kTomb) {
+      const long long b = 1 << 20, f = (1 << 21) - 1;
+      gone = voxel_far(a, double((long long) (key & f) - b), double((long long) ((key >> 21) & f) - b),
+                       double((long long) (key >> 42) - b));
+      if (gone) a.keys[s] = kTomb;
+    }
+  }
+  const unsigned g = __ballot_sync(0xffffffffu, gone);
+  if ((threadIdx.x & 31) == 0 && g) atomicAdd(&a.st->removed, (unsigned long long) __popc(g));
+}
+
+// over the rows (blockDim.x == gtb::kTile, a grid over the host's bound of M): keep flag of every row from the key of its
+// own xyz (the posed point the insert keyed: the same key, no table lookup), flags scanned per tile, first removed row
+__global__ void __launch_bounds__(gtb::kTile) k_map_keep(const __grid_constant__ RemoveArgs a) {
+  if (a.st->removed == 0) return;
+  const int M = int(a.st->M);
+  const int n_tiles = (M + gtb::kTile - 1) / gtb::kTile;
+  if (int(blockIdx.x) >= n_tiles) return;
+  const int i = blockIdx.x * gtb::kTile + threadIdx.x;
+  if (i == 0) a.tile[n_tiles] = 0;
+  int f = 0;
+  if (i < M) {
+    const double x = a.xyz[3 * size_t(i)], y = a.xyz[3 * size_t(i) + 1], z = a.xyz[3 * size_t(i) + 2];
+    f = !voxel_far(a, floor(__ddiv_rn(x, a.v)), floor(__ddiv_rn(y, a.v)), floor(__ddiv_rn(z, a.v)));
+    a.flag[i] = (unsigned char) f;
+  }
+  gtb::scan_tile_flag(f, M, a.G, a.tile);
+  // the first removed row of the tile is the one with every row before it kept
+  if (i < M && !f && a.G[i] == int(threadIdx.x)) atomicMin(&a.st->lo, (unsigned long long) i);
+}
+
+// one CTA of 1024: tile offsets in place (tile[n_tiles] becomes the new M), the counters, the mirror
+__global__ void __launch_bounds__(1024) k_map_evict_sums(const __grid_constant__ RemoveArgs a) {
+  State* st = a.st;
+  const unsigned long long removed = st->removed;
+  const int n_tiles = int((st->M + gtb::kTile - 1) / gtb::kTile);
+  if (removed) gtb::scan_tile_sums_body(a.tile, n_tiles + 1);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    st->base = st->M;
+    if (removed) {
+      st->M = (unsigned long long) a.tile[n_tiles];
+      st->V -= removed;
+      st->T += removed;
+      st->removed = 0;
+    }
+    volatile Mirror* m = a.mirror;
+    m->M = (long long) st->M;
+    m->V = (long long) st->V;
+    m->dropped = (long long) st->dropped;
+    m->T = (long long) st->T;
+    __threadfence_system();
+    m->seq = a.seq;
+  }
+}
+
+// rows [lo, old M) that stay go to their new place in the scratch (rows before lo keep theirs)
+__global__ void __launch_bounds__(kBlock) k_map_compact(const __grid_constant__ RemoveArgs a) {
+  const unsigned long long i = (unsigned long long) blockIdx.x * kBlock + threadIdx.x;
+  if (i < a.st->lo || i >= a.st->base || !a.flag[i]) return;
+  const size_t row = size_t(a.G[i] + a.tile[i / gtb::kTile]);
+  a.tmp_xyz[3 * row] = a.xyz[3 * i];
+  a.tmp_xyz[3 * row + 1] = a.xyz[3 * i + 1];
+  a.tmp_xyz[3 * row + 2] = a.xyz[3 * i + 2];
+  a.tmp_sr[2 * row] = a.sr[2 * i];
+  a.tmp_sr[2 * row + 1] = a.sr[2 * i + 1];
+}
+
+// the scratch rows [lo, new M) back into the map's rows
+__global__ void __launch_bounds__(kBlock) k_map_copy_back(const __grid_constant__ RemoveArgs a) {
+  const unsigned long long i = (unsigned long long) blockIdx.x * kBlock + threadIdx.x;
+  if (i < a.st->lo || i >= a.st->M) return;
+  a.xyz[3 * i] = a.tmp_xyz[3 * i];
+  a.xyz[3 * i + 1] = a.tmp_xyz[3 * i + 1];
+  a.xyz[3 * i + 2] = a.tmp_xyz[3 * i + 2];
+  a.sr[2 * i] = a.tmp_sr[2 * i];
+  a.sr[2 * i + 1] = a.tmp_sr[2 * i + 1];
 }
 
 }  // namespace vmap

@@ -250,6 +250,18 @@ class VoxelMap:
     def clear(self):
         check(capi.lib().madicp_map_clear(self._h), "madicp_map_clear")
 
+    def remove_far(self, origin, max_distance):
+        """Every voxel whose centre lies farther than max_distance from origin (3 floats) goes, with its rows; later
+        points that reach it start it afresh.  Asynchronous (madicp_map_remove_far)."""
+        o = np.ascontiguousarray(np.asarray(origin, np.float64).reshape(3))
+        check(capi.lib().madicp_map_remove_far(self._h, as_d(o), float(max_distance)), "madicp_map_remove_far")
+
+    def table(self):
+        """(slots, occupied, live) of the hash table, counted from its keys (madicp_debug_map_table).  Synchronises."""
+        out = [C.c_int64(0) for _ in range(3)]
+        check(capi.lib().madicp_debug_map_table(self._h, *[C.byref(x) for x in out]), "madicp_debug_map_table")
+        return tuple(x.value for x in out)
+
 
 class Registrar:
     """One GPU's registration context (reference: class MADicp + Pipeline's keyframe deque)."""

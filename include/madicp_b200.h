@@ -239,6 +239,24 @@ int madicp_map_clear(madicp_map_t* map);
  * sized from the live voxels; the row allocations stay at their peak (nothing shrinks), and the first removal
  * allocates a row-sized scratch for the compaction.  MADICP_ERR_INVALID for a bad argument, before any device work. */
 int madicp_map_remove_far(madicp_map_t* map, const double origin[3], double max_distance);
+/* Not in the reference.  The nearest map row of each of n query points within max_distance.  The candidates are the rows
+ * of the map after every operation enqueued before the call whose scan is < scan_below (INT64_MAX: every row).  For
+ * query q, d2_j = ((x_j - qx)^2 + (y_j - qy)^2) + (z_j - qz)^2, each operation float64 round-to-nearest without FMA,
+ * and r2 = max_distance^2 rounded on the host: row[i] is the candidate with the least d2_j among those with d2_j <= r2,
+ * ties to the smallest row, and d2[i] its d2_j; row[i] = -1 and d2[i] = +inf when there is none (always for a query
+ * with a non-finite coordinate).  The answer depends only on the rows and the query.  Either output may be NULL, not
+ * both.  max_distance: finite, >= 0 and <= 4 voxel sizes (0: exact coincidences only).  The first query after the map
+ * changed (an insert, a removal, a clear, a growth or a table rebuild) builds a row index on the device, kept with the
+ * map until the next change; a map that is never queried allocates none.  Host memory: queries n x 3 doubles, row n,
+ * d2 n.  Synchronises.  Returns n; MADICP_ERR_INVALID for a bad argument, before any device work. */
+int64_t madicp_map_nearest(madicp_map_t* map, const double* queries, int64_t n, double max_distance, int64_t scan_below,
+                           int64_t* row, double* d2);
+/* Not in the reference.  The same in device memory of the map's device, read and written in place: query i is x, y, z
+ * at queries + i * q_stride bytes, float32 (q_is_f32 != 0, widened exactly) or float64; row and d2 8-byte aligned.
+ * Ordered like madicp_search_cloud_dev: the context's stream waits for consumer_stream, the answers are ready on
+ * consumer_stream with no host sync (except when the index outgrows its allocation). */
+int64_t madicp_map_nearest_dev(madicp_map_t* map, const void* queries, int64_t n, int64_t q_stride, int q_is_f32,
+                               double max_distance, int64_t scan_below, int64_t* row, double* d2, void* consumer_stream);
 /* Audit dump of a DEVICE-BUILT tree in breadth-first order: mean n x 3, eigenvectors n x 9 (column-major), bbox
  * n x 3, num_points n (any may be NULL).  Valid for the most recently built tree of the context.  Synchronises. */
 int madtree_gpu_export(const madtree_gpu_t* t, double* mean, double* eigenvectors, double* bbox, int32_t* num_points);

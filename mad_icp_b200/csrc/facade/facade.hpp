@@ -263,6 +263,20 @@ class VoxelMap {
   void removeFar(const double origin[3], double max_distance) {
     check(madicp_map_remove_far(m_, origin, max_distance), "madicp_map_remove_far");
   }
+  // the nearest row within max_distance of each of n host queries (n x 3): row (-1: none) and its squared distance
+  // (+inf: none), among the rows whose scan is < scan_below (INT64_MAX: all)
+  void nearest(const double* queries, int64_t n, double max_distance, int64_t scan_below, int64_t* row, double* d2) {
+    check(int(std::min<int64_t>(0, madicp_map_nearest(m_, queries, n, max_distance, scan_below, row, d2))),
+          "madicp_map_nearest");
+  }
+  // the same in device memory of the context's device (queries row-strided, float32 or float64), ready on
+  // consumer_stream with no host sync
+  void nearestDev(const void* queries, int64_t n, int64_t stride, bool is_f32, double max_distance, int64_t scan_below,
+                  int64_t* row, double* d2, void* consumer_stream) {
+    check(int(std::min<int64_t>(0, madicp_map_nearest_dev(m_, queries, n, stride, is_f32 ? 1 : 0, max_distance,
+                                                           scan_below, row, d2, consumer_stream))),
+          "madicp_map_nearest_dev");
+  }
 
  private:
   madicp_map_t* m_ = nullptr;

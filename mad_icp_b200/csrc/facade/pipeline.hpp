@@ -331,6 +331,16 @@ class Pipeline {
     requireMap().pointsDev(xyz, scan_record, consumer_stream);
   }
   void clearMap() { requireMap().clear(); }
+  // The nearest map row within max_distance (<= 4 map voxel sizes) of each query point, among the rows whose scan is
+  // < scan_below (INT64_MAX: all): VoxelMap::nearest / nearestDev.  The current scan is in the map once compute returns:
+  // scan_below = its scan number asks for the map as it stood before it (less what its window removed).
+  void mapNearest(const double* queries, int64_t n, double max_distance, int64_t scan_below, int64_t* row, double* d2) {
+    requireMap().nearest(queries, n, max_distance, scan_below, row, d2);
+  }
+  void mapNearestDev(const void* queries, int64_t n, int64_t stride, bool is_f32, double max_distance, int64_t scan_below,
+                     int64_t* row, double* d2, void* consumer_stream) {
+    requireMap().nearestDev(queries, n, stride, is_f32, max_distance, scan_below, row, d2, consumer_stream);
+  }
 
   // test hook: the deskew step alone (poses 4x4 row-major)
   static ContainerType deskewOnly(ContainerType cloud, const Matrix4d& T_prev, const Matrix4d& T_now, double sensor_hz,

@@ -196,6 +196,29 @@ PYBIND11_MODULE(pypeline, m) {
            py::arg("device") = false)
       .def("mapDropped", &mb::Pipeline::mapDropped)
       .def("clearMap", &mb::Pipeline::clearMap)
+      // the nearest map row within max_distance (<= 4 map voxel sizes) of each point (N x 3), among the rows whose scan
+      // is < scan_below (None: every row): (row (N,) int64, -1 for none; d2 (N,) float64, +inf for none), as numpy
+      // arrays, or for device points (a CUDA tensor, a CuPy array, read in place) as torch tensors on the pipeline's
+      // device, ready on torch's current stream (records.map_nearest_dev)
+      .def("mapNearest", [](py::object self, const py::object& points, double max_distance, const py::object& scan_below)
+               -> py::object {
+             const int64_t below = scan_below.is_none() ? std::numeric_limits<int64_t>::max() : scan_below.cast<int64_t>();
+             if (on_device(points))
+               return py::module_::import("mad_icp_b200.records").attr("map_nearest_dev")(
+                   self.attr("_mapNearestDev"), self.attr("_device")(), points, max_distance, below);
+             mb::Pipeline& p = self.cast<mb::Pipeline&>();
+             const mb::ContainerType q = cloud_arg(points);
+             py::array_t<int64_t> row(q.size());
+             py::array_t<double> d2(q.size());
+             p.mapNearest(q.empty() ? nullptr : q[0].data(), int64_t(q.size()), max_distance, below, row.mutable_data(),
+                          d2.mutable_data());
+             return py::make_tuple(row, d2);
+           }, py::arg("points"), py::arg("max_distance"), py::arg("scan_below") = py::none())
+      .def("_mapNearestDev", [](mb::Pipeline& p, uintptr_t q, int64_t n, int64_t stride, bool is_f32, double max_distance,
+                                int64_t scan_below, uintptr_t row, uintptr_t d2, uintptr_t stream) {
+        p.mapNearestDev(reinterpret_cast<const void*>(q), n, stride, is_f32, max_distance, scan_below,
+                        reinterpret_cast<int64_t*>(row), reinterpret_cast<double*>(d2), reinterpret_cast<void*>(stream));
+      })
       .def("_mapDev", [](mb::Pipeline& p, uintptr_t xyz, uintptr_t sr, uintptr_t stream) {
         p.mapPointsDev(reinterpret_cast<double*>(xyz), reinterpret_cast<int64_t*>(sr), reinterpret_cast<void*>(stream));
       })

@@ -41,6 +41,14 @@ struct madicp_map {
   DevPtr<long long> tmp_sr;
   DevPtr<int> row_G, row_tile;
   DevPtr<unsigned char> row_flag;
+  // the row index of the queries (allocated by the first query, rebuilt by the first query after any change)
+  bool index_fresh = false;  // the index matches the rows and the table: no insert, removal, clear, growth or rebuild since
+  size_t cap_index_slots = 0, cap_index_rows = 0;
+  DevPtr<int> index_G, index_tile, index_fill, index_list;
+  // host queries and their answers (madicp_map_nearest), grown as needed
+  size_t cap_host_q = 0;
+  DevPtr<double> host_q, host_d2;
+  DevPtr<long long> host_row;
   DevPtr<vmap::State> st;
   HostPtr<vmap::Mirror> mirror;  // mapped
   vmap::Mirror* d_mirror = nullptr;
@@ -123,6 +131,7 @@ int reserve(madicp_map* m, int64_t points) {
   if (fits()) return MADICP_OK;
   cudaStream_t s = m->ctx->stream;
   if (int rc = settle(m)) return rc;  // (the stream is idle from here on: buffers can be replaced)
+  m->index_fresh = false;  // (a growth moves the rows; a rebuild moves every voxel's slot)
   const size_t need_M = size_t(m->known_M + points), need_V = size_t(m->known_V + points);
   if (need_M > m->cap_points) {
     size_t cap = m->cap_points ? m->cap_points : size_t(points);
@@ -172,6 +181,102 @@ int reserve(madicp_map* m, int64_t points) {
     CK(cudaMalloc(m->tile.put(), tiles * sizeof(int)));
     m->cap_scratch = cap;
   }
+  return MADICP_OK;
+}
+
+// The checks every query takes before any device work that do not read the map ...
+int query_check(const char* fn, madicp_map* m, int64_t n, const void* queries, const void* row, const void* d2,
+                double max_distance) {
+  if (!m) return map_error(fn, "null map");
+  if (n < 0) return map_error(fn, "n must be >= 0 (got " + std::to_string(n) + ")");
+  if (!row && !d2) return map_error(fn, "no output");
+  if (n > 0 && !queries) return map_error(fn, "null queries");
+  if (!std::isfinite(max_distance) || !(max_distance >= 0.0))
+    return map_error(fn, "max_distance must be finite and >= 0 (got " + std::to_string(max_distance) + ")");
+  return MADICP_OK;
+}
+// ... and the one that reads the map's voxel size: the cells a query visits are sized for max_distance <= 4 v
+int query_check_radius(const char* fn, const madicp_map* m, double max_distance) {
+  if (max_distance > 4.0 * m->v)
+    return map_error(fn, "max_distance must be <= 4 voxel sizes (" + std::to_string(4.0 * m->v) + ", got " +
+                         std::to_string(max_distance) + ")");
+  return MADICP_OK;
+}
+
+// The row index (voxel_map_kernels.cuh, k_mapq_*), on the context's stream, unless it matches the map already: the live
+// count of every slot scanned into offsets, then every row's id into its voxel's list.  3 launches, no host sync: the
+// row grid is sized from the host's bound on M, the kernels read the device's.
+int build_index(madicp_map* m, const char* fn) {
+  if (m->index_fresh || !m->slots) return MADICP_OK;
+  cudaStream_t s = m->ctx->stream;
+  refresh(m);
+  const size_t rows = std::min(m->cap_points, size_t(m->known_M + m->points_in - m->known_in));  // >= the device's M
+  if (rows > size_t(INT32_MAX) || m->slots > size_t(INT32_MAX - gtb::kTile))
+    return map_error(fn, "the map is too large for the row index");
+  if (m->cap_index_slots < m->slots || m->cap_index_rows < m->cap_points) {  // (earlier queries may still read them)
+    CK(cudaStreamSynchronize(s));
+    const size_t slots = std::max(m->cap_index_slots, m->slots), cap = std::max(m->cap_index_rows, m->cap_points);
+    CK(cudaMalloc(m->index_G.put(), slots * sizeof(int)));
+    CK(cudaMalloc(m->index_fill.put(), slots * sizeof(int)));
+    CK(cudaMalloc(m->index_tile.put(), ((slots + gtb::kTile - 1) / gtb::kTile) * sizeof(int)));
+    CK(cudaMalloc(m->index_list.put(), std::max<size_t>(cap, 1) * sizeof(int)));
+    m->cap_index_slots = slots;
+    m->cap_index_rows = cap;
+  }
+  vmap::IndexArgs a{};
+  a.keys = m->keys;
+  a.cnt = m->cnt;
+  a.slots = int(m->slots);
+  a.mask = m->slots - 1;
+  a.v = m->v;
+  a.xyz = m->xyz;
+  a.st = m->st;
+  a.G = m->index_G;
+  a.tile = m->index_tile;
+  a.fill = m->index_fill;
+  a.list = m->index_list;
+  const unsigned tiles = unsigned((m->slots + gtb::kTile - 1) / gtb::kTile);
+  const unsigned row_blocks = unsigned(std::max<size_t>(1, (rows + vmap::kBlock - 1) / vmap::kBlock));
+  vmap::k_mapq_offsets<<<tiles, gtb::kTile, 0, s>>>(a);
+  vmap::k_mapq_sums<<<1, 1024, 0, s>>>(a);
+  vmap::k_mapq_rows<<<row_blocks, vmap::kBlock, 0, s>>>(a);
+  m->ctx->launches += 3;
+  CK(cudaGetLastError());
+  m->index_fresh = true;
+  return MADICP_OK;
+}
+
+// The query kernel over n >= 1 queries in device memory, on the context's stream, after the index it reads
+int run_query(madicp_map* m, const char* fn, const void* queries, int64_t n, int64_t q_stride, int q_is_f32,
+              double max_distance, int64_t scan_below, int64_t* row, double* d2) {
+  if (int rc = build_index(m, fn)) return rc;
+  vmap::QueryArgs a{};
+  a.q = static_cast<const char*>(queries);
+  a.n = n;
+  a.stride = q_stride;
+  a.is_f32 = q_is_f32 ? 1 : 0;
+  a.r = max_distance;
+  a.v = m->v;
+  a.r2 = max_distance * max_distance;
+  const double rc = (max_distance / m->v) * (1.0 + 0x1p-20) + 0x1p-20;  // (the cell pruning bound: k_mapq_nearest)
+  a.rc2 = rc * rc;
+  a.scan_below = scan_below;
+  a.filter = scan_below != INT64_MAX;
+  if (m->slots) {
+    a.keys = m->keys;
+    a.cnt = m->cnt;
+    a.mask = m->slots - 1;
+    a.G = m->index_G;
+    a.tile = m->index_tile;
+    a.list = m->index_list;
+    a.xyz = m->xyz;
+    a.sr = m->sr;
+  }
+  a.row = reinterpret_cast<long long*>(row);
+  a.d2 = d2;
+  vmap::k_mapq_nearest<<<unsigned((n + vmap::kBlock - 1) / vmap::kBlock), vmap::kBlock, 0, m->ctx->stream>>>(a);
+  m->ctx->launches++;
+  CK(cudaGetLastError());
   return MADICP_OK;
 }
 
@@ -270,6 +375,7 @@ int madicp_map_insert(madicp_map_t* m, const madtree_gpu_t* t, const double X[12
   m->rounds += uint32_t(m->K);
   m->ops++;
   m->points_in += n;
+  m->index_fresh = false;
   return MADICP_OK;
   MADICP_CATCH(fn)
 }
@@ -330,6 +436,7 @@ int madicp_map_clear(madicp_map_t* m) {
   }
   CK(cudaMemsetAsync(m->st.get(), 0, sizeof(vmap::State), s));
   m->rounds = 0;
+  m->index_fresh = false;  // (a clear does not advance ops)
   vmap::Mirror* h = m->mirror.get();
   h->M = h->V = h->dropped = h->T = 0;
   h->seq = m->ops;
@@ -393,7 +500,62 @@ int madicp_map_remove_far(madicp_map_t* m, const double origin[3], double max_di
   c->launches += 5;
   CK(cudaGetLastError());
   m->ops++;
+  m->index_fresh = false;
   return MADICP_OK;
+  MADICP_CATCH(fn)
+}
+
+int64_t madicp_map_nearest(madicp_map_t* m, const double* queries, int64_t n, double max_distance, int64_t scan_below,
+                           int64_t* row, double* d2) {
+  const char* fn = "madicp_map_nearest";
+  if (int rc = query_check(fn, m, n, queries, row, d2, max_distance)) return rc;
+  if (int rc = query_check_radius(fn, m, max_distance)) return rc;
+  if (n == 0) return 0;
+  madicp_ctx* c = m->ctx;
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  if (size_t(n) > m->cap_host_q) {  // (an earlier query may still read the old buffers)
+    CK(cudaStreamSynchronize(s));
+    m->cap_host_q = 0;
+    CK(cudaMalloc(m->host_q.put(), size_t(n) * 3 * sizeof(double)));
+    CK(cudaMalloc(m->host_d2.put(), size_t(n) * sizeof(double)));
+    CK(cudaMalloc(m->host_row.put(), size_t(n) * sizeof(long long)));
+    m->cap_host_q = size_t(n);
+  }
+  CK(cudaMemcpyAsync(m->host_q.get(), queries, size_t(n) * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
+  if (int rc = run_query(m, fn, m->host_q.get(), n, 3 * sizeof(double), 0, max_distance, scan_below,
+                         row ? reinterpret_cast<int64_t*>(m->host_row.get()) : nullptr, d2 ? m->host_d2.get() : nullptr))
+    return rc;
+  if (row) CK(cudaMemcpyAsync(row, m->host_row.get(), size_t(n) * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+  if (d2) CK(cudaMemcpyAsync(d2, m->host_d2.get(), size_t(n) * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return n;
+  MADICP_CATCH(fn)
+}
+
+int64_t madicp_map_nearest_dev(madicp_map_t* m, const void* queries, int64_t n, int64_t q_stride, int q_is_f32,
+                               double max_distance, int64_t scan_below, int64_t* row, double* d2, void* consumer_stream) {
+  const char* fn = "madicp_map_nearest_dev";
+  if (int rc = query_check(fn, m, n, queries, row, d2, max_distance)) return rc;
+  const int64_t e = q_is_f32 ? 4 : 8;
+  if (n > 0 && (q_stride < 3 * e || q_stride % e))
+    return map_error(fn, "the row stride must hold x, y, z and be a multiple of the field size (got " +
+                         std::to_string(q_stride) + ")");
+  if (int rc = query_check_radius(fn, m, max_distance)) return rc;
+  if (n == 0) return 0;
+  madicp_ctx* c = m->ctx;
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  if (int rc = madicp_check_device_ptr(c, queries, int(e), "madicp_map_nearest_dev (queries)")) return rc;
+  if (row)
+    if (int rc = madicp_check_device_ptr(c, row, 8, "madicp_map_nearest_dev (rows)")) return rc;
+  if (d2)
+    if (int rc = madicp_check_device_ptr(c, d2, 8, "madicp_map_nearest_dev (d2)")) return rc;
+  if (int rc = madicp_stream_wait(c, c->stream, consumer_stream)) return rc;  // queries written, outputs allocated there
+  if (int rc = run_query(m, fn, queries, n, q_stride, q_is_f32, max_distance, scan_below, row, d2)) return rc;
+  if (int rc = madicp_stream_wait(c, consumer_stream, c->stream)) return rc;
+  return n;
   MADICP_CATCH(fn)
 }
 

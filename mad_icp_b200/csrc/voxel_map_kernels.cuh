@@ -22,6 +22,15 @@
 //   k_map_copy_back      the scratch rows from the first removed row on go back to the map's rows.
 // The row kernels return at once when k_map_evict removed nothing.  Tombstones keep their slots (a claim passes over
 // them like any foreign key) until the host rebuilds the table (k_map_rehash skips them).
+//
+// A nearest-row query (madicp_map_nearest*) reads a row index of the map in CSR form, voxel -> its rows, built by the
+// first query after the map changed, in 3 launches:
+//   k_mapq_offsets  over the slots: the live count of every slot (cnt[s] under a live key, 0 under an empty slot or a
+//                   tombstone, whose cnt is stale) scanned per tile; the fill counters zeroed;
+//   k_mapq_sums     one CTA: the tile offsets in place;
+//   k_mapq_rows     over the rows: every row finds its slot from the key of its own xyz and writes its id at the slot's
+//                   offset + a fill ticket (the order within a voxel is the atomics' order; nothing depends on it).
+// and then answers every query in one launch, k_mapq_nearest (one thread per query).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -327,6 +336,141 @@ __global__ void __launch_bounds__(kBlock) k_map_copy_back(const __grid_constant_
   a.xyz[3 * i + 2] = a.tmp_xyz[3 * i + 2];
   a.sr[2 * i] = a.tmp_sr[2 * i];
   a.sr[2 * i + 1] = a.tmp_sr[2 * i + 1];
+}
+
+struct IndexArgs {
+  const unsigned long long* keys;
+  const int* cnt;
+  int slots;
+  unsigned long long mask;  // slots - 1
+  double v;
+  const double* xyz;        // the map's rows
+  const State* st;          // st->M: the rows to index
+  int* G;                   // per slot: live rows of the slots before it in its tile
+  int* tile;                // per slot tile: its total, then its offset
+  int* fill;                // per slot: rows written so far
+  int* list;                // M row ids, voxel after voxel
+};
+
+// the slot of a key the table holds (linear probing from mix64, as the claim placed it)
+__device__ __forceinline__ unsigned long long find_slot(const unsigned long long* keys, unsigned long long mask,
+                                                        unsigned long long key) {
+  unsigned long long s = mix64(key) & mask;
+  while (keys[s] != key) s = (s + 1) & mask;
+  return s;
+}
+
+// over the slots (blockDim.x == gtb::kTile): live count per slot, scanned per tile; fill counters zeroed
+__global__ void __launch_bounds__(gtb::kTile) k_mapq_offsets(const __grid_constant__ IndexArgs a) {
+  const int s = blockIdx.x * gtb::kTile + threadIdx.x;
+  int c = 0;
+  if (s < a.slots) {
+    const unsigned long long key = a.keys[s];
+    if (key != kEmpty && key != kTomb) c = a.cnt[s];  // (a tombstone's cnt is stale: k_map_evict leaves it)
+    a.fill[s] = 0;
+  }
+  gtb::scan_tile_flag(c, a.slots, a.G, a.tile);
+}
+
+__global__ void __launch_bounds__(1024) k_mapq_sums(const __grid_constant__ IndexArgs a) {
+  gtb::scan_tile_sums_body(a.tile, (a.slots + gtb::kTile - 1) / gtb::kTile);
+}
+
+// over the rows (a grid over the host's bound of M; the device's M decides): row i's id into its voxel's list
+__global__ void __launch_bounds__(kBlock) k_mapq_rows(const __grid_constant__ IndexArgs a) {
+  const unsigned long long i = (unsigned long long) blockIdx.x * kBlock + threadIdx.x;
+  if (i >= a.st->M) return;
+  unsigned long long key = 0;
+  voxel_key(a.xyz[3 * i], a.xyz[3 * i + 1], a.xyz[3 * i + 2], a.v, key);  // (every row has a key in range)
+  const unsigned long long s = find_slot(a.keys, a.mask, key);
+  a.list[a.G[s] + a.tile[s / gtb::kTile] + atomicAdd(a.fill + s, 1)] = int(i);
+}
+
+struct QueryArgs {
+  const char* q;            // query i: x, y, z at q + i * stride, float64 or float32 (is_f32)
+  long long n, stride;
+  int is_f32;
+  double r2;                // max_distance^2, rounded on the host
+  double rc2;               // the cell pruning bound (k_mapq_nearest), computed on the host
+  double r, v;
+  long long scan_below;     // candidates: rows whose scan < scan_below
+  int filter;               // scan_below != INT64_MAX
+  const unsigned long long* keys;  // nullptr: a map without a table (nothing was ever inserted)
+  const int* cnt;
+  unsigned long long mask;
+  const int* G;
+  const int* tile;
+  const int* list;
+  const double* xyz;
+  const long long* sr;
+  long long* row;           // outputs (either may be null)
+  double* d2;
+};
+
+__device__ __forceinline__ double query_coord(const QueryArgs& a, long long i, int c) {
+  const char* p = a.q + i * a.stride;
+  return a.is_f32 ? double(reinterpret_cast<const float*>(p)[c]) : reinterpret_cast<const double*>(p)[c];
+}
+
+// One thread per query: the row with the least (d2, row) among the candidates with d2 <= r2, d2 as
+// ((x - qx)^2 + (y - qy)^2) + (z - qz)^2, every operation float64 round-to-nearest without FMA.
+//
+// The cells visited cover every such row.  Per axis the keys are floor(RN(RN(q - r) / v)) - 1 .. floor(RN(RN(q + r) / v))
+// + 1, clamped to the keys a row can have, (-2^20, 2^20).  A row x (key k = floor(RN(x / v)), |k| < 2^20, so |x| <
+// 2^20 v) with a computed d2 <= r2 has RN(dx dx) <= r2 on each axis (a rounded sum of non-negative terms is no smaller
+// than any of them), so |x - q| <= r (1 + 2^-50).  If |q| >= 2^21 v, |x - q| > 2^20 v > 4 v >= r (1 + 2^-50): no such
+// row exists.  Otherwise every value involved lies below 2^22 v in magnitude, so each rounding moves it by at most
+// 2^-31 v, and x >= RN(q - r) - 2^-30 v, hence RN(x / v) > RN(RN(q - r) / v) - 1 and k >= the first key; the last key
+// likewise.  Within that box a cell is skipped only when its points cannot be that close: with c = floor(RN(q / v)),
+// a point of cell k lies at least (|k - c| - 1) v - 2^-28 v from q per axis, so a cell whose g = max(0, |k - c| - 1)
+// per axis has gx^2 + gy^2 + gz^2 > rc2 = ((r / v)(1 + 2^-20) + 2^-20)^2 holds no row within r (1 + 2^-50).
+// The answer is a lexicographic minimum: it does not depend on the order cells or rows are visited in.
+__global__ void __launch_bounds__(kBlock) k_mapq_nearest(const __grid_constant__ QueryArgs a) {
+  const long long i = (long long) blockIdx.x * kBlock + threadIdx.x;
+  if (i >= a.n) return;
+  const double qx = query_coord(a, i, 0), qy = query_coord(a, i, 1), qz = query_coord(a, i, 2);
+  long long best = -1;
+  double bd = __longlong_as_double(0x7ff0000000000000ll);  // +inf
+  if (a.keys && isfinite(qx) && isfinite(qy) && isfinite(qz)) {
+    const double lim = kKeyLimit - 1.0;
+    auto first = [&](double q) { return fmax(__dsub_rn(floor(__ddiv_rn(__dsub_rn(q, a.r), a.v)), 1.0), -lim); };
+    auto last = [&](double q) { return fmin(__dadd_rn(floor(__ddiv_rn(__dadd_rn(q, a.r), a.v)), 1.0), lim); };
+    const double cx = floor(__ddiv_rn(qx, a.v)), cy = floor(__ddiv_rn(qy, a.v)), cz = floor(__ddiv_rn(qz, a.v));
+    const double hx = last(qx), hy = last(qy), hz = last(qz), ly = first(qy), lz = first(qz);
+    const long long b = 1 << 20;
+    for (double kx = first(qx); kx <= hx; kx += 1.0) {
+      const double gx = fmax(fabs(kx - cx) - 1.0, 0.0), sx = gx * gx;
+      if (sx > a.rc2) continue;
+      for (double ky = ly; ky <= hy; ky += 1.0) {
+        const double gy = fmax(fabs(ky - cy) - 1.0, 0.0), sy = sx + gy * gy;
+        if (sy > a.rc2) continue;
+        for (double kz = lz; kz <= hz; kz += 1.0) {
+          const double gz = fmax(fabs(kz - cz) - 1.0, 0.0);
+          if (sy + gz * gz > a.rc2) continue;
+          const unsigned long long key = (unsigned long long) ((long long) kx + b) |
+                                         ((unsigned long long) ((long long) ky + b) << 21) |
+                                         ((unsigned long long) ((long long) kz + b) << 42);
+          unsigned long long s = mix64(key) & a.mask;
+          unsigned long long k;
+          while ((k = a.keys[s]) != key && k != kEmpty) s = (s + 1) & a.mask;  // (tombstones: passed over)
+          if (k != key) continue;
+          const int off = a.G[s] + a.tile[s / gtb::kTile], end = off + a.cnt[s];
+          for (int e = off; e < end; ++e) {
+            const long long j = a.list[e];
+            const double dx = __dsub_rn(a.xyz[3 * j], qx), dy = __dsub_rn(a.xyz[3 * j + 1], qy),
+                         dz = __dsub_rn(a.xyz[3 * j + 2], qz);
+            const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+            if (!(d2 <= a.r2) || d2 > bd || (d2 == bd && j > best)) continue;
+            if (a.filter && a.sr[2 * j] >= a.scan_below) continue;
+            best = j;
+            bd = d2;
+          }
+        }
+      }
+    }
+  }
+  if (a.row) a.row[i] = best;
+  if (a.d2) a.d2[i] = bd;
 }
 
 }  // namespace vmap

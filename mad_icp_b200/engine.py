@@ -256,6 +256,30 @@ class VoxelMap:
         o = np.ascontiguousarray(np.asarray(origin, np.float64).reshape(3))
         check(capi.lib().madicp_map_remove_far(self._h, as_d(o), float(max_distance)), "madicp_map_remove_far")
 
+    def nearest(self, queries, max_distance, scan_below=None):
+        """The nearest row within max_distance (finite, >= 0, <= 4 voxel sizes) of each query point, among the rows
+        whose scan is < scan_below (None: every row): (row (N,) int64, -1 for none; d2 (N,) float64, the squared
+        distance ((x - qx)^2 + (y - qy)^2) + (z - qz)^2 in float64 without FMA, +inf for none), ties to the smaller row.
+        Host queries (N x 3) give numpy arrays (madicp_map_nearest, synchronises); device queries (a CUDA tensor or
+        array, float32 or float64, read in place) give torch tensors on the registrar's device, ready on torch's current
+        stream (madicp_map_nearest_dev)."""
+        below = np.iinfo(np.int64).max if scan_below is None else int(scan_below)
+        if hasattr(queries, "__cuda_array_interface__"):
+            from .records import map_nearest_dev
+
+            def run(q, n, stride, is_f32, r, sb, row, d2, stream):
+                check(capi.lib().madicp_map_nearest_dev(self._h, C.c_void_p(q), n, stride, int(is_f32), r, sb,
+                                                        C.c_void_p(row), C.c_void_p(d2), C.c_void_p(stream)),
+                      "madicp_map_nearest_dev")
+            return map_nearest_dev(run, self._reg.device, queries, max_distance, below)
+        q = np.ascontiguousarray(np.asarray(queries, np.float64))
+        if q.ndim != 2 or q.shape[1] != 3:
+            raise ValueError("queries: an (N, 3) array")
+        row, d2 = np.empty(q.shape[0], np.int64), np.empty(q.shape[0])
+        check(capi.lib().madicp_map_nearest(self._h, as_d(q), q.shape[0], float(max_distance), below,
+                                            row.ctypes.data_as(C.POINTER(C.c_int64)), as_d(d2)), "madicp_map_nearest")
+        return row, d2
+
     def table(self):
         """(slots, occupied, live) of the hash table, counted from its keys (madicp_debug_map_table).  Synchronises."""
         out = [C.c_int64(0) for _ in range(3)]

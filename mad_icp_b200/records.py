@@ -283,6 +283,25 @@ def search_cloud_arrays_dev(search_dev, queries):
     return P, N, D
 
 
+def map_nearest_dev(nearest_dev, device, queries, max_distance, scan_below):
+    """VoxelMap.nearest / Pipeline.mapNearest of device queries (2-D float32 / float64 with x, y, z in adjacent columns,
+    any row stride describe() accepts): (row (N,) int64, d2 (N,) float64) as torch tensors on the map's CUDA device,
+    written by the query kernel in place and ready on torch's current stream there (no host sync).
+    nearest_dev(q, n, stride, is_f32, max_distance, scan_below, row, d2, stream) runs madicp_map_nearest_dev."""
+    import torch
+    d = describe(queries)
+    e = 4 if d.is_f32 else 8
+    if list(d.offset) != [0, e, 2 * e]:
+        raise ValueError("queries: x, y, z must be adjacent columns -- pass a contiguous copy")
+    dev = torch.device("cuda", device)
+    n = int(d.n)
+    row = torch.empty(n, dtype=torch.int64, device=dev)
+    d2 = torch.empty(n, dtype=torch.float64, device=dev)
+    nearest_dev(int(d.data or 0), n, int(d.stride), bool(d.is_f32), float(max_distance), int(scan_below), row.data_ptr(),
+                d2.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+    return row, d2
+
+
 def leaves_array_dev(pipeline, model):
     """Pipeline.currentLeavesArray / modelLeavesArray(device=True): the leaf means as an (N, 3) float64 torch tensor on the
     pipeline's device, written by the gather kernel in place and ready on torch's current stream (no host sync).  With

@@ -87,6 +87,11 @@ int madicp_debug_chunk_poses(const double T_prev[12], const double T_now[12], do
 /* The voxel map's hash table (madicp_map_*): its slots, the occupied ones (live voxels and the tombstones of removed
  * ones) and the live ones, counted from the table's keys (any output may be NULL).  Synchronises. */
 int madicp_debug_map_table(madicp_map_t* map, int64_t* slots, int64_t* occupied, int64_t* live);
+/* The voxel map's count of acceptance rounds (madicp_map_insert tags its round words with 0xFFFFFFFF - round, and starts
+ * fresh round words once fewer than K tags are left): returns the count, then sets it to `rounds` unless rounds < 0.
+ * The count may only move forward, up to 0xFFFFFF00, so tests can reach the tag reset without 2^32 / K inserts.  Host
+ * state only: no device work, no synchronisation. */
+int64_t madicp_debug_map_set_rounds(madicp_map_t* map, int64_t rounds);
 
 #ifdef __cplusplus
 }

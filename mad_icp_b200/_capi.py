@@ -128,6 +128,7 @@ SYMBOLS = {
     "madicp_map_nearest": (C.c_int64, [vp, dp, C.c_int64, C.c_double, C.c_int64, C.POINTER(C.c_int64), dp]),
     "madicp_map_nearest_dev": (C.c_int64, [vp, vp, C.c_int64, C.c_int64, C.c_int, C.c_double, C.c_int64, vp, vp, vp]),
     "madicp_debug_map_table": (C.c_int, [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "madicp_debug_map_set_rounds": (C.c_int64, [vp, C.c_int64]),
     "madicp_debug_deskew_plan": (C.c_int, [pts_p, vc_p, dp, dp, C.c_double, C.c_int, C.c_int, ip,
                                            C.POINTER(C.c_uint16), dp, C.POINTER(C.c_int), C.POINTER(C.c_int64)]),
     "madicp_register_fetch_weight": (C.c_int, [vp, dp, dp, dp, bp, C.POINTER(C.c_int), dp]),

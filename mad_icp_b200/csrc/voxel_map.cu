@@ -580,4 +580,16 @@ int madicp_debug_map_table(madicp_map_t* m, int64_t* slots, int64_t* occupied, i
   MADICP_CATCH(fn)
 }
 
+int64_t madicp_debug_map_set_rounds(madicp_map_t* m, int64_t rounds) {
+  const char* fn = "madicp_debug_map_set_rounds";
+  if (!m) return map_error(fn, "null map");
+  const int64_t was = int64_t(m->rounds);
+  if (rounds < 0) return was;
+  // (forward only: the round words left behind carry the tags of smaller counts, which must stay above every later tag)
+  if (rounds < was || rounds > int64_t(0xFFFFFF00u))
+    return map_error(fn, "rounds must lie in [" + std::to_string(was) + ", 0xFFFFFF00] (got " + std::to_string(rounds) + ")");
+  m->rounds = uint32_t(rounds);
+  return was;
+}
+
 }  // extern "C"

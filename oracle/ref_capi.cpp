@@ -53,6 +53,16 @@ struct PipelineProbe : Pipeline {
   const Vector6d& velocity() const { return current_velocity_; }
   const Eigen::Isometry3d& pose() const { return frame_to_map_; }
   void deskewCloud(ContainerType* c, const Eigen::Isometry3d& a, const Eigen::Isometry3d& b) { deskew(c, a, b); }
+  // pipeline.cpp:197-204, over the flags the last compute left on current_leaves_ (NaN before the first registration)
+  double inliersRatio() const {
+    if (current_leaves_.empty()) return std::nan("");
+    int matched_leaves = 0;
+    for (MADtree* l : current_leaves_)
+      if (l->matched_) matched_leaves++;
+    return double(matched_leaves) / double(current_leaves_.size());
+  }
+  const std::deque<Frame*>& frames() const { return frames_; }
+  const std::deque<Frame*>& keyframes() const { return keyframes_; }
 };
 }  // namespace
 
@@ -177,7 +187,7 @@ void ref_pipeline_compute(void* p, double stamp, const double* pts, int n) {
   for (int i = 0; i < n; ++i) cloud[i] = Eigen::Vector3d(pts[3 * i], pts[3 * i + 1], pts[3 * i + 2]);
   static_cast<PipelineProbe*>(p)->compute(stamp, cloud);
 }
-// as orc_pipeline_state; out[16] (inliers ratio) is a local of Pipeline::compute and is reported as NaN
+// as orc_pipeline_state; out[16] (inliers ratio, a local of Pipeline::compute) is recounted from the leaves' flags
 void ref_pipeline_state(void* p, double* out) {
   PipelineProbe* P = static_cast<PipelineProbe*>(p);
   iso_to_rowmajor12(P->pose(), out);
@@ -185,8 +195,40 @@ void ref_pipeline_state(void* p, double* out) {
   out[13] = double(P->currentID());
   out[14] = double(P->keyframeID());
   out[15] = double(P->numKeyframes());
-  out[16] = std::nan("");
+  out[16] = P->inliersRatio();
   for (int i = 0; i < 6; ++i) out[17 + i] = P->velocity()(i);
+}
+// The frames window (frames_, oldest first): each frame's frame_ id and weight_ (either nullable); returns its size.
+int ref_pipeline_frames(void* p, int* ids, double* weights) {
+  const std::deque<Frame*>& f = static_cast<PipelineProbe*>(p)->frames();
+  for (size_t i = 0; i < f.size(); ++i) {
+    if (ids) ids[i] = f[i]->frame_;
+    if (weights) weights[i] = f[i]->weight_;
+  }
+  return int(f.size());
+}
+// keyframes_ in their order: each keyframe's frame_ id (nullable); returns their number
+int ref_pipeline_keyframes(void* p, int* ids) {
+  const std::deque<Frame*>& f = static_cast<PipelineProbe*>(p)->keyframes();
+  if (ids)
+    for (size_t i = 0; i < f.size(); ++i) ids[i] = f[i]->frame_;
+  return int(f.size());
+}
+// currentLeaves() (model == 0) or modelLeaves() as N x 3 doubles (out nullable); returns N
+int ref_pipeline_leaves(void* p, int model, double* out) {
+  PipelineProbe* P = static_cast<PipelineProbe*>(p);
+  const ContainerType l = model ? P->modelLeaves() : P->currentLeaves();
+  if (out)
+    for (size_t i = 0; i < l.size(); ++i)
+      for (int j = 0; j < 3; ++j) out[3 * i + j] = l[i](j);
+  return int(l.size());
+}
+// trajectory(): every pose as 3 x 4 row-major (out nullable); returns their number
+int ref_pipeline_trajectory(void* p, double* out) {
+  const std::vector<Eigen::Isometry3d>& t = static_cast<PipelineProbe*>(p)->trajectory();
+  if (out)
+    for (size_t i = 0; i < t.size(); ++i) iso_to_rowmajor12(t[i], out + 12 * i);
+  return int(t.size());
 }
 void ref_pipeline_deskew(void* p, double* pts, int n, const double* Tprev12, const double* Tnow12) {
   ContainerType c(n);

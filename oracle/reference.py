@@ -67,6 +67,35 @@ def lib():
     return _lib
 
 
+# The Pipeline probe's list entry points (oracle/ref_capi.cpp).  They are resolved on first use rather than in lib(): a
+# library built before they existed, where the reference sources are not at hand to rebuild it, still serves every
+# other caller, and has_probe() tells the callers that need them.
+PROBE = {"ref_pipeline_frames": [C.c_void_p, _ip, _dp], "ref_pipeline_keyframes": [C.c_void_p, _ip],
+         "ref_pipeline_leaves": [C.c_void_p, C.c_int, _dp], "ref_pipeline_trajectory": [C.c_void_p, _dp]}
+
+
+def has_probe():
+    """Whether the library exports the Pipeline probe's list entry points (frames, keyframes, leaves, trajectory) and
+    reports the inlier ratio in state()[16]."""
+    return all(hasattr(lib(), name) for name in PROBE)
+
+
+def exports_probe(path):
+    """has_probe() of the library file at `path`, without loading it (build() rebuilds a library that predates them)."""
+    with open(path, "rb") as f:
+        data = f.read()
+    return all(name.encode() + b"\0" in data for name in PROBE)
+
+
+def _probe(name):
+    fn = getattr(lib(), name, None)
+    if fn is None:
+        raise RuntimeError(f"{_SO} predates the Pipeline probe ({name}); rebuild it where the reference sources are "
+                           "(make -C oracle ref / ref_gpu)")
+    fn.restype, fn.argtypes = C.c_int, PROBE[name]
+    return fn
+
+
 class ReferenceTree:
     """The reference's MADtree (tools/mad_tree.{h,cpp}), built by its own constructor."""
 
@@ -138,7 +167,10 @@ def icp_run(keyframes, moving, X0, iters=15, min_ball=0.2, rho_ker=0.1, b_ratio=
 
 
 class ReferencePipeline:
-    """The reference's Pipeline (odometry/pipeline.{h,cpp}); state() as orc_pipeline_state."""
+    """The reference's Pipeline (odometry/pipeline.{h,cpp}); state() as orc_pipeline_state, with the inlier ratio of
+    pipeline.cpp:197-204 recounted from the current leaves' flags (NaN before the first registration, and from a
+    library that predates the probe: has_probe()).  frames(), keyframes(), current_leaves(), model_leaves() and
+    trajectory() need the probe."""
 
     def __init__(self, sensor_hz=10.0, deskew=False, b_max=0.2, rho_ker=0.1, p_th=0.8, b_min=0.1, b_ratio=0.02,
                  num_keyframes=4, num_threads=4, realtime=False):
@@ -158,6 +190,43 @@ class ReferencePipeline:
         st = np.zeros(23)
         lib().ref_pipeline_state(self._h, _d(st))
         return st
+
+    def frames(self):
+        """The frames window (frames_, oldest first): frame ids (int32) and weights det(H^-1)."""
+        n = _probe("ref_pipeline_frames")(self._h, None, None)
+        ids, w = np.empty(n, np.int32), np.empty(n)
+        _probe("ref_pipeline_frames")(self._h, _i(ids), _d(w))
+        return ids, w
+
+    def keyframes(self):
+        """keyframes_ in their order: frame ids (int32)."""
+        n = _probe("ref_pipeline_keyframes")(self._h, None)
+        ids = np.empty(n, np.int32)
+        _probe("ref_pipeline_keyframes")(self._h, _i(ids))
+        return ids
+
+    def _leaves(self, model):
+        n = _probe("ref_pipeline_leaves")(self._h, int(model), None)
+        out = np.empty((n, 3))
+        _probe("ref_pipeline_leaves")(self._h, int(model), _d(out))
+        return out
+
+    def current_leaves(self):
+        """currentLeaves(): the current scan's leaf means in the map frame, N x 3."""
+        return self._leaves(False)
+
+    def model_leaves(self):
+        """modelLeaves(): every keyframe's leaf means, keyframe after keyframe, N x 3."""
+        return self._leaves(True)
+
+    def trajectory(self):
+        """trajectory(): n x 4 x 4."""
+        n = _probe("ref_pipeline_trajectory")(self._h, None)
+        out = np.empty((n, 3, 4))
+        _probe("ref_pipeline_trajectory")(self._h, _d(out))
+        T = np.zeros((n, 4, 4))
+        T[:, :3], T[:, 3, 3] = out, 1.0
+        return T
 
     def deskew(self, pts, T_prev, T_now):
         out = np.ascontiguousarray(pts, dtype=np.float64).copy()

@@ -239,6 +239,21 @@ int madicp_map_clear(madicp_map_t* map);
  * sized from the live voxels; the row allocations stay at their peak (nothing shrinks), and the first removal
  * allocates a row-sized scratch for the compaction.  MADICP_ERR_INVALID for a bad argument, before any device work. */
 int madicp_map_remove_far(madicp_map_t* map, const double origin[3], double max_distance);
+/* Not in the reference.  Carving: removes the voxels that a scan's rays show to be empty, with all their rows.  The rays
+ * run from the origin o = X's translation (X[3], X[7], X[11]), or (0, 0, 0) for X == NULL, to the points of the tree's
+ * kept cloud posed by X exactly as madicp_map_insert poses them (NULL: untouched).  With the insert's keys a = key(o)
+ * and b = key(p) per endpoint p (an endpoint the insert would skip has no ray; an origin out of range carves nothing),
+ * d = b - a and n = max(|dx|, |dy|, |dz|), a ray visits the cells a + floor_div(2 d t + n, 2 n) per axis, t = 0 .. n
+ * (floor division: a 26-connected line from a to b through n + 1 cells), and carves the steps with
+ * double(t) < RN(reach * double(n)); so never its endpoint's own cell.  A ray with n == 0 or n > 16384 carves nothing.
+ * Every live voxel a carved step visits goes, unless it holds an endpoint of this call: a tombstone, its rows compacted
+ * away in order, forgotten as after madicp_map_remove_far (`dropped` unchanged).  The removed set is a union of
+ * idempotent marks: the same calls give the same bits, whatever the order rays run in.  reach: in (0, 1], smaller spares
+ * the last part of every ray (where grazing rays cross ground and walls).  The tree: of the map's context, built with
+ * its cloud kept (else MADICP_ERR_STATE).  Runs on the context's stream and never waits on the host; madicp_map_size
+ * counts it once enqueued.  The first carve allocates 8 bytes of mark per table slot.  MADICP_ERR_INVALID for a bad
+ * argument, before any device work. */
+int madicp_map_carve(madicp_map_t* map, const madtree_gpu_t* tree, const double X[12], double reach);
 /* Not in the reference.  The nearest map row of each of n query points within max_distance.  The candidates are the rows
  * of the map after every operation enqueued before the call whose scan is < scan_below (INT64_MAX: every row).  For
  * query q, d2_j = ((x_j - qx)^2 + (y_j - qy)^2) + (z_j - qz)^2, each operation float64 round-to-nearest without FMA,

@@ -125,6 +125,7 @@ SYMBOLS = {
     "madicp_map_points_dev": (C.c_int64, [vp, vp, vp, vp]),
     "madicp_map_clear": (C.c_int, [vp]),
     "madicp_map_remove_far": (C.c_int, [vp, dp, C.c_double]),
+    "madicp_map_carve": (C.c_int, [vp, vp, dp, C.c_double]),
     "madicp_map_nearest": (C.c_int64, [vp, dp, C.c_int64, C.c_double, C.c_int64, C.POINTER(C.c_int64), dp]),
     "madicp_map_nearest_dev": (C.c_int64, [vp, vp, C.c_int64, C.c_int64, C.c_int, C.c_double, C.c_int64, vp, vp, vp]),
     "madicp_debug_map_table": (C.c_int, [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),

@@ -263,6 +263,12 @@ class VoxelMap {
   void removeFar(const double origin[3], double max_distance) {
     check(madicp_map_remove_far(m_, origin, max_distance), "madicp_map_remove_far");
   }
+  // the voxels the rays from the tree's pose (none: the origin) to its posed kept cloud pass through in their first
+  // `reach` of steps go, with their rows, unless they hold one of its points (asynchronous)
+  void carve(const MADtree& t, double reach) {
+    if (!t.deviceHandle()) throw Error("VoxelMap.carve: the map takes device trees");
+    check(madicp_map_carve(m_, t.deviceHandle(), t.pose(), reach), "madicp_map_carve");
+  }
   // the nearest row within max_distance of each of n host queries (n x 3): row (-1: none) and its squared distance
   // (+inf: none), among the rows whose scan is < scan_below (INT64_MAX: all)
   void nearest(const double* queries, int64_t n, double max_distance, int64_t scan_below, int64_t* row, double* d2) {

@@ -238,9 +238,10 @@ class Pipeline {
 
   Pipeline(double sensor_hz, bool deskew, double b_max, double rho_ker, double p_th, double b_min, double b_ratio,
            int num_keyframes, int num_threads, bool realtime, int device = -1, bool keep_cloud = false,
-           double map_voxel_size = 0.0, int map_points_per_voxel = 1, double map_max_distance = 0.0)
+           double map_voxel_size = 0.0, int map_points_per_voxel = 1, double map_max_distance = 0.0,
+           double map_carve = 0.0)
       : sensor_hz_(sensor_hz), deskew_(deskew), b_max_(b_max), p_th_(p_th), b_min_(b_min), num_keyframes_(num_keyframes),
-        realtime_(realtime), keep_cloud_(keep_cloud), map_max_distance_(map_max_distance),
+        realtime_(realtime), keep_cloud_(keep_cloud), map_max_distance_(map_max_distance), map_carve_(map_carve),
         icp_(b_max, rho_ker, b_ratio, num_threads, resolveDevice(device), std::max(num_keyframes, 1)), vel_(sensor_hz) {
     frame_to_map_ = keyframe_to_map_ = detail::poseIdentity();
     device_ = resolveDevice(device);
@@ -253,6 +254,9 @@ class Pipeline {
       throw Error("Pipeline: map_max_distance must be finite and >= 0 (0: no window)");
     if (map_max_distance > 0.0 && !(map_voxel_size > 0.0))
       throw Error("Pipeline: map_max_distance > 0 needs a map (map_voxel_size > 0)");
+    if (!(map_carve >= 0.0 && map_carve <= 1.0)) throw Error("Pipeline: map_carve must lie in [0, 1] (0: no carving)");
+    if (map_carve > 0.0 && !(map_voxel_size > 0.0))
+      throw Error("Pipeline: map_carve > 0 needs a map (map_voxel_size > 0)");
     if (map_voxel_size > 0.0) {  // the map inserts each scan's kept cloud: every tree keeps one
       if (!gpu_build_) throw Error("Pipeline: a map (map_voxel_size > 0) needs device-built trees (MADICP_GPU_BUILD)");
       check(madicp_set_keep_cloud(icp_.context(), 1), "madicp_set_keep_cloud");
@@ -320,6 +324,9 @@ class Pipeline {
   // map_points_per_voxel points that reach it.  Rows in acceptance order with (scan, record): the scan's currentID()
   // before it was computed and the point's currentCloudIndices() value.  With map_max_distance > 0 (a window), every
   // insert is followed by the removal of the voxels whose centre lies farther than that from currentPose()'s translation.
+  // With map_carve = r > 0 (carving), every insert is followed by a carve of the scan's own rays, from currentPose()'s
+  // translation to its points, over their first r of steps: the voxels they pass through that hold none of the scan's
+  // points go, so what moved away leaves the map.
   size_t mapSize() { return requireMap().size(); }
   int64_t mapDropped() {
     int64_t dropped = 0;
@@ -457,10 +464,13 @@ class Pipeline {
     s.records = true;
     return s;
   }
-  // the scan's kept cloud into the map; with a window, then every voxel farther than map_max_distance from the sensor
-  // (currentPose()'s translation) goes
+  // the scan's kept cloud into the map; with carving, then the voxels the scan's rays show to be empty go (the scan's own
+  // rows stay: their voxels hold its points); with a window, then every voxel farther than map_max_distance from the
+  // sensor (currentPose()'s translation) goes.  The two removals commute (each takes a voxel on its own rule, and a
+  // voxel's rows all go with it); the order is fixed here: insert, carve, window.
   void insertIntoMap(const MADtree& t) {
     map_->insert(t, int64_t(seq_));
+    if (map_carve_ > 0.0) map_->carve(t, map_carve_);
     if (map_max_distance_ > 0.0) {
       const double origin[3] = {frame_to_map_.m[3], frame_to_map_.m[7], frame_to_map_.m[11]};
       map_->removeFar(origin, map_max_distance_);
@@ -721,6 +731,7 @@ class Pipeline {
   bool realtime_;
   bool keep_cloud_ = false;  // the current scan's tree keeps its cloud and record indices (currentCloud)
   double map_max_distance_ = 0.0;  // > 0: after each insert, the map drops the voxels farther than this from the sensor
+  double map_carve_ = 0.0;         // > 0: after each insert, the scan's rays carve this share of their steps
   bool gpu_build_ = true;   // MADICP_GPU_BUILD=0: host-built trees
   int device_ = 0;
   int num_threads_ = 1;

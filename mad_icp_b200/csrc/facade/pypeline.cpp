@@ -149,18 +149,20 @@ PYBIND11_MODULE(pypeline, m) {
       // (currentCloudArray / currentCloudIndices)
       // map_voxel_size > 0 (not in the reference): a voxel map of every scan builds itself on the device, keeping the
       // first map_points_per_voxel points of each voxel (mapArray / mapIndices); map_max_distance > 0 bounds it to the
-      // voxels whose centre lies within that distance of the sensor after each scan
+      // voxels whose centre lies within that distance of the sensor after each scan; map_carve = r in (0, 1] carves it
+      // along each scan's rays after its insert: the voxels the first r of a ray's steps pass through go unless they
+      // hold a point of the scan (madicp_map_carve)
       .def(py::init([](double sensor_hz, bool deskew, double b_max, double rho_ker, double p_th, double b_min, double b_ratio,
                        int num_keyframes, int num_threads, bool realtime, bool keep_cloud, double map_voxel_size,
-                       int map_points_per_voxel, double map_max_distance) {
+                       int map_points_per_voxel, double map_max_distance, double map_carve) {
              return new mb::Pipeline(sensor_hz, deskew, b_max, rho_ker, p_th, b_min, b_ratio, num_keyframes, num_threads,
                                      realtime, -1, keep_cloud, map_voxel_size, map_points_per_voxel,
-                                     map_max_distance);
+                                     map_max_distance, map_carve);
            }),
            py::arg("sensor_hz"), py::arg("deskew"), py::arg("b_max"), py::arg("rho_ker"), py::arg("p_th"), py::arg("b_min"),
            py::arg("b_ratio"), py::arg("num_keyframes"), py::arg("num_threads"), py::arg("realtime"),
            py::arg("keep_cloud") = false, py::arg("map_voxel_size") = 0.0, py::arg("map_points_per_voxel") = 1,
-           py::arg("map_max_distance") = 0.0)
+           py::arg("map_max_distance") = 0.0, py::arg("map_carve") = 0.0)
       .def("currentPose", [](const mb::Pipeline& p) { return pose_to_numpy(p.currentPose()); })
       .def("trajectory",
            [](const mb::Pipeline& p) {

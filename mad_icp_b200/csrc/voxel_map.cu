@@ -2,7 +2,8 @@
 // The kernels and the acceptance rule are in voxel_map_kernels.cuh.  An insert runs on the context's stream and never
 // waits on the host: the capacity it needs is bounded from the counters the previous operations left in mapped memory,
 // and the host synchronises only when that bound outgrows the allocations (the map then grows by doubling, or its table
-// is rebuilt without the tombstones of removed voxels).  A removal (madicp_map_remove_far) never waits on the host.
+// is rebuilt without the tombstones of removed voxels).  A removal (madicp_map_remove_far) and a carve (madicp_map_carve)
+// never wait on the host.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -27,6 +28,8 @@ struct madicp_map {
   size_t slots = 0;
   DevPtr<unsigned long long> keys, win;
   DevPtr<int> cnt;
+  // per slot: the tag of the last carve that marked it (allocated by the first carve, then with every new table)
+  DevPtr<unsigned long long> mark;
   // dense rows in acceptance order
   size_t cap_points = 0;
   DevPtr<double> xyz;
@@ -52,7 +55,7 @@ struct madicp_map {
   DevPtr<vmap::State> st;
   HostPtr<vmap::Mirror> mirror;  // mapped
   vmap::Mirror* d_mirror = nullptr;
-  uint64_t ops = 0;       // inserts and removals enqueued
+  uint64_t ops = 0;       // inserts, removals and carves enqueued
   int64_t points_in = 0;  // points handed to the inserts
   // the counters as of the last operation the host has seen complete (known_ops), and points_in at that time
   int64_t known_M = 0, known_V = 0, known_T = 0, known_dropped = 0, known_in = 0;
@@ -153,9 +156,13 @@ int reserve(madicp_map* m, int64_t points) {
     const size_t live_share = m->known_T ? 4 : 2;  // slots per live voxel after the rebuild, at least
     size_t slots = m->slots ? m->slots : pow2_at_least(2 * need_V);
     while (slots < live_share * need_V) slots <<= 1;
-    DevPtr<unsigned long long> keys, win;
+    DevPtr<unsigned long long> keys, win, mark;
     DevPtr<int> cnt;
     if (int rc = alloc_table(m, slots, &keys, &cnt, &win)) return rc;
+    if (m->mark) {  // (a map that carves: its marks start afresh with the new slots)
+      CK(cudaMalloc(mark.put(), slots * sizeof(unsigned long long)));
+      CK(cudaMemsetAsync(mark.get(), 0, slots * sizeof(unsigned long long), s));
+    }
     if (m->slots) {
       vmap::k_map_rehash<<<unsigned((m->slots + vmap::kBlock - 1) / vmap::kBlock), vmap::kBlock, 0, s>>>(
           m->keys, m->cnt, m->slots, keys, cnt, slots - 1);
@@ -167,6 +174,7 @@ int reserve(madicp_map* m, int64_t points) {
     m->keys = std::move(keys);
     m->cnt = std::move(cnt);
     m->win = std::move(win);
+    if (m->mark) m->mark = std::move(mark);
     m->slots = slots;
     m->rounds = 0;  // (fresh round words)
     m->known_T = 0;
@@ -277,6 +285,60 @@ int run_query(madicp_map* m, const char* fn, const void* queries, int64_t n, int
   vmap::k_mapq_nearest<<<unsigned((n + vmap::kBlock - 1) / vmap::kBlock), vmap::kBlock, 0, m->ctx->stream>>>(a);
   m->ctx->launches++;
   CK(cudaGetLastError());
+  return MADICP_OK;
+}
+
+// The grids of a removal: the table's slots, and the rows by tiles and by blocks over the host's bound of M
+struct RowGrids {
+  unsigned slot_blocks = 0, tiles = 0, row_blocks = 0;
+};
+
+// What every removal (window or carve) shares before its own slot and row passes: the row-sized scratch of the
+// compaction (allocated by the first removal, and again after the rows grew), the arguments, and the grids
+int removal_args(madicp_map* m, const char* fn, vmap::RemoveArgs* a, RowGrids* g) {
+  cudaStream_t s = m->ctx->stream;
+  refresh(m);
+  const size_t rows = std::min(m->cap_points, size_t(m->known_M + m->points_in - m->known_in));  // >= the device's M
+  if (rows > size_t(INT32_MAX - gtb::kTile)) return map_error(fn, "the map holds more rows than a removal can scan");
+  if (m->cap_rows < m->cap_points) {  // (after a growth of the rows: earlier removals may still read the old scratch)
+    CK(cudaStreamSynchronize(s));
+    const size_t cap = m->cap_points;
+    CK(cudaMalloc(m->tmp_xyz.put(), cap * 3 * sizeof(double)));
+    CK(cudaMalloc(m->tmp_sr.put(), cap * 2 * sizeof(long long)));
+    CK(cudaMalloc(m->row_G.put(), cap * sizeof(int)));
+    CK(cudaMalloc(m->row_flag.put(), cap));
+    CK(cudaMalloc(m->row_tile.put(), ((cap + gtb::kTile - 1) / gtb::kTile + 1) * sizeof(int)));
+    m->cap_rows = cap;
+  }
+  a->keys = m->keys;
+  a->slots = m->slots;
+  a->v = m->v;
+  a->xyz = m->xyz;
+  a->sr = m->sr;
+  a->tmp_xyz = m->tmp_xyz;
+  a->tmp_sr = m->tmp_sr;
+  a->flag = m->row_flag;
+  a->G = m->row_G;
+  a->tile = m->row_tile;
+  a->st = m->st;
+  a->mirror = m->d_mirror;
+  a->seq = m->ops + 1;
+  g->slot_blocks = unsigned((m->slots + vmap::kBlock - 1) / vmap::kBlock);
+  g->tiles = unsigned(std::max<size_t>(1, (rows + gtb::kTile - 1) / gtb::kTile));
+  g->row_blocks = unsigned(std::max<size_t>(1, (rows + vmap::kBlock - 1) / vmap::kBlock));
+  return MADICP_OK;
+}
+
+// ... and what it shares after them: the tile offsets and counters, the compaction, the operation's bookkeeping
+int finish_removal(madicp_map* m, const vmap::RemoveArgs& a, const RowGrids& g, int launched) {
+  cudaStream_t s = m->ctx->stream;
+  vmap::k_map_evict_sums<<<1, 1024, 0, s>>>(a);
+  vmap::k_map_compact<<<g.row_blocks, vmap::kBlock, 0, s>>>(a);
+  vmap::k_map_copy_back<<<g.row_blocks, vmap::kBlock, 0, s>>>(a);
+  m->ctx->launches += launched + 3;
+  CK(cudaGetLastError());
+  m->ops++;
+  m->index_fresh = false;
   return MADICP_OK;
 }
 
@@ -459,49 +521,67 @@ int madicp_map_remove_far(madicp_map_t* m, const double origin[3], double max_di
   MADICP_TRY
   CK(cudaSetDevice(c->device));
   if (!m->slots) return MADICP_OK;  // nothing was ever inserted
-  cudaStream_t s = c->stream;
-  refresh(m);
-  const size_t rows = std::min(m->cap_points, size_t(m->known_M + m->points_in - m->known_in));  // >= the device's M
-  if (rows > size_t(INT32_MAX - gtb::kTile)) return map_error(fn, "the map holds more rows than a removal can scan");
-  if (m->cap_rows < m->cap_points) {  // (after a growth of the rows: earlier removals may still read the old scratch)
-    CK(cudaStreamSynchronize(s));
-    const size_t cap = m->cap_points;
-    CK(cudaMalloc(m->tmp_xyz.put(), cap * 3 * sizeof(double)));
-    CK(cudaMalloc(m->tmp_sr.put(), cap * 2 * sizeof(long long)));
-    CK(cudaMalloc(m->row_G.put(), cap * sizeof(int)));
-    CK(cudaMalloc(m->row_flag.put(), cap));
-    CK(cudaMalloc(m->row_tile.put(), ((cap + gtb::kTile - 1) / gtb::kTile + 1) * sizeof(int)));
-    m->cap_rows = cap;
-  }
   vmap::RemoveArgs a{};
-  a.keys = m->keys;
-  a.slots = m->slots;
-  a.v = m->v;
+  RowGrids g;
+  if (int rc = removal_args(m, fn, &a, &g)) return rc;
   for (int k = 0; k < 3; ++k) a.o[k] = origin[k];
   a.D2 = max_distance * max_distance;
-  a.xyz = m->xyz;
-  a.sr = m->sr;
-  a.tmp_xyz = m->tmp_xyz;
-  a.tmp_sr = m->tmp_sr;
-  a.flag = m->row_flag;
-  a.G = m->row_G;
-  a.tile = m->row_tile;
-  a.st = m->st;
-  a.mirror = m->d_mirror;
-  a.seq = m->ops + 1;
-  const unsigned slot_blocks = unsigned((m->slots + vmap::kBlock - 1) / vmap::kBlock);
-  const unsigned tiles = unsigned(std::max<size_t>(1, (rows + gtb::kTile - 1) / gtb::kTile));
-  const unsigned row_blocks = unsigned(std::max<size_t>(1, (rows + vmap::kBlock - 1) / vmap::kBlock));
-  vmap::k_map_evict<<<slot_blocks, vmap::kBlock, 0, s>>>(a);
-  vmap::k_map_keep<<<tiles, gtb::kTile, 0, s>>>(a);
-  vmap::k_map_evict_sums<<<1, 1024, 0, s>>>(a);
-  vmap::k_map_compact<<<row_blocks, vmap::kBlock, 0, s>>>(a);
-  vmap::k_map_copy_back<<<row_blocks, vmap::kBlock, 0, s>>>(a);
-  c->launches += 5;
-  CK(cudaGetLastError());
-  m->ops++;
-  m->index_fresh = false;
-  return MADICP_OK;
+  cudaStream_t s = c->stream;
+  vmap::k_map_evict<<<g.slot_blocks, vmap::kBlock, 0, s>>>(a);
+  vmap::k_map_keep<<<g.tiles, gtb::kTile, 0, s>>>(a);
+  return finish_removal(m, a, g, 2);
+  MADICP_CATCH(fn)
+}
+
+int madicp_map_carve(madicp_map_t* m, const madtree_gpu_t* t, const double X[12], double reach) {
+  const char* fn = "madicp_map_carve";
+  if (!m || !t) return map_error(fn, "null map or tree");
+  if (!(reach > 0.0 && reach <= 1.0))
+    return map_error(fn, "reach must lie in (0, 1] (got " + std::to_string(reach) + ")");
+  if (t->ctx != m->ctx) return map_error(fn, "the tree lives on another context than the map");
+  if (!t->cloud) {
+    set_error(std::string(fn) + ": the tree kept no cloud (madicp_set_keep_cloud was off when it was built, or the cloud "
+              "was released)");
+    return MADICP_ERR_STATE;
+  }
+  const int64_t n = t->n_points;
+  madicp_ctx* c = m->ctx;
+  MADICP_TRY
+  CK(cudaSetDevice(c->device));
+  if (!m->slots || n == 0) return MADICP_OK;  // nothing was ever inserted, or no rays
+  cudaStream_t s = c->stream;
+  if (!m->mark) {  // the first carve: marks for the current table (a growth or rebuild allocates them afresh)
+    CK(cudaMalloc(m->mark.put(), m->slots * sizeof(unsigned long long)));
+    CK(cudaMemsetAsync(m->mark.get(), 0, m->slots * sizeof(unsigned long long), s));
+  }
+  vmap::RemoveArgs a{};
+  RowGrids g;
+  if (int rc = removal_args(m, fn, &a, &g)) return rc;
+  a.mark = m->mark;
+  a.mask = m->slots - 1;
+  vmap::CarveArgs r{};
+  r.xyz = t->cloud->xyz + 3 * size_t(t->cloud_off);
+  r.n = int(n);
+  r.has_pose = X ? 1 : 0;
+  if (X) {
+    std::memcpy(r.X, X, 12 * sizeof(double));
+    r.o[0] = X[3];
+    r.o[1] = X[7];
+    r.o[2] = X[11];
+  }
+  r.v = m->v;
+  r.reach = reach;
+  r.keys = m->keys;
+  r.mask = m->slots - 1;
+  r.mark = m->mark;
+  r.tag = a.seq;
+  const unsigned point_blocks = unsigned((n + vmap::kBlock - 1) / vmap::kBlock);
+  const unsigned mark_blocks = unsigned(std::min<int64_t>(vmap::kCarveBlocks, (n + vmap::kBlock - 1) / vmap::kBlock));
+  vmap::k_map_carve_mark<<<mark_blocks, vmap::kBlock, 0, s>>>(r);
+  vmap::k_map_carve_spare<<<point_blocks, vmap::kBlock, 0, s>>>(r);
+  vmap::k_map_carve_evict<<<g.slot_blocks, vmap::kBlock, 0, s>>>(a);
+  vmap::k_map_carve_keep<<<g.tiles, gtb::kTile, 0, s>>>(a);
+  return finish_removal(m, a, g, 4);
   MADICP_CATCH(fn)
 }
 

@@ -23,6 +23,17 @@
 // The row kernels return at once when k_map_evict removed nothing.  Tombstones keep their slots (a claim passes over
 // them like any foreign key) until the host rebuilds the table (k_map_rehash skips them).
 //
+// A carve (madicp_map_carve) removes the voxels a scan's rays pass through, in 7 launches: its own first four, then the
+// removal's last three, unchanged:
+//   k_map_carve_mark   one warp per ray, lanes over its steps: every live voxel a carved step finds gets the carve's tag
+//                      (its operation sequence number, so the per-slot mark words never need clearing);
+//   k_map_carve_spare  over the scan's points: the voxel of each gets mark 0, never a tag;
+//   k_map_carve_evict  over the slots: a voxel still marked with the tag becomes kTomb (k_map_evict's body);
+//   k_map_carve_keep   over the rows: a row stays iff the key of its own xyz is still live in the table (k_map_keep's
+//                      body, with a table lookup in place of the distance rule);
+//   k_map_evict_sums, k_map_compact, k_map_copy_back.
+// The removed set is a union of idempotent marks: nothing depends on the order rays run or atomics land.
+//
 // A nearest-row query (madicp_map_nearest*) reads a row index of the map in CSR form, voxel -> its rows, built by the
 // first query after the map changed, in 3 launches:
 //   k_mapq_offsets  over the slots: the live count of every slot (cnt[s] under a live key, 0 under an empty slot or a
@@ -91,26 +102,43 @@ __device__ __forceinline__ unsigned long long mix64(unsigned long long k) {  // 
   return k ^ (k >> 31);
 }
 
-// point i of the insert as the map stores it: posed with iso_apply's operand order, or untouched without a pose
-__device__ __forceinline__ void map_point(const InsertArgs& a, int i, double& x, double& y, double& z) {
-  x = a.xyz[3 * size_t(i)];
-  y = a.xyz[3 * size_t(i) + 1];
-  z = a.xyz[3 * size_t(i) + 2];
-  if (a.has_pose) {
+// point i of a kept cloud as the map stores it: posed with iso_apply's operand order, or untouched without a pose
+__device__ __forceinline__ void map_point(const double* xyz, int has_pose, const double* X, int i, double& x, double& y,
+                                          double& z) {
+  x = xyz[3 * size_t(i)];
+  y = xyz[3 * size_t(i) + 1];
+  z = xyz[3 * size_t(i) + 2];
+  if (has_pose) {
     double px, py, pz;
-    iso_apply(a.X, x, y, z, px, py, pz);
+    iso_apply(X, x, y, z, px, py, pz);
     x = px; y = py; z = pz;
   }
 }
+__device__ __forceinline__ void map_point(const InsertArgs& a, int i, double& x, double& y, double& z) {
+  map_point(a.xyz, a.has_pose, a.X, i, x, y, z);
+}
 
 // floor(c / v) per axis; false for a point with a key outside (-2^20, 2^20) or a non-finite coordinate
-__device__ __forceinline__ bool voxel_key(double x, double y, double z, double v, unsigned long long& key) {
+__device__ __forceinline__ bool voxel_cell(double x, double y, double z, double v, int& ix, int& iy, int& iz) {
   const double kx = floor(__ddiv_rn(x, v)), ky = floor(__ddiv_rn(y, v)), kz = floor(__ddiv_rn(z, v));
   if (!(kx > -kKeyLimit && kx < kKeyLimit && ky > -kKeyLimit && ky < kKeyLimit && kz > -kKeyLimit && kz < kKeyLimit))
     return false;  // (NaN compares false)
-  const long long b = 1 << 20;
-  key = (unsigned long long) ((long long) kx + b) | ((unsigned long long) ((long long) ky + b) << 21) |
-        ((unsigned long long) ((long long) kz + b) << 42);
+  ix = int(kx);
+  iy = int(ky);
+  iz = int(kz);
+  return true;
+}
+
+// the 64-bit key of a cell in range: three 21-bit fields, each key + 2^20
+__device__ __forceinline__ unsigned long long pack_key(int ix, int iy, int iz) {
+  const int b = 1 << 20;
+  return (unsigned long long) (ix + b) | ((unsigned long long) (iy + b) << 21) | ((unsigned long long) (iz + b) << 42);
+}
+
+__device__ __forceinline__ bool voxel_key(double x, double y, double z, double v, unsigned long long& key) {
+  int ix, iy, iz;
+  if (!voxel_cell(x, y, z, v, ix, iy, iz)) return false;
+  key = pack_key(ix, iy, iz);
   return true;
 }
 
@@ -241,6 +269,9 @@ struct RemoveArgs {
   State* st;
   Mirror* mirror;
   unsigned long long seq;
+  // a carve (madicp_map_carve) only: the per-slot mark words, and the table's mask for the row pass's lookups
+  const unsigned long long* mark;
+  unsigned long long mask;
 };
 
 // the voxel with key k (per axis, as a double) goes when its centre (k + 0.5) v lies farther than D from the origin:
@@ -252,17 +283,16 @@ __device__ __forceinline__ bool voxel_far(const RemoveArgs& a, double kx, double
   return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)) > a.D2;
 }
 
-// over the slots: a far voxel's key becomes a tombstone; the removed voxels are counted
-__global__ void __launch_bounds__(kBlock) k_map_evict(const __grid_constant__ RemoveArgs a) {
+// over the slots: a live voxel for which gone(slot, key) holds becomes a tombstone; the removed voxels are counted
+template <class Gone>
+__device__ __forceinline__ void evict_slots(const RemoveArgs& a, Gone gone_at) {
   const unsigned long long s = (unsigned long long) blockIdx.x * kBlock + threadIdx.x;
-  if (s == 0) a.st->lo = ~0ull;  // (k_map_keep lowers it; nothing reads it before)
+  if (s == 0) a.st->lo = ~0ull;  // (the row pass lowers it; nothing reads it before)
   bool gone = false;
   if (s < a.slots) {
     const unsigned long long key = a.keys[s];
     if (key != kEmpty && key != kTomb) {
-      const long long b = 1 << 20, f = (1 << 21) - 1;
-      gone = voxel_far(a, double((long long) (key & f) - b), double((long long) ((key >> 21) & f) - b),
-                       double((long long) (key >> 42) - b));
+      gone = gone_at(s, key);
       if (gone) a.keys[s] = kTomb;
     }
   }
@@ -270,9 +300,10 @@ __global__ void __launch_bounds__(kBlock) k_map_evict(const __grid_constant__ Re
   if ((threadIdx.x & 31) == 0 && g) atomicAdd(&a.st->removed, (unsigned long long) __popc(g));
 }
 
-// over the rows (blockDim.x == gtb::kTile, a grid over the host's bound of M): keep flag of every row from the key of its
-// own xyz (the posed point the insert keyed: the same key, no table lookup), flags scanned per tile, first removed row
-__global__ void __launch_bounds__(gtb::kTile) k_map_keep(const __grid_constant__ RemoveArgs a) {
+// over the rows (blockDim.x == gtb::kTile, a grid over the host's bound of M): keep flag of every row from its own xyz
+// (kept(x, y, z)), flags scanned per tile, first removed row
+template <class Kept>
+__device__ __forceinline__ void keep_rows(const RemoveArgs& a, Kept kept) {
   if (a.st->removed == 0) return;
   const int M = int(a.st->M);
   const int n_tiles = (M + gtb::kTile - 1) / gtb::kTile;
@@ -281,13 +312,29 @@ __global__ void __launch_bounds__(gtb::kTile) k_map_keep(const __grid_constant__
   if (i == 0) a.tile[n_tiles] = 0;
   int f = 0;
   if (i < M) {
-    const double x = a.xyz[3 * size_t(i)], y = a.xyz[3 * size_t(i) + 1], z = a.xyz[3 * size_t(i) + 2];
-    f = !voxel_far(a, floor(__ddiv_rn(x, a.v)), floor(__ddiv_rn(y, a.v)), floor(__ddiv_rn(z, a.v)));
+    f = kept(a.xyz[3 * size_t(i)], a.xyz[3 * size_t(i) + 1], a.xyz[3 * size_t(i) + 2]);
     a.flag[i] = (unsigned char) f;
   }
   gtb::scan_tile_flag(f, M, a.G, a.tile);
   // the first removed row of the tile is the one with every row before it kept
   if (i < M && !f && a.G[i] == int(threadIdx.x)) atomicMin(&a.st->lo, (unsigned long long) i);
+}
+
+// the window's slot pass: far voxels go
+__global__ void __launch_bounds__(kBlock) k_map_evict(const __grid_constant__ RemoveArgs a) {
+  evict_slots(a, [&](unsigned long long, unsigned long long key) {
+    const long long b = 1 << 20, f = (1 << 21) - 1;
+    return voxel_far(a, double((long long) (key & f) - b), double((long long) ((key >> 21) & f) - b),
+                     double((long long) (key >> 42) - b));
+  });
+}
+
+// the window's row pass: a row's voxel is far from the key of its own xyz (the posed point the insert keyed: the same
+// key, no table lookup)
+__global__ void __launch_bounds__(gtb::kTile) k_map_keep(const __grid_constant__ RemoveArgs a) {
+  keep_rows(a, [&](double x, double y, double z) {
+    return !voxel_far(a, floor(__ddiv_rn(x, a.v)), floor(__ddiv_rn(y, a.v)), floor(__ddiv_rn(z, a.v)));
+  });
 }
 
 // one CTA of 1024: tile offsets in place (tile[n_tiles] becomes the new M), the counters, the mirror
@@ -471,6 +518,112 @@ __global__ void __launch_bounds__(kBlock) k_mapq_nearest(const __grid_constant__
   }
   if (a.row) a.row[i] = best;
   if (a.d2) a.d2[i] = bd;
+}
+
+// ----------------------------------------------------------------------------------------------------------- carving
+constexpr int kMaxRay = 16384;      // a ray of more Chebyshev steps carves nothing: 2 |d| t + n < 2^30 stays in an int
+constexpr int kCarveBlocks = 1024;  // k_map_carve_mark's grid: about one wave of warps on an H100; larger clouds loop
+
+struct CarveArgs {
+  const double* xyz;  // the tree's kept cloud (n x 3), posed by X as the insert poses it
+  int n;
+  int has_pose;
+  double X[12];
+  double o[3];        // the rays' origin: X's translation, or 0
+  double v;
+  double reach;       // (0, 1]: a ray of n steps carves the steps t with t < RN(reach n)
+  const unsigned long long* keys;
+  unsigned long long mask;
+  unsigned long long* mark;  // per slot: the tag of the last carve whose rays crossed it (0: spared, or never)
+  unsigned long long tag;    // this carve's operation sequence number (>= 1)
+};
+
+// the slot holding `key`, or the empty slot that ends its probe (tombstones are passed over, as the claim does)
+__device__ __forceinline__ unsigned long long probe_slot(const unsigned long long* keys, unsigned long long mask,
+                                                         unsigned long long key, bool& found) {
+  unsigned long long s = mix64(key) & mask, k;
+  while ((k = keys[s]) != key && k != kEmpty) s = (s + 1) & mask;
+  found = k == key;
+  return s;
+}
+
+// floor(p / q) for q > 0 (C's division truncates toward zero)
+__device__ __forceinline__ int floor_div(int p, int q) {
+  const int t = p / q;
+  return (p % q != 0 && p < 0) ? t - 1 : t;
+}
+
+// One warp per ray, lanes over its steps.  A warp takes 32 rays at a time: lane j keys endpoint j, then the warp walks
+// each ray in turn from the lanes' shuffled copy of its (d, n, steps).  Step t of a ray from cell a with d = b - a and
+// n = max |d| visits a + floor_div(2 d t + n, 2 n) per axis: closed form, so the steps are independent.  A live voxel
+// it finds gets the tag (read first: near the sensor thousands of rays cross the same voxels).
+__global__ void __launch_bounds__(kBlock) k_map_carve_mark(const __grid_constant__ CarveArgs a) {
+  int ax, ay, az;
+  if (!voxel_cell(a.o[0], a.o[1], a.o[2], a.v, ax, ay, az)) return;  // (the origin's key is out of range: no carving)
+  const int lane = threadIdx.x & 31;
+  const int warps = gridDim.x * (kBlock / 32), groups = (a.n + 31) / 32;
+  for (int g = blockIdx.x * (kBlock / 32) + (threadIdx.x >> 5); g < groups; g += warps) {
+    const int i = g * 32 + lane;
+    int dx = 0, dy = 0, dz = 0, n = 0, steps = 0;
+    if (i < a.n) {
+      double x, y, z;
+      map_point(a.xyz, a.has_pose, a.X, i, x, y, z);
+      int bx, by, bz;
+      if (voxel_cell(x, y, z, a.v, bx, by, bz)) {
+        dx = bx - ax;
+        dy = by - ay;
+        dz = bz - az;
+        n = max(max(abs(dx), abs(dy)), abs(dz));
+        if (n > 0 && n <= kMaxRay) {
+          // the carved steps t < RN(reach n): t < ceil of it, which is at most n since reach <= 1
+          steps = int(ceil(__dmul_rn(a.reach, double(n))));
+        }
+      }
+    }
+    for (int j = 0; j < 32; ++j) {
+      const int sj = __shfl_sync(0xffffffffu, steps, j);
+      if (sj == 0) continue;  // (warp-uniform)
+      const int nj = __shfl_sync(0xffffffffu, n, j), two_n = 2 * nj;
+      const int ex = 2 * __shfl_sync(0xffffffffu, dx, j), ey = 2 * __shfl_sync(0xffffffffu, dy, j),
+                ez = 2 * __shfl_sync(0xffffffffu, dz, j);
+      for (int t = lane; t < sj; t += 32) {
+        const unsigned long long key = pack_key(ax + floor_div(ex * t + nj, two_n), ay + floor_div(ey * t + nj, two_n),
+                                                az + floor_div(ez * t + nj, two_n));
+        bool found;
+        const unsigned long long s = probe_slot(a.keys, a.mask, key, found);
+        if (found && a.mark[s] != a.tag) a.mark[s] = a.tag;
+      }
+    }
+  }
+}
+
+// over the call's endpoints: the voxel of an endpoint is never carved (its mark becomes 0, never a tag)
+__global__ void __launch_bounds__(kBlock) k_map_carve_spare(const __grid_constant__ CarveArgs a) {
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  if (i >= a.n) return;
+  double x, y, z;
+  map_point(a.xyz, a.has_pose, a.X, i, x, y, z);
+  unsigned long long key;
+  if (!voxel_key(x, y, z, a.v, key)) return;
+  bool found;
+  const unsigned long long s = probe_slot(a.keys, a.mask, key, found);
+  if (found) a.mark[s] = 0;
+}
+
+// the carve's slot pass: a voxel that kept this carve's tag goes
+__global__ void __launch_bounds__(kBlock) k_map_carve_evict(const __grid_constant__ RemoveArgs a) {
+  evict_slots(a, [&](unsigned long long s, unsigned long long) { return a.mark[s] == a.seq; });
+}
+
+// the carve's row pass: a row stays iff the key of its own xyz is still live in the table
+__global__ void __launch_bounds__(gtb::kTile) k_map_carve_keep(const __grid_constant__ RemoveArgs a) {
+  keep_rows(a, [&](double x, double y, double z) {
+    unsigned long long key = 0;
+    voxel_key(x, y, z, a.v, key);  // (every row has a key in range)
+    bool found;
+    probe_slot(a.keys, a.mask, key, found);
+    return int(found);
+  });
 }
 
 }  // namespace vmap

@@ -256,6 +256,13 @@ class VoxelMap:
         o = np.ascontiguousarray(np.asarray(origin, np.float64).reshape(3))
         check(capi.lib().madicp_map_remove_far(self._h, as_d(o), float(max_distance)), "madicp_map_remove_far")
 
+    def carve(self, tree, T=None, reach=1.0):
+        """Free-space carving: the rays from T's translation (None: the origin) to the points of the DeviceTree's kept
+        cloud, posed by T as `insert` poses them, remove every live voxel they pass through in their first `reach` (in
+        (0, 1]) of steps, with its rows, except the voxels that hold an endpoint.  Asynchronous (madicp_map_carve)."""
+        X = None if T is None else pose12(T)
+        check(capi.lib().madicp_map_carve(self._h, tree._h, as_d(X), float(reach)), "madicp_map_carve")
+
     def nearest(self, queries, max_distance, scan_below=None):
         """The nearest row within max_distance (finite, >= 0, <= 4 voxel sizes) of each query point, among the rows
         whose scan is < scan_below (None: every row): (row (N,) int64, -1 for none; d2 (N,) float64, the squared
